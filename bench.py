@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native generate path.
+"""bench.py — headline benchmark of the H100-native generate path.
 
 Workload (BASELINE.json configs[1], "C2"): Qwen2-VL-2B bf16, 1 synthetic image
 336x336 (144 merged image tokens), 128 text-side prompt tokens (T = 272),
@@ -15,6 +15,10 @@ Prints ONE JSON line (rank 0).  `value` = decode tokens/s with inputs resident i
 HBM (CUDA events, max over ranks); `e2e` = the same request through the public
 API `generate(model, processor, prompt, image)` with a HOST image (preprocessing,
 pinned H2D of pixel_values, per-token D2H inside the timed region).
+
+`--dump-outputs DIR` writes what the last timed request computed (its N_OUT + 1 generated token ids,
+the first sampled by the prefill, and the logprobs of its last decode step) as DIR/<name>.npy, so that two builds can be compared output for
+output: the weights, image and prompt are seeded, so the inputs are identical from run to run.
 """
 import argparse
 import json
@@ -43,7 +47,7 @@ def _peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def _tensor_peak():
@@ -53,18 +57,7 @@ def _tensor_peak():
         with open(p) as f:
             d = json.load(f)
         return float(d["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md ~1.4 PFLOP/s sustained)"
-
-
-def _ncu_traffic():
-    """dram bytes (read + write) of ONE decode-kernel launch from the committed ncu capture
-    (profiles/decode_traffic.json: written by tools/ncu_traffic.py from an `ncu --set full` run)."""
-    p = os.path.join(ROOT, "profiles", "decode_traffic.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return d.get("dram_bytes"), d.get("source", "profiles/decode_traffic.json")
-    return None, "no ncu capture committed"
+    return 989.0, "fallback (H100 SXM data sheet, 989 TFLOP/s dense bf16)"
 
 
 def _cpu_model():
@@ -246,9 +239,14 @@ def lockstep_2b(world, rank, dev, args, model, processor, ids, pvd, grid):
         torch.cuda.synchronize()
         return time.perf_counter() - t0, n
 
-    run()
-    dt, n = run()
-    assert n == rows * n_out
+    for _ in range(args.warmup):
+        run()
+    dt = 0.0
+    for _ in range(args.steps):
+        d, n = run()
+        dt += d
+        assert n == rows * n_out
+    dt /= args.steps
     step_ms = eng.last_decode_ms()
     t = torch.tensor([dt, step_ms], dtype=torch.float64, device=dev)
     if world > 1:
@@ -258,7 +256,7 @@ def lockstep_2b(world, rank, dev, args, model, processor, ids, pvd, grid):
     bytes_step = W_BYTES_2B + rows * KV_BYTES_PER_POS * (N_TEXT + 144 + n_out / 2)
     return {"workload": f"Qwen2-VL-2B, {rows} lock-step rows per GPU (the C2 request x {rows}), {n_out} tokens out each, "
                         "admission + prefill of the rows inside the timed region",
-            "rows_per_gpu": rows, "seconds": dt, "tokens_per_s": world * rows * n_out / dt,
+            "rows_per_gpu": rows, "seconds": dt, "steps": args.steps, "tokens_per_s": world * rows * n_out / dt,
             "decode_ms_per_step": step_ms,
             "roofline": {"bound": "hbm", "achieved": bytes_step / (step_ms / 1e3) / 1e9 if step_ms > 0 else None,
                          "peak": peak, "unit": "GB/s", "peak_source": peak_src,
@@ -319,9 +317,14 @@ def c5_leg(world, rank, dev, args):
         torch.cuda.synchronize()
         return time.perf_counter() - t0, toks
 
-    run()                      # warm-up (GEMM configurations are measured on first use, graphs captured)
-    dt, toks = run()
-    assert all(len(toks[i]) == n_out for i in shard_requests(n_req, world, rank))
+    for _ in range(args.warmup):  # GEMM configurations are measured on first use, graphs captured
+        run()
+    dt = 0.0
+    for _ in range(args.steps):
+        d, toks = run()
+        dt += d
+        assert all(len(toks[i]) == n_out for i in shard_requests(n_req, world, rank))
+    dt /= args.steps
     # device time of one lock-step step, from a dedicated slice of 64 steps on the warm engine
     step_ms = eng.last_decode_ms()
     t = torch.tensor([dt, step_ms], dtype=torch.float64, device=dev)
@@ -334,7 +337,7 @@ def c5_leg(world, rank, dev, args):
     out = {"workload": f"C5: Qwen2-VL-7B bf16, {n_req} concurrent requests ({rows} per GPU) over {world} GPU(s), "
                        f"1x336x336 image + 128 text tokens in, {n_out} out each, continuous batching "
                        "(lock-step rows, one weight stream per step), router: request i -> rank i mod N",
-           "requests": n_req, "rows_per_gpu": rows, "seconds": dt,
+           "requests": n_req, "rows_per_gpu": rows, "seconds": dt, "steps": args.steps,
            "requests_per_s": n_req / dt, "tokens_per_s": n_req * n_out / dt,
            "tokens_per_s_per_gpu": rows * n_out / dt,
            "decode_ms_per_step": step_ms,
@@ -354,7 +357,7 @@ def c3_leg(dev, args):
     """BASELINE config 3: LLaVA-1.5-7B (CLIP-ViT-L/14-336 + Llama-7B geometry) bf16, batch = 8 images,
     prefill only: pinned-host pixel_values -> CLIP tower (23 of 24 blocks: feature layer -2) -> projector
     -> merge -> LM prefill of the 8 requests (576 image + 32 text tokens each) incl. the first token.
-    The tower is fp32-accurate like the reference's (split-operand tcgen05 GEMMs: every Linear runs as
+    The tower is fp32-accurate like the reference's (split-operand wgmma GEMMs: every Linear runs as
     W.x_hi + W.x_lo, i.e. 2x the algorithmic MMA flops; attention / LayerNorm in fp32 on the CUDA cores)."""
     import numpy as np
     import torch
@@ -391,11 +394,11 @@ def c3_leg(dev, args):
         eng.stream.synchronize()
         return ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])
 
-    for _ in range(3):
+    for _ in range(args.warmup):
         step()
-    K = max(2, min(args.steps, 5))
+    K = args.steps
     torch.cuda.synchronize()
-    sampler = ClockSampler(dev.index or 0)     # this leg is the power-hungry one (dense tcgen05 work for ~0.1 s per step)
+    sampler = ClockSampler(dev.index or 0)     # this leg is the power-hungry one (dense tensor-core work for ~0.1 s per step)
     sampler.start()
     t0 = time.perf_counter()
     tw, pf, per_step = 0.0, 0.0, []
@@ -478,9 +481,9 @@ def c4_leg(dev, args):
         eng.stream.synchronize()
         return ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2]), ev[2].elapsed_time(ev[3])
 
-    for _ in range(2):
+    for _ in range(args.warmup):
         step()
-    K = max(2, min(args.steps, 3))
+    K = args.steps
     l0 = eng.launch_count
     acc = [0.0, 0.0, 0.0]
     for _ in range(K):
@@ -528,8 +531,12 @@ def main():
     ap.add_argument("--pdl", action="store_true")
     ap.add_argument("--no-mega", action="store_true")
     ap.add_argument("--mega-mode", type=int, default=None,
-                    help="decode kernel: 0 per-phase kernels, 1 k_mega (CUDA cores), 2 k_mega_tc (tcgen05)")
+                    help="decode kernel: 0 per-phase kernels, 1 k_mega (CUDA cores), 2 k_mega_tc (wgmma)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed request as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -541,7 +548,7 @@ def main():
                           "tokens in (T=272), 512 greedy tokens out, batch 1",
               "global_batch": world, "parallelism": f"dp{world} (one replica per GPU, "
               "no per-step collective)", "l2": "weights streamed per token (3.09 GB) exceed the "
-              "126 MB L2; no flush needed"}
+              "50 MB L2 of the H100; no flush needed"}
 
     # ------------------------------------------------------------ reference arm
     if args.impl == "reference":
@@ -575,7 +582,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------ CUDA arm
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -659,6 +666,18 @@ def main():
     wall = time.perf_counter() - t0
     launches = eng.launch_count - l0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # the last request's greedy ids (device token ring, index = token number % capacity): the token
+        # sampled by the prefill head, then the N_OUT decode steps; and the logprobs of its last decode
+        # step, as a caller of the timed path receives them
+        n_tok, cap = eng.tokens_launched, eng.token_log_capacity
+        idx = torch.arange(n_tok - N_OUT - 1, n_tok, device=dev) % cap
+        with torch.cuda.stream(eng.stream):
+            toks = eng.token_log_view()[idx].cpu().numpy().astype(np.float64)
+            lps = eng.logprobs_view().float().cpu().numpy()
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "tokens.npy"), toks)
+        np.save(os.path.join(args.dump_outputs, "last_logprobs.npy"), lps)
 
     # ---- e2e through the public API with a host image --------------------------
     def e2e_step():
@@ -701,7 +720,7 @@ def main():
         img_tps = world * K * 144 / (pre_ms / 1e3)
         peak, peak_src = _peaks()
         tpeak, tpeak_src = _tensor_peak()
-        traffic, traffic_src = _ncu_traffic()
+        traffic, traffic_src = None, "not measured"
         pre_tflops = (VIT_GFLOP + PREFILL_GFLOP_T272) / (pre_ms / K)   # GFLOP / ms = TFLOP/s
         mean_ctx = T + N_OUT / 2
         bytes_per_step = W_BYTES_2B + KV_BYTES_PER_POS * mean_ctx
@@ -733,7 +752,7 @@ def main():
                          "traffic": traffic, "traffic_source": traffic_src},
             # the other half of the metric: ViT + merge + LM prefill (T=272) on the tensor cores
             "roofline_prefill": {"kernels": "ViT (32 blocks) + merge + LM prefill (28 layers, T=272): "
-                                            "tcgen05 GEMMs + tcgen05 attention + row ops",
+                                            "wgmma GEMMs + wgmma attention + row ops",
                                  "bound": "tensor", "achieved": pre_tflops, "peak": tpeak,
                                  "unit": "TFLOP/s", "frac": pre_tflops / tpeak, "peak_source": tpeak_src,
                                  "algorithmic_gflop": VIT_GFLOP + PREFILL_GFLOP_T272},

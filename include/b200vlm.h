@@ -1,5 +1,5 @@
 /*
- * b200vlm — C ABI of the B200-native generate path (libb200vlm.so).
+ * b200vlm — C ABI of the H100-native generate path (libb200vlm.so).
  *
  * The reference (Blaizzy/mlx-vlm) has NO FFI: its hot path is Python calling the
  * third-party `mlx` array library.  This header is the boundary a maintainer
@@ -29,7 +29,7 @@ extern "C" {
 #define B200_OK 0
 #define B200_ERR_INVALID 1     /* bad argument / unsupported shape            */
 #define B200_ERR_CUDA 2        /* a CUDA runtime / driver call failed         */
-#define B200_ERR_UNSUPPORTED 3 /* device is not sm_100                        */
+#define B200_ERR_UNSUPPORTED 3 /* device is not sm_90 (Hopper)                */
 #define B200_ERR_STATE 4       /* engine used before weights / cache bound    */
 
 #define B200_ABI_VERSION 1
@@ -65,7 +65,7 @@ int b200_cast_f32_bf16(const float* src, void* dst, long n, void* stream);
 /* nn.Linear / nn.Conv3d(kernel==stride) / Embedding.as_linear:
  *   C[M,N] = epi( bf16( A[M,K] . W[N,K]^T + bias[N] ) )  then, if residual,
  *   C = bf16(residual + C).   A row pitch lda, C/residual row pitch ldc/ldr
- *   (elements).  tcgen05 tensor cores, TMA-fed, fp32 accumulate in TMEM.
+ *   (elements).  Hopper tensor cores (wgmma), TMA-fed, fp32 accumulate in registers.
  *   Replaces every nn.Linear in models/qwen2_vl/{vision,language}.py and
  *   PatchEmbed.proj (vision.py:83-102).  K*2 bytes and lda*2 bytes must be
  *   multiples of 16. */
@@ -239,7 +239,7 @@ long b200_engine_launch_count(const b200_engine* e);
 int b200_engine_set_graph(b200_engine* e, int enabled);
 /* decode-step implementation.  0: one kernel per phase (28 x 5 + 2 launches);
  * 1: ONE persistent kernel, CUDA-core GEMV consumers (k_mega: weight ring + software grid
- * barrier); 2: the same step with tcgen05 GEMV consumers on pre-packed tile images of
+ * barrier); 2: the same step with wgmma GEMV consumers on pre-packed tile images of
  * the weights (k_mega_tc; the engine allocates the packed copy on first use);
  * 3: as 2 with a full 16-row activation operand (debugging);
  * 4: k_mega in dataflow mode (three of the five per-layer grid barriers replaced by polling

@@ -1,10 +1,10 @@
-"""mlx_vlm_b200 — B200-native drop-in for the generate path of Blaizzy/mlx-vlm.
+"""mlx_vlm_b200 — H100-native drop-in for the generate path of Blaizzy/mlx-vlm.
 
 `import mlx_vlm_b200 as mlx_vlm` gives the reference's generate-path surface
 (reference mlx_vlm/__init__.py:7-20): load, generate, stream_generate,
 generate_step, batch_generate / BatchGenerator, prepare_inputs, GenerationResult,
 PromptCacheState.  The
-arithmetic lives in libb200vlm.so (hand-written sm_100a CUDA behind the C ABI of
+arithmetic lives in libb200vlm.so (hand-written sm_90a CUDA behind the C ABI of
 include/b200vlm.h); importing the package does not need a GPU, calling a model
 does (there is no CPU fallback).
 """

@@ -1,4 +1,4 @@
-"""Build libb200vlm.so (sm_100a only) in-tree with nvcc.
+"""Build libb200vlm.so (sm_90a only) in-tree with nvcc.
 
 `python -m mlx_vlm_b200.build` or `build()`; the .so lands next to this file so
 it travels with the repo snapshot to the GPU box (it is git-ignored).
@@ -13,10 +13,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200vlm.so")
-SOURCES = ["engine.cu", "gemm_tcgen05.cu", "rowops.cu", "attention.cu", "decode.cu", "decode_mega.cu",
+SOURCES = ["engine.cu", "gemm_tn.cu", "rowops.cu", "attention.cu", "decode.cu", "decode_mega.cu",
            "decode_mega_tc.cu", "attention_tc.cu", "gemm_wt.cu", "attention_fa.cu", "decode_batch.cu", "tower_f32.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -59,7 +59,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed building libb200vlm.so")
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
            "-Xcompiler", "-fPIC"]
     subprocess.check_call(cmd)
     with open(stamp, "w") as f:

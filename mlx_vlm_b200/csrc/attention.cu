@@ -7,7 +7,7 @@
 // is lossless since they are already rounded), not an online-softmax.
 //
 // v1: CUDA-core FMA, one CTA per (16 query rows, head); K/V tiles are re-read
-// through L1 by the 8 warps of the CTA.  [round 2: HMMA/tcgen05 version]
+// through L1 by the 8 warps of the CTA.  The tensor-core version is attention_tc.cu.
 #include <stdlib.h>
 
 #include "common.cuh"

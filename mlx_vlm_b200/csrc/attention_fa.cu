@@ -1,22 +1,17 @@
-// Prefill / vision attention, pipelined: TMA-fed, warp-specialised, tcgen05 with double-buffered
-// score tiles in TMEM.  Same arithmetic and rounding points as attention_tc.cu (the reference's
-// mlx-CPU SDPA: oracle/mlx_semantics.py::sdpa; models/base.py:305-373, qwen2_vl/vision.py:154):
+// Prefill / vision attention: TMA-fed, warp-specialised, wgmma (Hopper) with the scores and the
+// output in registers.  The loads are pipelined (a producer warpgroup fills double-buffered K and
+// V^T slots ahead of the consumers); the MMAs of a consumer are not: Q.K^T, softmax and P.V of a
+// tile run one after another.  Same arithmetic and rounding points as attention_tc.cu (the
+// reference's mlx-CPU SDPA: oracle/mlx_semantics.py::sdpa; models/base.py:305-373, qwen2_vl/vision.py:154):
 //     qs = bf16(q * bf16(scale))       -- done by the rotary kernels that already touch q
 //     s  = bf16(qs . k^T);  p = bf16(softmax_fp32(s));  o = bf16(p . v)
 // p is rounded AFTER normalisation with the final row max / sum, so the kernel is two-pass over
 // the keys and the second pass recomputes the score tile on the tensor cores.
-//
-// attention_tc.cu (round 1) staged every tile with the compute threads and ran
-// load -> sync -> MMA -> wait -> softmax strictly in sequence (61 us per ViT layer, 2 % of the
-// tensor peak).  Here, per CTA = 128 query rows of one head:
-//   warp 0      TMA producer: Q once, K tiles for both passes, V^T tiles for pass 2 (3-D tensor
-//               maps over the packed qkv buffer / the KV cache, 128B swizzle, zero-filled tails)
-//   warp 1      MMA issuer:  S[i % 2] = Qs . K^T  (M128 x N128, TMEM cols 0..255)
-//                            O += P . V           (M128 x N=hd, TMEM cols 256..)
-//               the P.V of tile j is issued AFTER the Q.K^T of tile j+1, so the tensor core
-//               computes the next scores while the softmax warps work on the current ones
-//   warps 2..9  softmax: two threads per query row (64 score columns each), TMEM -> registers,
-//               pass 1: running max / sum of exp;  pass 2: p -> shared memory (the A operand)
+// Per CTA = 128 query rows of one head:
+//   warpgroup 0     TMA producer: Q once, K tiles for both passes, V^T tiles for pass 2 (3-D tensor
+//                   maps over the packed qkv buffer / the KV cache, 128B swizzle, zero-filled tails)
+//   warpgroups 1,2  64 query rows each: S = Qs . K^T (m64n128), softmax in registers (a row is held
+//                   by the 4 threads of a quad), O += P . V with P as the register A operand
 // V is consumed as V^T ([head][dim][key], keys contiguous): a K-major B operand that TMA can
 // load directly; the rotary kernels emit it (rowops.cu: *_qkv_post).
 #include <mutex>
@@ -24,6 +19,7 @@
 
 #include "common.cuh"
 #include "decode.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
@@ -31,7 +27,7 @@ namespace {
 
 constexpr int FA_TQ = 128, FA_TK = 128;
 constexpr int FA_BLK = 16 * 1024;       // one 128-row x 64-column bf16 operand block
-constexpr int FA_THREADS = 320;         // producer warp, MMA warp, 8 softmax warps
+constexpr int FA_THREADS = 384;         // producer warpgroup, 2 consumer warpgroups
 
 struct FaParams {
   bf16* out;
@@ -43,8 +39,7 @@ struct FaParams {
 };
 
 struct FaBars {
-  uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2], s_full[2], s_empty[2], p_full, p_empty,
-      o_full;
+  uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
 __device__ __forceinline__ uint32_t f_u32(const void* p) {
@@ -81,55 +76,21 @@ __device__ __forceinline__ void f_tma_3d(void* dst, const CUtensorMap* tmap, uin
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(c2), "r"(f_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void f_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void f_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void f_fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void f_umma(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc,
-                                       uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void f_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(f_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ uint32_t f_desc_lo(uint32_t addr) { return ((addr & 0x3FFFFu) >> 4) | (1u << 16); }
-constexpr uint32_t F_DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-
-__device__ __forceinline__ void f_tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void f_tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void f_sbar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 // 2^x on the SFU (one MUFU instruction, rel. error 2^-22: far below the bf16 rounding of p that follows)
 __device__ __forceinline__ float f_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+
+// row max / sum over the 4 threads of a quad (they hold the same accumulator rows)
+__device__ __forceinline__ float f_quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float f_quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 __global__ void __launch_bounds__(FA_THREADS, 1)
@@ -143,15 +104,12 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   extern __shared__ uint8_t fa_smem_raw[];
   __shared__ FaBars bars;
-  __shared__ uint32_t tmem_slot;
-  __shared__ float2 stat[2][FA_TQ];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(fa_smem_raw) + 1023) &
                                            ~static_cast<uintptr_t>(1023));
   uint8_t* Qs = sm;                          // [128 q][128 d]            2 k-blocks
   uint8_t* Ks = sm + 2 * FA_BLK;             // 2 slots x [128 keys][128 d]
   uint8_t* Vs = sm + 6 * FA_BLK;             // 2 slots x 2 key-blocks x [hdp d][64 keys]
-  uint8_t* Ps = sm + 10 * FA_BLK;            // [128 q][128 keys]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int h = blockIdx.y, kvh = h / (p.n_heads / p.n_kv);
   const int row0 = blockIdx.x * FA_TQ;
   const int S = p.S;
@@ -169,32 +127,18 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     f_init(&bars.q_full, 1);
     for (int i = 0; i < 2; ++i) {
       f_init(&bars.k_full[i], 1);
-      f_init(&bars.k_empty[i], 1);
+      f_init(&bars.k_empty[i], 8);   // one arrival per consumer warp
       f_init(&bars.v_full[i], 1);
-      f_init(&bars.v_empty[i], 1);
-      f_init(&bars.s_full[i], 1);
-      f_init(&bars.s_empty[i], 256);
+      f_init(&bars.v_empty[i], 8);
     }
-    f_init(&bars.p_full, 256);
-    f_init(&bars.p_empty, 1);
-    f_init(&bars.o_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(f_u32(&tmem_slot)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  f_fence_before();
   __syncthreads();
-  f_fence_after();
-  const uint32_t tmem = tmem_slot;
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
-  if (warp == 0) {
-    if (lane == 0) {  // ===== TMA producer =====
+  if (wg == 0) {
+    if (threadIdx.x == 0) {  // ===== TMA producer =====
       f_expect_tx(&bars.q_full, (uint32_t)kbq * FA_BLK);
       for (int c = 0; c < kbq; ++c) f_tma_3d(Qs + c * FA_BLK, &tmQ, &bars.q_full, c * 64, h, p.q0 + row0);
       for (int i = 0; i < 2 * n_tiles; ++i) {
@@ -212,164 +156,138 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer =====
-      const uint32_t idesc_s = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(FA_TK >> 3) << 17) | (8u << 24);
-      const uint32_t idesc_o = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.hdp >> 3) << 17) | (8u << 24);
-      const uint32_t q_lo = f_desc_lo(f_u32(Qs)), p_lo = f_desc_lo(f_u32(Ps));
-      const int ksteps = p.hdp >> 4;
-      auto do_pv = [&](int j) {
-        const int sv = j & 1;
-        f_wait(&bars.p_full, j & 1);
-        f_wait(&bars.v_full[sv], (j >> 1) & 1);
-        f_fence_after();
-        const uint32_t v_lo = f_desc_lo(f_u32(Vs + sv * 2 * FA_BLK));
-        for (int ks = 0; ks < FA_TK / 16; ++ks) {
-          const uint32_t a = p_lo + (uint32_t)((ks >> 2) * (FA_BLK >> 4) + (ks & 3) * 2);
-          const uint32_t b = v_lo + (uint32_t)((ks >> 2) * (vblk >> 4) + (ks & 3) * 2);
-          f_umma(tmem + 256, a, b, F_DESC_HI, idesc_o, (j > 0 || ks > 0) ? 1u : 0u);
-        }
-        f_commit(&bars.p_empty);
-        f_commit(&bars.v_empty[sv]);
-      };
-      f_wait(&bars.q_full, 0);
-      for (int i = 0; i < 2 * n_tiles; ++i) {
-        const int s = i & 1;
-        f_wait(&bars.k_full[s], (i >> 1) & 1);
-        f_wait(&bars.s_empty[s], ((i >> 1) & 1) ^ 1);
-        f_fence_after();
-        const uint32_t k_lo = f_desc_lo(f_u32(Ks + s * 2 * FA_BLK));
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint32_t off = (uint32_t)((ks >> 2) * (FA_BLK >> 4) + (ks & 3) * 2);
-          f_umma(tmem + (uint32_t)s * 128u, q_lo + off, k_lo + off, F_DESC_HI, idesc_s, ks > 0 ? 1u : 0u);
-        }
-        f_commit(&bars.k_empty[s]);
-        f_commit(&bars.s_full[s]);
-        if (i > n_tiles) do_pv(i - n_tiles - 1);  // P.V of the previous pass-2 tile, under this Q.K^T
-      }
-      do_pv(n_tiles - 1);
-      f_commit(&bars.o_full);
+    return;
+  }
+
+  // ===== consumers: warpgroup c = wg - 1 owns query rows [64 c, 64 c + 64) of the tile; its thread holds
+  // rows r0 and r0 + 8 of the score / output accumulators (wgmma.cuh) =====
+  const int c = wg - 1;
+  const int r0 = c * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  int vis[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int qi = row0 + r0 + 8 * hr;
+    vis[hr] = (qi < p.Lq) ? (p.causal ? min(S, S - p.Lq + qi + 1) : S) : S;
+  }
+  const int col0 = 2 * (lane & 3);
+  constexpr float LOG2E = 1.4426950408889634f;
+  const uint32_t q_a = wg_smem(Qs) + c * 64 * 128;
+  const int ksteps = p.hdp >> 4;
+  float sacc[64];
+  // S = Qs . K^T of the tile in ring slot s (M64 x N128 per warpgroup), then the slot is released
+  auto scores = [&](int s, uint32_t par) {
+    f_wait(&bars.k_full[s], par);
+    const uint32_t k_a = wg_smem(Ks + s * 2 * FA_BLK);
+    wg_fence_acc(sacc);
+    wg_arrive();
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const uint32_t off = (uint32_t)((ks >> 2) * FA_BLK + (ks & 3) * 32);
+      wgmma_n128_ss(sacc, wg_desc(q_a + off), wg_desc(k_a + off), ks > 0 ? 1u : 0u);
     }
-  } else {
-    // ===== softmax warps: thread = (query row, score-column half) =====
-    const int q4 = warp & 3, half = (warp - 2) >> 2;
-    const int row = q4 * 32 + lane;
-    const int qi = row0 + row;
-    const int vis = (qi < p.Lq) ? (p.causal ? min(S, S - p.Lq + qi + 1) : S) : S;
-    const uint32_t t_row = tmem + ((uint32_t)(q4 * 32) << 16);
-    constexpr float LOG2E = 1.4426950408889634f;
-    // The softmax warps are the instruction-bound part of the kernel (2 warps per scheduler, 288+ score
-    // elements per thread and pass), so the inner loops are kept to ~6 instructions per element: bf16
-    // rounding by cvt + shift, one FMA into the exponent, ex2 on the SFU, multiplication by 1/l.
-    float m = -INFINITY, l = 0.f;
-    for (int i = 0; i < n_tiles; ++i) {  // ---- pass 1: row max and sum of exp over bf16 scores ----
-      const int s = i & 1;
-      f_wait(&bars.s_full[s], (i >> 1) & 1);
-      f_fence_after();
-      const int jbase = i * FA_TK + half * 64;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t r[32];
-        f_tmem_ld32(t_row + (uint32_t)(s * 128 + half * 64 + c0), r);
-        float sc[32];
-        float cm = -INFINITY;
-        if (jbase + c0 + 32 <= vis) {  // whole chunk visible: no per-element mask
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(sacc);
+    __syncwarp();
+    if (lane == 0) f_arrive(&bars.k_empty[s]);
+  };
+  f_wait(&bars.q_full, 0);
+  // The softmax is the instruction-bound part: the inner loops are kept to a few instructions per element
+  // (bf16 rounding, one FMA into the exponent, ex2 on the SFU, multiplication by 1/l).
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  for (int i = 0; i < n_tiles; ++i) {  // ---- pass 1: row max and sum of exp over bf16 scores ----
+    scores(i & 1, (i >> 1) & 1);
+    const int jbase = i * FA_TK + col0;
 #pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            sc[e] = rbf(__uint_as_float(r[e]));
-            cm = fmaxf(cm, sc[e]);
-          }
-        } else {
+    for (int hr = 0; hr < 2; ++hr) {
+      float cm = -INFINITY;
 #pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            sc[e] = (jbase + c0 + e < vis) ? rbf(__uint_as_float(r[e])) : -INFINITY;
-            cm = fmaxf(cm, sc[e]);
-          }
-        }
-        if (cm > -INFINITY) {
-          const float mn = fmaxf(m, cm);
-          const float nb = -mn * LOG2E;
-          float add = 0.f;
+      for (int e = 0; e < 64; e += 4) {
 #pragma unroll
-          for (int e = 0; e < 32; ++e) add += f_ex2(fmaf(sc[e], LOG2E, nb));
-          l = l * f_ex2((m - mn) * LOG2E) + add;
-          m = mn;
+        for (int u = 0; u < 2; ++u) {
+          const int idx = e + 2 * hr + u;
+          const float v = (jbase + 8 * (e >> 2) + u < vis[hr]) ? rbf(sacc[idx]) : -INFINITY;
+          sacc[idx] = v;
+          cm = fmaxf(cm, v);
         }
       }
-      f_fence_before();
-      f_arrive(&bars.s_empty[s]);
-    }
-    stat[half][row] = make_float2(m, l);
-    f_sbar();
-    {
-      const float2 a = stat[0][row], b = stat[1][row];
-      m = fmaxf(a.x, b.x);
-      l = (a.y > 0.f ? a.y * f_ex2((a.x - m) * LOG2E) : 0.f) + (b.y > 0.f ? b.y * f_ex2((b.x - m) * LOG2E) : 0.f);
-    }
-    const float inv_l = 1.0f / l;
-    const float nbm = -m * LOG2E;
-    for (int j = 0; j < n_tiles; ++j) {  // ---- pass 2: p = bf16(exp(s - m) / l) -> shared memory ----
-      const int i = n_tiles + j, s = i & 1;
-      f_wait(&bars.s_full[s], (i >> 1) & 1);
-      f_fence_after();
-      f_wait(&bars.p_empty, (j & 1) ^ 1);  // the previous P.V has consumed the P tile
-      uint8_t* prow = Ps + half * FA_BLK + row * 128;
-      const int jbase = j * FA_TK + half * 64;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t r[32];
-        f_tmem_ld32(t_row + (uint32_t)(s * 128 + half * 64 + c0), r);
-        const bool full = jbase + c0 + 32 <= vis;
+      cm = f_quad_max(cm);
+      if (cm > -INFINITY) {
+        const float mn = fmaxf(m[hr], cm);
+        const float nb = -mn * LOG2E;
+        float add = 0.f;
 #pragma unroll
-        for (int e = 0; e < 32; e += 8) {
-          float pv[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const float pe = f_ex2(fmaf(rbf(__uint_as_float(r[e + u])), LOG2E, nbm)) * inv_l;
-            pv[u] = (full || jbase + c0 + e + u < vis) ? pe : 0.f;
-          }
-          uint4 o;
-          o.x = pack2(pv[0], pv[1]); o.y = pack2(pv[2], pv[3]); o.z = pack2(pv[4], pv[5]); o.w = pack2(pv[6], pv[7]);
-          const int chunk = (c0 + e) >> 3;
-          *reinterpret_cast<uint4*>(prow + ((chunk ^ (row & 7)) << 4)) = o;
-        }
-      }
-      f_fence_before();
-      f_arrive(&bars.s_empty[s]);
-      f_fence_async();  // generic-proxy writes of P -> visible to the tensor core (async proxy)
-      f_arrive(&bars.p_full);
-    }
-    // ---- epilogue: O row -> bf16 -> global (16-column chunks alternate between the row's two threads) ----
-    f_wait(&bars.o_full, 0);
-    f_fence_after();
-    bf16* orow = p.out + (long)(p.q0 + qi) * p.o_ts + (long)h * p.hd;
-    for (int c0 = 16 * half; c0 < p.hd; c0 += 32) {
-      uint32_t r[16];
-      f_tmem_ld16(t_row + 256u + (uint32_t)c0, r);
-      if (qi < p.Lq) {
-        if (c0 + 16 <= p.hd) {
-          uint4 o0, o1;
-          o0.x = pack2(__uint_as_float(r[0]), __uint_as_float(r[1]));
-          o0.y = pack2(__uint_as_float(r[2]), __uint_as_float(r[3]));
-          o0.z = pack2(__uint_as_float(r[4]), __uint_as_float(r[5]));
-          o0.w = pack2(__uint_as_float(r[6]), __uint_as_float(r[7]));
-          o1.x = pack2(__uint_as_float(r[8]), __uint_as_float(r[9]));
-          o1.y = pack2(__uint_as_float(r[10]), __uint_as_float(r[11]));
-          o1.z = pack2(__uint_as_float(r[12]), __uint_as_float(r[13]));
-          o1.w = pack2(__uint_as_float(r[14]), __uint_as_float(r[15]));
-          *reinterpret_cast<uint4*>(orow + c0) = o0;
-          *reinterpret_cast<uint4*>(orow + c0 + 8) = o1;
-        } else {
-          for (int e = 0; e < 16 && c0 + e < p.hd; ++e) orow[c0 + e] = f2bf(__uint_as_float(r[e]));
-        }
+        for (int e = 0; e < 64; e += 4) add += f_ex2(fmaf(sacc[e + 2 * hr], LOG2E, nb)) + f_ex2(fmaf(sacc[e + 2 * hr + 1], LOG2E, nb));
+        l[hr] = l[hr] * f_ex2((m[hr] - mn) * LOG2E) + add;
+        m[hr] = mn;
       }
     }
   }
-  f_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    f_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+  float inv_l[2], nbm[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    inv_l[hr] = 1.0f / f_quad_sum(l[hr]);
+    nbm[hr] = -m[hr] * LOG2E;
+  }
+  float oacc[8][8];
+#pragma unroll
+  for (int ch = 0; ch < 8; ++ch)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) oacc[ch][e] = 0.f;
+  const int n_och = p.hdp >> 4;
+  for (int j = 0; j < n_tiles; ++j) {  // ---- pass 2: p = bf16(exp(s - m) / l), O += P . V ----
+    const int i = n_tiles + j;
+    scores(i & 1, (i >> 1) & 1);
+    const int jbase = j * FA_TK + col0;
+    uint32_t pa[8][4];  // P as the A operand of 8 k-steps of 16 keys
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {  // q: (row half, column group) of the A fragment
+        const int hr = q & 1, g = 2 * ks + (q >> 1);
+        float pv[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const float pe = f_ex2(fmaf(rbf(sacc[4 * g + 2 * hr + u]), LOG2E, nbm[hr])) * inv_l[hr];
+          pv[u] = (jbase + 8 * g + u < vis[hr]) ? pe : 0.f;
+        }
+        pa[ks][q] = pack2(pv[0], pv[1]);
+      }
+    }
+    const int sv = j & 1;
+    f_wait(&bars.v_full[sv], (j >> 1) & 1);
+    const uint32_t v_a = wg_smem(Vs + sv * 2 * FA_BLK);
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) wg_fence_acc(oacc[ch]);
+    wg_arrive();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t koff = (uint32_t)((ks >> 2) * vblk + (ks & 3) * 32);
+#pragma unroll
+      for (int ch = 0; ch < 8; ++ch)
+        if (ch < n_och) wgmma_n16_rs(oacc[ch], pa[ks], wg_desc(v_a + koff + ch * 2048), 1u);
+    }
+    wg_commit();
+    wg_wait<0>();
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) wg_fence_acc(oacc[ch]);
+    __syncwarp();
+    if (lane == 0) f_arrive(&bars.v_empty[sv]);
+  }
+  // ---- epilogue: O -> bf16 -> global, two columns per store ----
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int qi = row0 + r0 + 8 * hr;
+    if (qi >= p.Lq) continue;
+    bf16* orow = p.out + (long)(p.q0 + qi) * p.o_ts + (long)h * p.hd;
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) {
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        const int col = ch * 16 + g * 8 + col0;
+        if (col < p.hd)
+          *reinterpret_cast<uint32_t*>(orow + col) = pack2(oacc[ch][4 * g + 2 * hr], oacc[ch][4 * g + 2 * hr + 1]);
+      }
+    }
   }
 }
 
@@ -480,7 +398,7 @@ int attention_fa(const void* q, long q_ts, long q_hs, const void* k, long k_ts, 
   static unsigned long long set_mask = 0ull;
   int dev = 0;
   B200_CUDA(cudaGetDevice(&dev));
-  const size_t smem = 12 * FA_BLK + 1024;
+  const size_t smem = 10 * FA_BLK + 1024;
   if (!(set_mask >> (dev & 63) & 1ull)) {
     B200_CUDA(cudaFuncSetAttribute(attention_fa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     set_mask |= 1ull << (dev & 63);

@@ -1,4 +1,4 @@
-// Prefill / vision attention on the 5th-gen tensor cores, with the reference's mlx-CPU
+// Prefill / vision attention on the Hopper tensor cores (wgmma), with the reference's mlx-CPU
 // rounding points (oracle/mlx_semantics.py::sdpa; models/base.py:305-373,
 // qwen2_vl/vision.py:154):   qs = bf16(q*bf16(scale)); s = bf16(qs.k^T);
 // p = bf16(softmax_fp32(s)); o = bf16(p.v).
@@ -6,17 +6,17 @@
 // p must be rounded AFTER normalisation with the final row max / sum, so the kernel is
 // two-pass over the keys, and the second pass RECOMPUTES the score tile on the tensor
 // cores instead of keeping [rows x S] scores around (v1, attention.cu, kept them in shared
-// memory and ran on CUDA cores: 289 us per ViT layer at 576 tokens; this: see profiles/).
+// memory and ran on CUDA cores).
 //
-// One CTA = 128 query rows of one head; thread t owns row t == TMEM lane t, so the softmax
-// statistics are thread-local (no shuffles).
-//   S[128 x 128 keys] = Qs . K^T      tcgen05.mma, A = Qs, B = K tile, both K-major in
-//                                     128B-swizzled shared memory, fp32 in TMEM cols 0..127
-//   O[128 x hd]      += P . V         A = P (bf16, written by the threads), B = V^T tile
-//                                     (transposed on the way into shared memory), TMEM cols 128..
+// One CTA = 128 query rows of one head, two warpgroups of 64 rows each:
+//   S[64 x 128 keys] = Qs . K^T      wgmma m64n128k16, A = Qs, B = K tile, both K-major in
+//                                    128B-swizzled shared memory, fp32 in registers
+//   O[64 x hd]      += P . V         A = P (bf16 in registers), B = V^T tile
+//                                    (transposed on the way into shared memory)
 // Tiles are staged by the threads themselves (16-byte loads, swizzled stores): the head
 // dimension (80 for the ViT) is zero-padded to 128 on the fly, q is scaled while staged.
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
@@ -34,74 +34,16 @@ struct AttnTcParams {
   float scale_bf;
 };
 
-__device__ __forceinline__ uint32_t sa_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void a_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void a_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
 __device__ __forceinline__ void a_fence_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void a_mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  const uint32_t addr = sa_u32(bar);
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-  } while (!done);
+__device__ __forceinline__ float a_quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-__device__ __forceinline__ void a_umma(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi,
-                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void a_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   sa_u32(bar))
-               : "memory");
-}
-// K-major, 128B swizzle, 8-row groups 1024 B apart (see gemm_tcgen05.cu::make_smem_desc)
-__device__ __forceinline__ uint32_t a_desc_lo(uint32_t addr) {
-  return ((addr & 0x3FFFFu) >> 4) | (1u << 16);
-}
-constexpr uint32_t A_DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-
-__device__ __forceinline__ void a_tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void a_tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ float a_quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 // byte offset of element (row r, column c) of a [128 x 128] bf16 operand stored as two
@@ -111,7 +53,7 @@ __device__ __forceinline__ uint32_t sw_off(int r, int c) {
   return (uint32_t)(blk * KBLK + r * 128 + ((((cc >> 3) ^ (r & 7))) << 4) + ((cc & 7) << 1));
 }
 
-constexpr int ATC_THREADS = 256;  // two threads per query row (64 score columns each)
+constexpr int ATC_THREADS = 256;  // two warpgroups, 64 query rows each
 
 // stage `rows` x hd (zero-padded to 128 x 128) of a row-major source into an operand tile.
 // All loads of a thread are issued before its first store (one memory latency per tile; the
@@ -182,189 +124,146 @@ __device__ __forceinline__ void stage_vt(uint8_t* dst, const bf16* v, long row_s
 
 __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const AttnTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_s, bar_o;
-  __shared__ uint32_t tmem_slot;
-  __shared__ float2 stat[2][TQ];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                            ~static_cast<uintptr_t>(1023));
   uint8_t* Qs = sm;                 // [128 q][128 d]
   uint8_t* Ks = sm + 2 * KBLK;      // [128 keys][128 d]
   uint8_t* Vt = sm + 4 * KBLK;      // [128 d][128 keys]
-  uint8_t* Ps = sm + 6 * KBLK;      // [128 q][128 keys]
-  const int t = threadIdx.x, warp = t >> 5;
-  const int row = t & (TQ - 1), half = t >> 7;  // warps 4..7 share the TMEM lanes of warps 0..3
+  const int t = threadIdx.x, lane = t & 31;
+  const int wg = t >> 7;            // warpgroup wg owns query rows [64 wg, 64 wg + 64)
   const int h = blockIdx.y, kvh = h / (p.n_heads / p.n_kv);
   const int row0 = blockIdx.x * TQ;
   const int hd = p.hd, S = p.S;
 
-  if (t == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sa_u32(&bar_s)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sa_u32(&bar_o)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     sa_u32(&tmem_slot)),
-                 "r"(256u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   stage_rows<true>(Qs, p.q + (long)h * p.q_hs, p.q_ts, row0, p.Lq, hd, p.scale_bf);
-  a_fence_before();
-  a_fence_async();
-  __syncthreads();
-  a_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t t_s = tmem + ((uint32_t)((warp & 3) * 32) << 16) + half * 64;  // lane quarter, column half
-  const uint32_t t_o = tmem + ((uint32_t)((warp & 3) * 32) << 16) + 128;
 
   const bf16* kb = p.k + (long)kvh * p.k_hs;
   const bf16* vb = p.v + (long)kvh * p.v_hs;
-  const int qi = row0 + row;
-  // visible keys of this row (bottom-right aligned causal mask); rows past Lq compute on
-  // finite garbage and are never stored
-  const int vis = (qi < p.Lq) ? (p.causal ? min(S, S - p.Lq + qi + 1) : S) : S;
+  // this thread holds accumulator rows r0 and r0 + 8 (wgmma.cuh); visible keys per row (bottom-right
+  // aligned causal mask); rows past Lq compute on finite garbage and are never stored
+  const int r0 = wg * 64 + ((t >> 5) & 3) * 16 + (lane >> 2);
+  const int col0 = 2 * (lane & 3);
+  int vis[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int qi = row0 + r0 + 8 * hr;
+    vis[hr] = (qi < p.Lq) ? (p.causal ? min(S, S - p.Lq + qi + 1) : S) : S;
+  }
   const int q_last = min(row0 + TQ, p.Lq) - 1;
   const int vis_tile = p.causal ? min(S, S - p.Lq + q_last + 1) : S;
   const int n_tiles = (vis_tile + TK - 1) / TK;
 
-  const uint32_t q_lo = a_desc_lo(sa_u32(Qs)), k_lo = a_desc_lo(sa_u32(Ks));
-  const uint32_t p_lo = a_desc_lo(sa_u32(Ps)), v_lo = a_desc_lo(sa_u32(Vt));
-  // D = f32, A = B = bf16, K-major; M = 128; N = 128 keys (scores) / hd (output)
-  const uint32_t idesc_s = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TK >> 3) << 17) | (8u << 24);
-  const uint32_t idesc_o = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(hd >> 3) << 17) | (8u << 24);
+  const uint32_t q_a = wg_smem(Qs) + wg * 64 * 128, k_a = wg_smem(Ks), v_a = wg_smem(Vt);
   const int ksteps = hd >> 4;  // 16 dims per MMA
-  uint32_t ph_s = 0, ph_o = 0;
-
-  auto issue_scores = [&]() {
+  float sacc[64];
+  auto scores = [&]() {
+    wg_fence_acc(sacc);
+    wg_arrive();
     for (int ks = 0; ks < ksteps; ++ks) {
-      const uint32_t off = (uint32_t)((ks >> 2) * (KBLK >> 4) + (ks & 3) * 2);
-      a_umma(tmem, q_lo + off, k_lo + off, A_DESC_HI, idesc_s, ks > 0 ? 1u : 0u);
+      const uint32_t off = (uint32_t)((ks >> 2) * KBLK + (ks & 3) * 32);
+      wgmma_n128_ss(sacc, wg_desc(q_a + off), wg_desc(k_a + off), ks > 0 ? 1u : 0u);
     }
-    a_commit(&bar_s);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(sacc);
   };
   constexpr float LOG2E = 1.4426950408889634f;
 
   // ---------------- pass 1: row max and sum of exp over the bf16-rounded scores ----------------
-  float m = -INFINITY, l = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   for (int jt = 0; jt < n_tiles; ++jt) {
+    if (jt > 0) __syncthreads();  // every warpgroup's MMAs have read the previous K tile
     stage_rows<false>(Ks, kb, p.k_ts, jt * TK, S, hd, 0.f);
     a_fence_async();
     __syncthreads();
-    if (t == 0) {
-      a_fence_after();
-      issue_scores();
-    }
-    a_mbar_wait(&bar_s, ph_s);
-    ph_s ^= 1u;
-    a_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < 64; c0 += 32) {
-      uint32_t r[32];
-      a_tmem_ld32(t_s + c0, r);
-      float s[32];
+    scores();
+    const int jbase = jt * TK + col0;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
       float cm = -INFINITY;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int j = jt * TK + half * 64 + c0 + i;
-        s[i] = (j < vis) ? rbf(__uint_as_float(r[i])) : -INFINITY;
-        cm = fmaxf(cm, s[i]);
+      for (int e = 0; e < 64; e += 4) {
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int idx = e + 2 * hr + u;
+          const float v = (jbase + 8 * (e >> 2) + u < vis[hr]) ? rbf(sacc[idx]) : -INFINITY;
+          sacc[idx] = v;
+          cm = fmaxf(cm, v);
+        }
       }
+      cm = a_quad_max(cm);
       if (cm > -INFINITY) {
-        const float mn = fmaxf(m, cm);
+        const float mn = fmaxf(m[hr], cm);
         float add = 0.f;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) add += exp2f((s[i] - mn) * LOG2E);
-        l = l * exp2f((m - mn) * LOG2E) + add;
-        m = mn;
+        for (int e = 0; e < 64; e += 4)
+          add += exp2f((sacc[e + 2 * hr] - mn) * LOG2E) + exp2f((sacc[e + 2 * hr + 1] - mn) * LOG2E);
+        l[hr] = l[hr] * exp2f((m[hr] - mn) * LOG2E) + add;
+        m[hr] = mn;
       }
     }
-    a_fence_before();
-    __syncthreads();  // every thread has read its scores before the next tile overwrites them
   }
-  // combine the two column halves of each row
-  stat[half][row] = make_float2(m, l);
-  __syncthreads();
-  {
-    const float2 a = stat[0][row], b = stat[1][row];
-    m = fmaxf(a.x, b.x);
-    l = (a.y > 0.f ? a.y * exp2f((a.x - m) * LOG2E) : 0.f) + (b.y > 0.f ? b.y * exp2f((b.x - m) * LOG2E) : 0.f);
-  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) l[hr] = a_quad_sum(l[hr]);
 
   // ---------------- pass 2: p = bf16(exp(s - m) / l), O += P . V ----------------
+  float oacc[8][8];
+#pragma unroll
+  for (int ch = 0; ch < 8; ++ch)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) oacc[ch][e] = 0.f;
+  const int n_och = hd >> 4;
   for (int jt = 0; jt < n_tiles; ++jt) {
-    if (jt > 0) {  // the previous P.V must have consumed Ps / Vt
-      a_mbar_wait(&bar_o, ph_o);
-      ph_o ^= 1u;
-    }
+    __syncthreads();  // the previous tile's MMAs have read Ks / Vt
     stage_rows<false>(Ks, kb, p.k_ts, jt * TK, S, hd, 0.f);
     stage_vt(Vt, vb, p.v_ts, jt * TK, S, hd);
     a_fence_async();
     __syncthreads();
-    if (t == 0) {
-      a_fence_after();
-      issue_scores();
-    }
-    a_mbar_wait(&bar_s, ph_s);
-    ph_s ^= 1u;
-    a_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < 64; c0 += 32) {
-      uint32_t r[32];
-      a_tmem_ld32(t_s + c0, r);
+    scores();
+    const int jbase = jt * TK + col0;
+    uint32_t pa[8][4];  // P as the A operand of 8 k-steps of 16 keys
 #pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        float pv[8];
+    for (int ks = 0; ks < 8; ++ks) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int j = jt * TK + half * 64 + c0 + i + e;
-          pv[e] = (j < vis) ? exp2f((rbf(__uint_as_float(r[i + e])) - m) * LOG2E) / l : 0.f;
-        }
-        uint4 o;
-        o.x = pack2(pv[0], pv[1]); o.y = pack2(pv[2], pv[3]); o.z = pack2(pv[4], pv[5]); o.w = pack2(pv[6], pv[7]);
-        *reinterpret_cast<uint4*>(Ps + sw_off(row, half * 64 + c0 + i)) = o;
+      for (int q = 0; q < 4; ++q) {
+        const int hr = q & 1, g = 2 * ks + (q >> 1);
+        float pv[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+          pv[u] = (jbase + 8 * g + u < vis[hr]) ? exp2f((rbf(sacc[4 * g + 2 * hr + u]) - m[hr]) * LOG2E) / l[hr] : 0.f;
+        pa[ks][q] = pack2(pv[0], pv[1]);
       }
     }
-    a_fence_before();
-    a_fence_async();
-    __syncthreads();
-    if (t == 0) {
-      a_fence_after();
-      for (int ks = 0; ks < TK / 16; ++ks) {
-        const uint32_t off = (uint32_t)((ks >> 2) * (KBLK >> 4) + (ks & 3) * 2);
-        a_umma(tmem + 128, p_lo + off, v_lo + off, A_DESC_HI, idesc_o, (jt > 0 || ks > 0) ? 1u : 0u);
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) wg_fence_acc(oacc[ch]);
+    wg_arrive();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t koff = (uint32_t)((ks >> 2) * KBLK + (ks & 3) * 32);
+#pragma unroll
+      for (int ch = 0; ch < 8; ++ch)
+        if (ch < n_och) wgmma_n16_rs(oacc[ch], pa[ks], wg_desc(v_a + koff + ch * 2048), 1u);
+    }
+    wg_commit();
+    wg_wait<0>();
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) wg_fence_acc(oacc[ch]);
+  }
+  // ---------------- epilogue: O -> bf16 -> global, two columns per store ----------------
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int qi = row0 + r0 + 8 * hr;
+    if (qi >= p.Lq) continue;
+    bf16* orow = p.out + (long)qi * p.o_ts + (long)h * hd;
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) {
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        const int col = ch * 16 + g * 8 + col0;
+        if (col < hd)
+          *reinterpret_cast<uint32_t*>(orow + col) = pack2(oacc[ch][4 * g + 2 * hr], oacc[ch][4 * g + 2 * hr + 1]);
       }
-      a_commit(&bar_o);
     }
-  }
-  a_mbar_wait(&bar_o, ph_o);
-  a_fence_after();
-  // ---------------- epilogue: O row -> bf16 -> global (16-column chunks alternate between
-  // the two threads of a row) ----------------
-  bf16* orow = p.out + (long)qi * p.o_ts + (long)h * hd;
-  for (int c0 = 16 * half; c0 < hd; c0 += 32) {
-    uint32_t r[16];
-    a_tmem_ld16(t_o + c0, r);
-    if (qi < p.Lq) {
-      uint4 o0, o1;
-      o0.x = pack2(__uint_as_float(r[0]), __uint_as_float(r[1]));
-      o0.y = pack2(__uint_as_float(r[2]), __uint_as_float(r[3]));
-      o0.z = pack2(__uint_as_float(r[4]), __uint_as_float(r[5]));
-      o0.w = pack2(__uint_as_float(r[6]), __uint_as_float(r[7]));
-      o1.x = pack2(__uint_as_float(r[8]), __uint_as_float(r[9]));
-      o1.y = pack2(__uint_as_float(r[10]), __uint_as_float(r[11]));
-      o1.z = pack2(__uint_as_float(r[12]), __uint_as_float(r[13]));
-      o1.w = pack2(__uint_as_float(r[14]), __uint_as_float(r[15]));
-      *reinterpret_cast<uint4*>(orow + c0) = o0;
-      *reinterpret_cast<uint4*>(orow + c0 + 8) = o1;
-    }
-  }
-  a_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    a_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(256u)
-                 : "memory");
   }
 }
 
@@ -382,7 +281,7 @@ int attention_tc(const void* q, long q_ts, long q_hs, const void* k, long k_ts, 
                  const void* v, long v_ts, long v_hs, void* out, long o_ts, int n_heads, int n_kv,
                  int hd, int Lq, int S, int causal, float scale, cudaStream_t st) {
   static unsigned long long set_mask = 0ull;
-  const size_t smem = 8 * KBLK + 1024;
+  const size_t smem = 6 * KBLK + 1024;
   if (first_use_on_device(&set_mask)) {
     B200_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (int)smem));

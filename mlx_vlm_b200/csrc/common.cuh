@@ -1,4 +1,4 @@
-// Common device/host helpers for the b200vlm kernels (sm_100a only).
+// Common device/host helpers for the b200vlm kernels (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -130,7 +130,7 @@ __device__ __forceinline__ void l2_prefetch_span(const void* base, long bytes, i
 
 // ---- programmatic dependent launch -------------------------------------------------
 // Every kernel of the prefill / vision / batched-decode sequences starts with pdl_prologue():
-// it lets the NEXT kernel of the stream begin (its barrier / TMEM set-up and the prefetch of its
+// it lets the NEXT kernel of the stream begin (its barrier set-up and the prefetch of its
 // weights overlap this kernel) and then waits until everything the PREVIOUS kernels wrote is visible.
 __device__ __forceinline__ void pdl_prologue() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");

@@ -801,9 +801,9 @@ __global__ void k_set_state(DecState* st, int tok, int ctx, int pos, int use_for
 // ---------------------------------------------------------------------------
 // host-side launchers
 // ---------------------------------------------------------------------------
-static int g_sm_count = 148;
-static bool g_pdl = false;  // measured on B200: no gain for this kernel mix (DESIGN.md)
-void decode_set_sm_count(int n) { g_sm_count = n > 0 ? n : 148; }
+static int g_sm_count = 132;
+static bool g_pdl = false;  // off by default; programmatic dependent launch for this kernel mix: not measured on the H100
+void decode_set_sm_count(int n) { g_sm_count = n > 0 ? n : 132; }
 void decode_set_pdl(bool on) { g_pdl = on; }
 
 template <typename... KArgs, typename... Args>

@@ -73,7 +73,7 @@ struct MegaP {
 int mega_fill(MegaP& p, int sm_count);
 int mega_launch(const MegaP& p, int sm_count, cudaStream_t s);
 
-// ---- k_mega_tc (decode_mega_tc.cu): the same step with tcgen05 GEMV phases ---------
+// ---- k_mega_tc (decode_mega_tc.cu): the same step with wgmma GEMV phases -----------
 struct LayerWT {
   const uint8_t *wqkv, *wo, *wgu, *wd;  // tile images (128 rows x 64 cols, 128B swizzle)
 };
@@ -176,7 +176,7 @@ int embed_merge(const int* ids, int B, int T, const void* table, int hidden, con
                 cudaStream_t st);
 int gemm_bf16_tn(const void* A, long lda, const void* W, const void* bias, const void* residual,
                  long ldr, void* C, long ldc, int M, int N, int K, int epilogue, cudaStream_t st);
-// weight-major tcgen05 GEMM (gemm_wt.cu) + the row op that finishes its split-K partials
+// weight-major wgmma GEMM (gemm_wt.cu) + the row op that finishes its split-K partials
 struct WtConfig {
   int TN, KS, stages, split;
 };

@@ -6,7 +6,7 @@
 // the KV pool is (layer, k/v, row, kv head, capacity, head_dim), the per-row state (next token,
 // cache length, rope position) lives in device arrays, and one captured CUDA graph per step
 // replays unchanged while rows join and leave:
-//   per layer   qkv      gemm_wt (weight-major tcgen05 GEMM, token tile 16, split-K partials)
+//   per layer   qkv      gemm_wt (weight-major wgmma GEMM, token tile 16, split-K partials)
 //               bd_attn  finishes q/k/v from the partials (+bias, M-RoPE at the row's position,
 //                        KV append at the row's length) and attends over the row's keys
 //               o_proj   gemm_wt partials -> finish_rows (+residual, RMSNorm)
@@ -553,10 +553,9 @@ static int bd_attn_launch(int ag, dim3 grid, size_t smem, cudaStream_t s, const 
   }
 }
 
-// L2 prefetch budget of the latency-bound kernels of a step, in bytes (B200_BD_PREFETCH_MB).  DEFAULT 0 = off: measured on
-// C5 (Qwen2-VL-7B, 8 rows) the step got SLOWER with it — 3.672 ms off, 3.745 ms at 60 MB, 3.804 ms at 96 MB
-// (profiles/r2_bd_l2_prefetch_ab.txt): the prefetch traffic lengthens the attention kernel's dependent round trips by
-// more than the L2-resident weights save the GEMMs.  Kept as a tuning knob.
+// L2 prefetch budget of the latency-bound kernels of a step, in bytes (B200_BD_PREFETCH_MB).  DEFAULT 0 = off: the
+// prefetch traffic can lengthen the attention kernel's dependent round trips by more than the L2-resident weights save
+// the GEMMs (not measured on the H100, whose L2 is 50 MB).  Kept as a tuning knob.
 static long bd_prefetch_budget() {
   static long v = -1;
   if (v < 0) {

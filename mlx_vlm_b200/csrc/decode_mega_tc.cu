@@ -1,86 +1,40 @@
-// k_mega_tc: the decode step as one persistent kernel whose GEMV phases run on the 5th-gen
-// tensor cores (tcgen05.mma, fp32 accumulators in TMEM).
+// k_mega_tc: the decode step as one persistent kernel whose GEMV phases run on the tensor
+// cores (wgmma.mma_async, fp32 accumulators in the registers of warpgroup 0).
 //
-// Why: in k_mega (decode_mega.cu) the 8 consumer warps need ~0.9 us of CUDA-core
-// instructions per 48 KB weight tile, while HBM delivers a tile per SM every ~1.08 us only
-// if nothing else is in the way; the step ends up instruction-latency bound (43 % of the
-// measured HBM peak).  Here a weight tile is consumed by 12 tcgen05.mma instructions issued
-// by ONE thread (~0.2 us), so the stream is bounded by HBM and by the phase boundaries only,
-// and the N dimension of the MMA (16 columns) is free for up to 16 batched sequences.
+// Why: in k_mega (decode_mega.cu) the 8 consumer warps spend CUDA-core instructions on every
+// weight element; here a weight tile is consumed by a few wgmma instructions, so the stream is
+// bounded by HBM and by the phase boundaries only.
 //
 //   * weights are re-packed once at load into TILE IMAGES: row block (128 rows) x K block
-//     (64 columns) = 16 KB in the 128-byte-swizzled K-major layout tcgen05 reads, K blocks of
+//     (64 columns) = 16 KB in the 128-byte-swizzled K-major layout wgmma reads, K blocks of
 //     a row block contiguous -> the producer's plain 1-D cp.async.bulk lands a ready A operand;
-//   * the activation vector is the B operand: 8 (aliased to 16) rows x K, row 0 = x;
-//   * D[128 x 16] per unit lives in TMEM (4 slots of 16 columns); warps 0..3 read their lane
-//     quarter with tcgen05.ld and run the per-row epilogue, thread 128 issues the MMAs;
+//   * the activation vector is the B operand: 8 rows x K, row 0 = x (m64n8k16, two per 128 rows);
+//   * warps 0..3 issue the MMAs of a unit, exchange column 0 through shared memory and run the
+//     per-row epilogue (thread = row);
 //   * phases with few rows (qkv, o_proj, down) are split along K over the SMs; their fp32
 //     partial sums are reduced, in a fixed order, by the prologue of the NEXT phase, which
 //     also carries the residual stream in shared memory (no global round trip for h).
 // Rounding points: oracle/qwen2vl.py::lm_layers_forward (fp32 accumulation, one bf16 rounding
 // per Linear, RMSNorm 2 roundings, residual add 1).
 #include "mega_common.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
 namespace {
 
 constexpr int TC_SUB = 16 * 1024;   // one tile image: 128 rows x 64 bf16, 128B swizzle
-constexpr int TC_ACC_SLOTS = 4;
-constexpr int TC_ACC_COLS = 16;
 
 struct TcShared {
   MegaShared m;
-  uint64_t acc_full[TC_ACC_SLOTS], acc_empty[TC_ACC_SLOTS];
-  uint32_t tmem_slot;
+  float vrow[128];      // column 0 of a unit's accumulator: one value per row of the row block
   float xch[64];        // gate/up exchange between the lane halves of a row block
   float redf[8];
   float2 lse_w[4];
 };
 
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
 __device__ __forceinline__ void fence_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-// descriptors are passed as (lo, hi) 32-bit words: the start-address field lives in the low
-// word, so walking an operand is ONE 32-bit add per MMA on the issuing thread (which is the
-// only thread feeding the tensor core: ~25 instructions per MMA made the first version
-// issue-bound at ~1 us per 48 KB tile)
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi,
-                                          uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   s_u32(bar))
-               : "memory");
-}
-// K-major operand, 128B swizzle: rows of 128 B, 8-row groups `sbo` bytes apart.
-// low word: start address >> 4 [0,14), LBO (unused) [16,30); high word: SBO >> 4 [0,14),
-// descriptor version 1 at bit 14 (46), SWIZZLE_128B = 2 at bits 29..31 (61..63)
-__device__ __forceinline__ uint32_t desc_lo(uint32_t addr) {
-  return ((addr & 0x3FFFFu) >> 4) | (1u << 16);
-}
-__device__ __forceinline__ uint32_t desc_hi(uint32_t sbo) {
-  return (sbo >> 4) | (1u << 14) | (2u << 29);
-}
-__device__ __forceinline__ float tmem_ld1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  return __uint_as_float(r);
 }
 __device__ __forceinline__ void ebar() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
 
@@ -144,56 +98,6 @@ __device__ __forceinline__ void tc_l2_prefetch(const MegaTcP& P, const MegaTcPha
                    "r"((uint32_t)n * TC_SUB)
                    : "memory");
     }
-  }
-}
-
-// ---- MMA issuer (one thread) ---------------------------------------------------------
-__device__ __forceinline__ void tc_mma(const MegaTcP& P, const MegaTcPhase& g, uint8_t* ring,
-                                       const uint8_t* xop, TcShared* sh, Ring& rg,
-                                       uint32_t& acc_it, uint32_t tmem_base, bool xfull,
-                                       long long* tdbg) {
-  int tn = 0;
-  if (tdbg) tdbg[tn++] = gtimer();
-  // D = f32, A = B = bf16, both K-major, N = 16, M = 128
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_ACC_COLS >> 3) << 17) |
-                         ((uint32_t)(128 >> 4) << 24);
-  const uint32_t xop_lo = desc_lo(s_u32(xop));
-  const uint32_t ring_lo = desc_lo(s_u32(ring));
-  const uint32_t a_hi = desc_hi(1024), b_hi = desc_hi((uint32_t)P.x_sbo);
-  const uint32_t kstep = (uint32_t)P.x_kstride >> 4, stage16 = (uint32_t)P.base.stage_bytes >> 4;
-  for (int u = blockIdx.x; u < g.units; u += gridDim.x) {
-    const TcUnit t = tc_unit(g, u);
-    const uint32_t slot = acc_it % TC_ACC_SLOTS, par = (acc_it / TC_ACC_SLOTS) & 1u;
-    ++acc_it;
-    mb_wait(&sh->acc_empty[slot], par ^ 1u, &sh->m.err);
-    tc_fence_after();
-    const uint32_t dcol = tmem_base + slot * TC_ACC_COLS;
-    uint32_t accum = 0;
-    for (int kb = t.kb0; kb < t.kb1; kb += P.sps) {
-      const int n = min(P.sps, t.kb1 - kb);
-      const int s = rg.slot();
-      mb_wait(&sh->m.full_bar[s], rg.parity(), &sh->m.err);
-      tc_fence_after();
-      if (tdbg && tn < 27) tdbg[tn++] = gtimer();
-      const uint32_t a0 = ring_lo + (uint32_t)s * stage16;
-      // the operand holds either the whole vector (norm phases) or this unit's K slice
-      const uint32_t b0 = xop_lo + (uint32_t)(kb - (xfull ? 0 : t.kb0)) * kstep;
-#pragma unroll
-      for (int sb = 0; sb < 3; ++sb) {
-        if (sb < n) {
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            umma_bf16(dcol, a0 + sb * (TC_SUB >> 4) + kk * 2, a_hi, b0 + sb * kstep + kk * 2, b_hi,
-                      idesc, accum);
-            accum = 1;
-          }
-        }
-      }
-      umma_commit(&sh->m.empty_bar[s]);  // the ring slot is free once these MMAs retire
-      if (tdbg && tn < 27) tdbg[tn++] = gtimer();
-      rg.advance();
-    }
-    umma_commit(&sh->acc_full[slot]);
   }
 }
 
@@ -344,24 +248,67 @@ __device__ __forceinline__ void pro_slice(const MegaTcP& P, uint8_t* xop, const 
   PRO_STAMP();
 }
 
-// ---- epilogues (warps 0..3, thread = one row of the row block) ---------------------------
+// ---- consumers (warpgroup 0 = warps 0..3): the MMAs of a unit, then its per-row epilogue ----------
+// D[128 rows x 8] = W tile . X^T as two m64n8k16 halves per 16-wide K step; only column 0 (operand
+// row 0 = the activation vector) is used.  Thread r of the warpgroup then owns row r of the block.
 template <int MODE>
-__device__ __forceinline__ void tc_epilogue(const MegaTcP& P, const MegaTcPhase& g, TcShared* sh,
-                                            uint32_t& acc_it, uint32_t tmem_base, long long* acc_out,
-                                            bf16* out) {
+__device__ __forceinline__ void tc_consume(const MegaTcP& P, const MegaTcPhase& g, uint8_t* ring,
+                                           const uint8_t* xop, TcShared* sh, Ring& rg, bool xfull,
+                                           long long* acc_out, bf16* out, long long* tdbg) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r = warp * 32 + lane;
+  int tn = 0;
+  if (tdbg && r == 0) tdbg[tn++] = gtimer();
+  const uint32_t xop_a = wg_smem(xop), ring_a = wg_smem(ring);
   float run_m = -INFINITY, run_l = 0.f;
   for (int u = blockIdx.x; u < g.units; u += gridDim.x) {
     const TcUnit t = tc_unit(g, u);
-    const uint32_t slot = acc_it % TC_ACC_SLOTS, par = (acc_it / TC_ACC_SLOTS) & 1u;
-    ++acc_it;
-    mb_wait(&sh->acc_full[slot], par, &sh->m.err);
-    tc_fence_after();
-    const float v = tmem_ld1(tmem_base + ((uint32_t)(warp * 32) << 16) + slot * TC_ACC_COLS);
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mb_arrive(&sh->acc_empty[slot]);
+    float acc[2][4];
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[hf][i] = 0.f;
+    for (int kb = t.kb0; kb < t.kb1; kb += P.sps) {
+      const int n = min(P.sps, t.kb1 - kb);
+      const int s = rg.slot();
+      mb_wait(&sh->m.full_bar[s], rg.parity(), &sh->m.err);
+      if (tdbg && r == 0 && tn < 27) tdbg[tn++] = gtimer();
+      const uint32_t a0 = ring_a + (uint32_t)s * (uint32_t)P.base.stage_bytes;
+      // the operand holds either the whole vector (norm phases) or this unit's K slice
+      const uint32_t b0 = xop_a + (uint32_t)(kb - (xfull ? 0 : t.kb0)) * (uint32_t)P.x_kstride;
+      wg_fence_acc(acc[0]);
+      wg_fence_acc(acc[1]);
+      wg_arrive();
+#pragma unroll
+      for (int sb = 0; sb < 3; ++sb) {
+        if (sb < n) {
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const uint64_t db = wg_desc(b0 + sb * P.x_kstride + kk * 32);
+            wgmma_n8_ss(acc[0], wg_desc(a0 + sb * TC_SUB + kk * 32), db, 1u);
+            wgmma_n8_ss(acc[1], wg_desc(a0 + sb * TC_SUB + 64 * 128 + kk * 32), db, 1u);
+          }
+        }
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(acc[0]);
+      wg_fence_acc(acc[1]);
+      __syncwarp();
+      if (lane == 0) mb_arrive(&sh->m.empty_bar[s]);  // this warp's MMAs have read the ring slot
+      if (tdbg && r == 0 && tn < 27) tdbg[tn++] = gtimer();
+      rg.advance();
+    }
+    if ((lane & 3) == 0) {
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        sh->vrow[hf * 64 + warp * 16 + (lane >> 2)] = acc[hf][0];
+        sh->vrow[hf * 64 + warp * 16 + (lane >> 2) + 8] = acc[hf][2];
+      }
+    }
+    ebar();
+    const float v = sh->vrow[r];
+    ebar();
     if (MODE == PH_GATEUP) {
       // rows 0..63 = gate, 64..127 = up of the same 64 intermediate channels
       if (r >= 64) sh->xch[r - 64] = v;
@@ -405,23 +352,12 @@ __device__ __forceinline__ void tc_epilogue(const MegaTcP& P, const MegaTcPhase&
 
 template <int MODE>
 __device__ __forceinline__ void tc_run(const MegaTcP& P, const MegaTcPhase& g, uint8_t* ring,
-                                       const uint8_t* xop, TcShared* sh, Ring& rg, uint32_t& acc_it,
-                                       uint32_t tmem_base, long long* acc_out, bf16* out,
+                                       const uint8_t* xop, TcShared* sh, Ring& rg, long long* acc_out, bf16* out,
                                        long long* tdbg = nullptr) {
-  const int warp = threadIdx.x >> 5;
-  if (warp == 4) {
-    if ((threadIdx.x & 31) == 0)
-      tc_mma(P, g, ring, xop, sh, rg, acc_it, tmem_base,
-             MODE == PH_QKV || MODE == PH_GATEUP || MODE == PH_HEAD, tdbg);
-    else {
-      for (int u = blockIdx.x; u < g.units; u += gridDim.x) ++acc_it;
-    }
-    __syncwarp();
-  } else if (warp < 4) {
-    tc_epilogue<MODE>(P, g, sh, acc_it, tmem_base, acc_out, out);
+  if ((threadIdx.x >> 5) < 4) {
+    tc_consume<MODE>(P, g, ring, xop, sh, rg, MODE == PH_QKV || MODE == PH_GATEUP || MODE == PH_HEAD, acc_out, out,
+                     tdbg);
     if (tdbg && threadIdx.x == 0) tdbg[28] = gtimer();
-  } else {
-    for (int u = blockIdx.x; u < g.units; u += gridDim.x) ++acc_it;
   }
 }
 
@@ -443,11 +379,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega_tc(const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.n_stages; ++s) {
       mb_init(&sh.m.full_bar[s], 1);
-      mb_init(&sh.m.empty_bar[s], 1);
-    }
-    for (int s = 0; s < TC_ACC_SLOTS; ++s) {
-      mb_init(&sh.acc_full[s], 1);
-      mb_init(&sh.acc_empty[s], 4);
+      mb_init(&sh.m.empty_bar[s], 4);  // one arrival per consumer warp
     }
     sh.m.err = 0;
     for (int i = 0; i < d.hd / 2; ++i) sh.m.invf[i] = p.inv_freq[i];
@@ -456,17 +388,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega_tc(const __grid_consta
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 4) {  // whole warp: tcgen05.alloc is .sync.aligned
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     s_u32(&sh.tmem_slot)),
-                 "r"((uint32_t)(TC_ACC_SLOTS * TC_ACC_COLS))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sh.tmem_slot;
   Ring rg;
   rg.cur = 0;
   rg.ph = 0;
@@ -496,7 +418,6 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega_tc(const __grid_consta
 
   // ===== consumers =====
   unsigned bidx = 0;
-  uint32_t acc_it = 0;
   const int ctx = p.st->ctx, pos = p.st->pos;
   for (int l = 0; l < p.n_layers; ++l) {
     const LayerW& lw = p.layers[l];
@@ -504,7 +425,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega_tc(const __grid_consta
     bf16* vc = kc + p.kv_v_offset;
     // ---- qkv: h (+ previous layer's down partials) -> norm -> split-K partials ----
     pro_norm(P, xop, hres, &sh, P.d_acc, l == 0, lw.ln1);
-    tc_run<PH_QKV>(P, P.ph[PH_QKV], ring, xop, &sh, rg, acc_it, tmem_base, P.qkv_acc, nullptr);
+    tc_run<PH_QKV>(P, P.ph[PH_QKV], ring, xop, &sh, rg, P.qkv_acc, nullptr);
     grid_barrier(p, &sh.m, bidx);
     // ---- attention (finishes q/k/v from the partials) ----
     if ((int)blockIdx.x < p.attn_ctas) {
@@ -516,14 +437,14 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega_tc(const __grid_consta
     // ---- o_proj: split-K partials ----
     zero_acc(P.d_acc, d.hidden);  // last read by this layer's qkv prologue, next written by down
     pro_attn_slice(P, xop, P.ph[PH_ORES]);
-    tc_run<PH_ORES>(P, P.ph[PH_ORES], ring, xop, &sh, rg, acc_it, tmem_base, P.o_acc, nullptr);
+    tc_run<PH_ORES>(P, P.ph[PH_ORES], ring, xop, &sh, rg, P.o_acc, nullptr);
     grid_barrier(p, &sh.m, bidx);
     // ---- gate/up: h += o ; norm ; SwiGLU ----
     long long* td = (p.dbg && l == 5 && blockIdx.x == 0) ? p.dbg + 4096 : nullptr;
     if (td && threadIdx.x == 128) td[0] = gtimer();
     zero_acc(P.qkv_acc, P.ph[PH_QKV].N);  // read by this layer's attention, next written by qkv
     pro_norm(P, xop, hres, &sh, P.o_acc, false, lw.ln2, td ? p.dbg + 4096 + 160 : nullptr);
-    tc_run<PH_GATEUP>(P, P.ph[PH_GATEUP], ring, xop, &sh, rg, acc_it, tmem_base, nullptr, p.act,
+    tc_run<PH_GATEUP>(P, P.ph[PH_GATEUP], ring, xop, &sh, rg, nullptr, p.act,
                       td ? td + 1 : nullptr);
     grid_barrier(p, &sh.m, bidx);
     // ---- down: split-K partials ----
@@ -531,19 +452,13 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega_tc(const __grid_consta
     if (td && threadIdx.x == 128) td[0] = gtimer();
     zero_acc(P.o_acc, d.hidden);  // read by this layer's gate/up prologue, next written by o_proj
     pro_slice(P, xop, P.ph[PH_DRES], p.act, td ? p.dbg + 4096 + 176 : nullptr);
-    tc_run<PH_DRES>(P, P.ph[PH_DRES], ring, xop, &sh, rg, acc_it, tmem_base, P.d_acc, nullptr,
+    tc_run<PH_DRES>(P, P.ph[PH_DRES], ring, xop, &sh, rg, P.d_acc, nullptr,
                     td ? td + 1 : nullptr);
     grid_barrier(p, &sh.m, bidx);
   }
   pro_norm(P, xop, hres, &sh, P.d_acc, p.n_layers == 0, p.final_norm);
-  tc_run<PH_HEAD>(P, P.ph[PH_HEAD], ring, xop, &sh, rg, acc_it, tmem_base, nullptr, p.logits);
+  tc_run<PH_HEAD>(P, P.ph[PH_HEAD], ring, xop, &sh, rg, nullptr, p.logits);
   grid_barrier(p, &sh.m, bidx);
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"((uint32_t)(TC_ACC_SLOTS * TC_ACC_COLS))
-                 : "memory");
-  }
   mega_sample_finalize(p, sh.m, bidx);
 }
 

@@ -35,7 +35,7 @@ using namespace b200;
 
 struct b200_engine {
   b200_qwen2vl_config cfg;
-  int device = 0, sm_count = 148;
+  int device = 0, sm_count = 132;
   std::unordered_map<std::string, const bf16*> w;
   std::unordered_map<std::string, long> wn;
   bool resolved = false;
@@ -78,7 +78,7 @@ struct b200_engine {
   cudaEvent_t loc_ev = nullptr;
   // captured CUDA graphs of the vision tower / the prefill layers, keyed by everything that is baked
   // into their nodes (shapes, workspace, KV binding): the sequences are ~500 small launches, which
-  // the host cannot enqueue as fast as the B200 executes them
+  // the host cannot enqueue as fast as the GPU executes them
   struct SeqGraph {
     std::vector<long> key;
     cudaGraphExec_t exec = nullptr;
@@ -105,7 +105,7 @@ struct b200_engine {
   int attn_cluster = 8;
   int prepared_cap = -1, prepared_cluster = -1;
   // megakernel
-  int use_mega = 1;  // 0: one kernel per phase, 1: k_mega (CUDA cores), 2: k_mega_tc (tcgen05)
+  int use_mega = 1;  // 0: one kernel per phase, 1: k_mega (CUDA cores), 2: k_mega_tc (wgmma)
   bool mega_fits = true;  // false: this shape / cache capacity does not fit the persistent kernel
   int active_mega() const { return mega_fits ? use_mega : 0; }
   MegaTcP tp;
@@ -245,7 +245,7 @@ static int mega_prepare(b200_engine* e, cudaStream_t s) {
   p.partials = e->partials; p.st = e->st; p.token_log = e->token_log; p.log_cap = e->log_cap;
   p.force = e->force; p.inv_freq = e->lm_inv_freq; p.bar = e->bar; p.advance = 1;
   p.dbg = e->dbg;
-  // tuning aids (defaults chosen from the sweeps recorded in profiles/)
+  // tuning aids
   p.max_inflight = e->fma_inflight;
   p.flow = e->flow;
   {
@@ -761,8 +761,8 @@ int b200_abi_version(void) { return B200_ABI_VERSION; }
 int b200_device_check(int device, int* sm_count) {
   cudaDeviceProp prop;
   B200_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major,
               prop.minor);
     return B200_ERR_UNSUPPORTED;
   }
@@ -1219,7 +1219,7 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   if (e->use_mega && e->mega_fits && !e->mega_ready) {
     if ((rc = mega_prepare(e, s))) {
       // a geometry the persistent kernel cannot hold (very long cache: the attention scratch
-      // leaves no room for the weight ring; > 148 attention CTAs; ...): same step, one kernel per
+      // leaves no room for the weight ring; > 132 attention CTAs; ...): same step, one kernel per
       // phase — still this library's CUDA path.  b200_last_error() keeps the reason.
       if (rc != B200_ERR_INVALID) return rc;
       e->mega_fits = false;

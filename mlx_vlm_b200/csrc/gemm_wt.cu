@@ -1,27 +1,23 @@
 // gemm_wt: the Linear layers of the prefill / vision / batched-decode paths as a WEIGHT-MAJOR
-// tcgen05 GEMM:   D[n, t] = sum_k W[n, k] * X[t, k]      (C[t, n] = D[n, t])
+// wgmma GEMM:   D[n, t] = sum_k W[n, k] * X[t, k]      (C[t, n] = D[n, t])
 //
-// Why weight-major ("swap AB"): the token count of this path is small and awkward for the
-// tensor core's M = 128 side (T = 272 -> 3 tiles, one of them 88 % padding; T = 576 -> 4.5
-// tiles; batched decode T <= 16), while the weight rows are many and regular.  So the
-// weight rows take the UMMA M side (128 rows per CTA, streamed exactly once per token tile)
-// and the tokens the N side, whose width TN is any multiple of 16 up to 256 and is chosen per
-// problem (T = 272 -> 2 x 144, T = 576 -> 3 x 192, decode batch -> 16): no padded MMA rows,
-// 2-3x less weight re-streaming than 128-row token tiles.
+// Why weight-major ("swap AB"): the token count of this path is small and awkward for a 64- or
+// 128-row M side, while the weight rows are many and regular.  So the weight rows take the M side
+// (128 rows per CTA, 64 per consumer warpgroup, streamed exactly once per token tile) and the
+// tokens the N side, whose width TN is any multiple of 16 up to 256 and is chosen per problem.
 //
 //   * TMA (cp.async.bulk.tensor, 128B swizzle) feeds a shared-memory ring of `n_stages` stages
-//     of KS k-blocks (64 columns each); one elected thread issues tcgen05.mma (fp32 accumulators
-//     in TMEM: 128 lanes = weight rows x TN columns = tokens);
+//     of KS k-blocks (64 columns each); warpgroup 0 is the producer, warpgroups 1 and 2 issue
+//     wgmma m64n16k16 per 16 tokens (fp32 accumulators in registers);
 //   * programmatic dependent launch: the weight tiles of the first stages do not depend on the
 //     previous kernel and are requested BEFORE griddepcontrol.wait, so the cold-HBM latency of a
-//     layer's weights overlaps the previous kernel's tail; shared memory is kept <= 113 KB where
-//     that does not hurt so that two CTAs (of this or the next kernel) share an SM;
+//     layer's weights overlaps the previous kernel's tail;
 //   * split-K over gridDim.z for the GEMMs with few weight rows and long K (o_proj, down, fc2):
 //     fp32 partial tiles, summed in a FIXED order by the row-op kernel that follows
 //     (finish_rows: bias + residual + RMSNorm / LayerNorm of the next block, fused);
-//   * epilogue: TMEM -> registers (lane = weight row) -> transposed through shared memory ->
-//     coalesced 16-byte rows of C (bias / GELU / residual), or SwiGLU of interleaved gate/up
-//     row blocks (64 + 64 rows per tile, two TMA boxes), or fp32 partial tiles.
+//   * epilogue: registers -> transposed through shared memory -> coalesced 16-byte rows of C
+//     (bias / GELU / residual), or SwiGLU of interleaved gate/up row blocks (64 + 64 rows per
+//     tile, two TMA boxes), or fp32 partial tiles.
 //
 // Replaces nn.Linear of the reference (models/qwen2_vl/vision.py:83-102,108-119,132-133,168-169;
 // language.py:52-55; mlp.py:9-15; activations.py:8-10).  Rounding points follow
@@ -32,6 +28,7 @@
 
 #include "common.cuh"
 #include "decode.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
@@ -42,6 +39,8 @@ constexpr int WT_BK = 64;           // one k-block: 64 bf16 = 128 B = one swizzl
 constexpr int WT_WBLK = WT_ROWS * 128;  // bytes of one weight k-block tile
 constexpr int WT_MAX_STAGES = 16;
 constexpr int WT_EPI_TOK = 64;      // tokens staged per epilogue pass
+constexpr int WT_THREADS = 384;    // producer warpgroup + 2 consumer warpgroups
+constexpr int WT_TN_AUTO = 128;    // widest token tile the automatic / measured choice uses
 
 struct WtParams {
   const bf16* bias;
@@ -102,92 +101,67 @@ __device__ __forceinline__ void w_tma_2d(void* dst, const CUtensorMap* tmap, uin
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(w_smem_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void w_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void w_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// descriptors as (lo, hi) words: walking an operand is one 32-bit add per MMA
-__device__ __forceinline__ void w_umma(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi,
-                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void w_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   w_smem_u32(bar))
-               : "memory");
-}
-// K-major, 128B swizzle, 8-row groups 1024 B apart
-__device__ __forceinline__ uint32_t w_desc_lo(uint32_t addr) {
-  return ((addr & 0x3FFFFu) >> 4) | (1u << 16);
-}
-constexpr uint32_t W_DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-
-__device__ __forceinline__ void w_tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void w_pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void w_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void w_ebar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void w_ebar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // the 2 consumer warpgroups
 
-// TMEM registers of one lane (weight row) -> bf16 staging tile [token][row]: + bias, one rounding, activation
+// accumulator -> bf16 staging element: + bias, one rounding, activation
 template <int EPI>
-__device__ __forceinline__ void wt_stage_bf16(const uint32_t (&a)[32], float bias_v, bf16* sb) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    float v = rbf(__uint_as_float(a[j]) + bias_v);
-    if constexpr (EPI == B200_EPI_GELU_FAST) v = gelu_fast_bf(v);
-    if constexpr (EPI == B200_EPI_GELU_EXACT) v = gelu_exact_bf(v);
-    sb[j * WT_ROWS] = f2bf(v);
-  }
+__device__ __forceinline__ bf16 wt_stage_bf16(float acc, float bias_v) {
+  float v = rbf(acc + bias_v);
+  if constexpr (EPI == B200_EPI_GELU_FAST) v = gelu_fast_bf(v);
+  if constexpr (EPI == B200_EPI_GELU_EXACT) v = gelu_exact_bf(v);
+  return f2bf(v);
 }
 
 // the fp32-accurate paths: no rounding anywhere
 template <int EPI>
-__device__ __forceinline__ void wt_stage_f32(const uint32_t (&a)[32], float bias_v, float* sf) {
+__device__ __forceinline__ float wt_stage_f32(float acc, float bias_v) {
+  float v = acc + bias_v;
+  if constexpr (EPI == B200_EPI_GELU_FAST) v = v * sigmoid_f(1.702f * v);
+  if constexpr (EPI == B200_EPI_GELU_EXACT) v = v * (1.0f + erff(v / 1.41421356237309515f)) * 0.5f;
+  if constexpr (EPI == B200_EPI_GELU_TANH) {
+    const float u = 0.7978845608028654f * (v + 0.044715f * v * v * v);
+    v = 0.5f * v * (1.0f + tanhf(u));
+  }
+  return v;
+}
+
+// Accumulator chunks (16 tokens each) of pass c0 -> staging tile [token][weight row].  KIND: 0 = raw fp32
+// (partial tiles), 1 = bf16 with the epilogue EPI, 2 = fp32 with the epilogue EPI.
+template <int KIND, int EPI, int WT_MAX_CH>
+__device__ __forceinline__ void wt_stage(const float (&acc)[WT_MAX_CH][8], int n_ch, int c0, int row_lo,
+                                         const float (&bias_v)[2], uint8_t* stg) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    float v = __uint_as_float(a[j]) + bias_v;
-    if constexpr (EPI == B200_EPI_GELU_FAST) v = v * sigmoid_f(1.702f * v);
-    if constexpr (EPI == B200_EPI_GELU_EXACT) v = v * (1.0f + erff(v / 1.41421356237309515f)) * 0.5f;
-    if constexpr (EPI == B200_EPI_GELU_TANH) {
-      const float u = 0.7978845608028654f * (v + 0.044715f * v * v * v);
-      v = 0.5f * v * (1.0f + tanhf(u));
+  for (int c = 0; c < WT_MAX_CH; ++c) {
+    if (c >= n_ch || c * 16 < c0 || c * 16 >= c0 + WT_EPI_TOK) continue;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int hr = (i >> 1) & 1;
+      const int row = row_lo + 8 * hr;
+      const int tl = c * 16 - c0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      if constexpr (KIND == 0) reinterpret_cast<float*>(stg)[tl * WT_ROWS + row] = acc[c][i];
+      else if constexpr (KIND == 1) reinterpret_cast<bf16*>(stg)[tl * WT_ROWS + row] = wt_stage_bf16<EPI>(acc[c][i], bias_v[hr]);
+      else reinterpret_cast<float*>(stg)[tl * WT_ROWS + row] = wt_stage_f32<EPI>(acc[c][i], bias_v[hr]);
     }
-    sf[j * WT_ROWS] = v;
   }
 }
 
 // TOWER = false: the bf16 paths (B200_WT_BF16 / PARTIAL / SWIGLU); TOWER = true: the fp32-accurate paths
 // (B200_WT_F32 / SPLIT).  Two instantiations keep each one's code small (tools/wt_ab_probe.py A/B-times builds).
-template <bool TOWER>
-__global__ void __launch_bounds__(256, 2)
+// WT_MAX_CH: 16-token accumulator chunks per thread, 8 (TN <= 128) or 16 (TN <= 256).  The 16-chunk
+// instantiation spills (168 registers per thread at 384 threads); it serves explicit configurations
+// only, the automatic and measured choices stay at TN <= WT_TN_AUTO.
+template <bool TOWER, int WT_MAX_CH>
+__global__ void __launch_bounds__(WT_THREADS, 1)
 gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
                const WtParams p) {
   extern __shared__ uint8_t wt_smem_raw[];
   __shared__ uint64_t full_bar[WT_MAX_STAGES], empty_bar[WT_MAX_STAGES];
-  __shared__ uint64_t tmem_full;
-  __shared__ uint32_t tmem_slot;
   uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wt_smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const bool swiglu = !TOWER && (p.mode == B200_WT_SWIGLU);
   const int rb = blockIdx.x;
   const int n0 = rb * (swiglu ? 64 : WT_ROWS);  // first output feature (SwiGLU: channel) of the tile
@@ -200,8 +174,6 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
   const int xblk = p.TN * 128;                      // bytes of one token k-block tile
   const int stage_bytes = p.KS * (WT_WBLK + xblk);
   const int NS = p.n_stages;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < p.TN) tmem_cols <<= 1;
 
   w_pdl_launch();  // the next kernel may start its prologue / weight prefetch as SM resources free up
 
@@ -234,34 +206,23 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
   };
 
   const int pre = n_it < NS ? n_it : NS;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmX)) : "memory");
     for (int s = 0; s < NS; ++s) {
       w_mbar_init(&full_bar[s], 1);
-      w_mbar_init(&empty_bar[s], 1);
+      w_mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
-    w_mbar_init(&tmem_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     // weights never depend on the previous kernel: request them before waiting for it
     for (int it = 0; it < pre; ++it) issue_w(it, it);
   }
-  if (warp == 2) {  // whole warp: tcgen05.alloc is .sync.aligned
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     w_smem_u32(&tmem_slot)),
-                 "r"(tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  w_fence_before();
   __syncthreads();
-  w_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   w_pdl_wait();  // everything the previous kernels wrote (X, residual) is visible from here on
 
-  if (warp == 0) {
-    if (lane == 0) {  // ===== TMA producer =====
+  if (wg == 0) {
+    if (threadIdx.x == 0) {  // ===== TMA producer =====
       for (int it = 0; it < pre; ++it) issue_x(it, it);
       for (int it = pre; it < n_it; ++it) {
         const int s = it % NS;
@@ -270,67 +231,71 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
         issue_x(it, s);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer =====
-      // D = f32, A = B = bf16, both K-major; M = 128 weight rows, N = TN tokens
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.TN >> 3) << 17) |
-                             ((uint32_t)(WT_ROWS >> 4) << 24);
-      uint32_t acc = 0;
-      for (int it = 0; it < n_it; ++it) {
-        const int s = it % NS;
-        w_mbar_wait(&full_bar[s], (it / NS) & 1);
-        w_fence_after();
-        if (!(p.flags & 1u)) {
-          const uint32_t w_lo = w_desc_lo(w_smem_u32(ring + (long)s * stage_bytes));
-          const uint32_t x_lo = w_desc_lo(w_smem_u32(ring + (long)s * stage_bytes + p.KS * WT_WBLK));
-          const int cnt = min(p.KS, kb1 - kb0 - it * p.KS);
-          for (int j = 0; j < cnt; ++j) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              w_umma(tmem_base, w_lo + (uint32_t)(j * (WT_WBLK >> 4) + kk * 2),
-                     x_lo + (uint32_t)(j * (xblk >> 4) + kk * 2), W_DESC_HI, idesc, acc);
-              acc = 1;
-            }
-          }
-        }
-        w_commit(&empty_bar[s]);  // frees the ring slot when these MMAs retire
-      }
-      w_commit(&tmem_full);
-    }
+    return;
   }
-  __syncwarp();
 
-  // ===== epilogue (all 8 warps): warp w reads TMEM lane quarter w % 4, token half w / 4 =====
-  w_mbar_wait(&tmem_full, 0);
-  w_fence_after();
-  const int q = warp & 3, half = warp >> 2;
-  const int row = q * 32 + lane;  // weight row of the tile == TMEM lane
-  float bias_v = 0.f;
-  if ((TOWER || p.mode == B200_WT_BF16) && p.bias && n0 + row < p.N) bias_v = bf2f(p.bias[n0 + row]);
-  uint8_t* stg = ring;  // every TMA load has landed and every MMA has retired: the ring is free
-  const int tid = threadIdx.x;
-  for (int c0 = 0; c0 < p.TN; c0 += WT_EPI_TOK) {
-    const int cc = c0 + half * 32;
-    if (cc < p.TN && !(p.flags & 1u)) {
-      uint32_t a[32];
-      w_tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, a);
-      if (!TOWER && p.mode == B200_WT_PARTIAL) {
-        float* sf = reinterpret_cast<float*>(stg);
+  // ===== consumers: warpgroup c = wg - 1 multiplies weight rows [64 c, 64 c + 64) by the TN tokens,
+  // 16 tokens per wgmma (accumulator chunk ch = tokens [16 ch, 16 ch + 16)) =====
+  const int c = wg - 1;
+  const int n_ch = p.TN >> 4;
+  float acc[WT_MAX_CH][8];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) sf[(half * 32 + j) * WT_ROWS + row] = __uint_as_float(a[j]);
+  for (int ch = 0; ch < WT_MAX_CH; ++ch)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[ch][i] = 0.f;
+  for (int it = 0; it < n_it; ++it) {
+    const int s = it % NS;
+    w_mbar_wait(&full_bar[s], (it / NS) & 1);
+    if (!(p.flags & 1u)) {
+      const uint32_t w_a = wg_smem(ring + (long)s * stage_bytes) + c * 64 * 128;
+      const uint32_t x_a = wg_smem(ring + (long)s * stage_bytes + p.KS * WT_WBLK);
+      const int cnt = min(p.KS, kb1 - kb0 - it * p.KS);
+#pragma unroll
+      for (int ch = 0; ch < WT_MAX_CH; ++ch) wg_fence_acc(acc[ch]);
+      wg_arrive();
+      for (int j = 0; j < cnt; ++j) {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t dw = wg_desc(w_a + j * WT_WBLK + kk * 32);
+#pragma unroll
+          for (int ch = 0; ch < WT_MAX_CH; ++ch)
+            if (ch < n_ch) wgmma_n16_ss(acc[ch], dw, wg_desc(x_a + j * xblk + ch * 2048 + kk * 32), 1u);
+        }
+      }
+      wg_commit();
+      wg_wait<0>();
+#pragma unroll
+      for (int ch = 0; ch < WT_MAX_CH; ++ch) wg_fence_acc(acc[ch]);
+    }
+    __syncwarp();
+    if (lane == 0) w_mbar_arrive(&empty_bar[s]);  // this warp's MMAs have read the ring slot
+  }
+
+  // ===== epilogue (the 256 consumer threads) =====
+  const int tid = threadIdx.x - 128;
+  const int row_lo = c * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);  // weight rows row_lo and row_lo + 8
+  float bias_v[2] = {0.f, 0.f};
+  if ((TOWER || p.mode == B200_WT_BF16) && p.bias) {
+    if (n0 + row_lo < p.N) bias_v[0] = bf2f(p.bias[n0 + row_lo]);
+    if (n0 + row_lo + 8 < p.N) bias_v[1] = bf2f(p.bias[n0 + row_lo + 8]);
+  }
+  uint8_t* stg = ring;  // reused once both warpgroups have finished reading the ring
+  w_ebar();
+  for (int c0 = 0; c0 < p.TN; c0 += WT_EPI_TOK) {
+    if (!(p.flags & 1u)) {
+      if (!TOWER && p.mode == B200_WT_PARTIAL) {
+        wt_stage<0, B200_EPI_NONE, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
       } else if constexpr (TOWER) {
-        float* sf = reinterpret_cast<float*>(stg) + (half * 32) * WT_ROWS + row;
-        if (p.epilogue == B200_EPI_GELU_FAST) wt_stage_f32<B200_EPI_GELU_FAST>(a, bias_v, sf);
-        else if (p.epilogue == B200_EPI_GELU_EXACT) wt_stage_f32<B200_EPI_GELU_EXACT>(a, bias_v, sf);
-        else if (p.epilogue == B200_EPI_GELU_TANH) wt_stage_f32<B200_EPI_GELU_TANH>(a, bias_v, sf);
-        else wt_stage_f32<B200_EPI_NONE>(a, bias_v, sf);
+        if (p.epilogue == B200_EPI_GELU_FAST) wt_stage<2, B200_EPI_GELU_FAST, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
+        else if (p.epilogue == B200_EPI_GELU_EXACT) wt_stage<2, B200_EPI_GELU_EXACT, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
+        else if (p.epilogue == B200_EPI_GELU_TANH) wt_stage<2, B200_EPI_GELU_TANH, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
+        else wt_stage<2, B200_EPI_NONE, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
       } else {
-        // one unrolled loop per epilogue kind, chosen OUTSIDE the loop: left to itself the compiler merged the
-        // three kinds into one predicated body of ~90 instructions per element (6-7 us per launch, A/B measured)
-        bf16* sb = reinterpret_cast<bf16*>(stg) + (half * 32) * WT_ROWS + row;
-        if (p.epilogue == B200_EPI_GELU_FAST) wt_stage_bf16<B200_EPI_GELU_FAST>(a, bias_v, sb);
-        else if (p.epilogue == B200_EPI_GELU_EXACT) wt_stage_bf16<B200_EPI_GELU_EXACT>(a, bias_v, sb);
-        else wt_stage_bf16<B200_EPI_NONE>(a, bias_v, sb);
+        // one unrolled loop per epilogue kind, chosen OUTSIDE the loop: left to itself the compiler merges the
+        // three kinds into one predicated body per element
+        if (p.epilogue == B200_EPI_GELU_FAST) wt_stage<1, B200_EPI_GELU_FAST, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
+        else if (p.epilogue == B200_EPI_GELU_EXACT) wt_stage<1, B200_EPI_GELU_EXACT, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
+        else wt_stage<1, B200_EPI_NONE, WT_MAX_CH>(acc, n_ch, c0, row_lo, bias_v, stg);
       }
     }
     w_ebar();
@@ -444,14 +409,6 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
       }
     }
     w_ebar();
-  }
-  w_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    w_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(tmem_cols)
-                 : "memory");
   }
 }
 
@@ -667,15 +624,18 @@ void gemm_wt_set_pdl(bool on) { g_wt_pdl = on; }
 
 static int round16(int x) { return (x + 15) & ~15; }
 
-// Tile / pipeline configuration for (T, row blocks, K): a small cost model calibrated on the round-2
-// sweep (profiles/r2_gemm_wt_sweep.txt, B200):
-//   * a CTA costs ~4.5 us of fixed latency (launch, barrier/TMEM set-up, first TMA round trip,
-//     epilogue) + per k-block max(MMA time, shared-memory fill time at ~130 GB/s per SM);
-//   * two CTAs share an SM when a configuration needs <= ~110 KB of shared memory: the fixed part of
-//     one overlaps the main loop of the other, which wins whenever more than one wave exists;
+// Tile / pipeline configuration for (T, row blocks, K) from a small cost model.  Its rates are H100
+// SXM estimates, not measurements: gemm_wt_tuned times candidate configurations on the device by
+// default and uses this model only where it cannot measure (stream capture, B200_WT_TUNE=0).
+//   * one CTA per SM (384 threads at 168 registers fill the register file);
+//   * a CTA costs a few us of fixed latency (launch, barrier set-up, first TMA round trip, epilogue)
+//     + per k-block max(MMA time at the data-sheet 989 TFLOP/s spread over 132 SMs, shared-memory
+//     fill time at ~130 GB/s per SM);
+//   * token tiles are at most WT_TN_AUTO = 128 wide: wider tiles need the 16-chunk accumulator
+//     instantiation, which spills;
 //   * split-K buys parallelism for the GEMMs with few weight rows at the price of fp32 partial
 //     traffic (written here, read by finish_rows);
-//   * the weights are streamed from HBM once: nothing is faster than bytes / ~6 TB/s.
+//   * the weights are streamed from HBM once: nothing is faster than bytes / 3.35 TB/s.
 void gemm_wt_auto(int T, int row_blocks, int K, bool allow_split, WtConfig* best, int sm_count) {
   const int kb_total = cdiv(K, WT_BK);
   const int t16 = round16(T);
@@ -683,18 +643,18 @@ void gemm_wt_auto(int T, int row_blocks, int K, bool allow_split, WtConfig* best
   int n_tn = 0;
   auto add_tn = [&](int tn) {
     if (tn < 16) tn = 16;
-    if (tn > 256) tn = 256;
+    if (tn > WT_TN_AUTO) tn = WT_TN_AUTO;
     if (tn > t16) tn = t16;
     for (int i = 0; i < n_tn; ++i)
       if (tn_c[i] == tn) return;
     tn_c[n_tn++] = tn;
   };
   for (int k = 1; k <= 3; ++k) add_tn(round16(cdiv(T, k)));
-  if (T > 256) {
-    const int nt = cdiv(T, 256);
+  if (T > WT_TN_AUTO) {
+    const int nt = cdiv(T, WT_TN_AUTO);
     for (int k = 0; k < 3; ++k) add_tn(round16(cdiv(T, nt + k)));
   }
-  add_tn(96); add_tn(128); add_tn(144); add_tn(192);
+  add_tn(64); add_tn(96); add_tn(112); add_tn(128);
   double best_t = 1e30;
   best->TN = tn_c[0]; best->KS = 1; best->stages = 2; best->split = 1;
   for (int it = 0; it < n_tn; ++it) {
@@ -703,12 +663,10 @@ void gemm_wt_auto(int T, int row_blocks, int K, bool allow_split, WtConfig* best
     const long base = (long)row_blocks * tt;
     for (int KS = 1; KS <= 4; KS *= 2) {
       const int stage = KS * (WT_WBLK + TN * 128);
-      for (int occ = 2; occ >= 1; --occ) {
-        const int budget = occ == 2 ? 110 * 1024 : 208 * 1024;
-        int st = budget / stage;
+      {
+        int st = 208 * 1024 / stage;
         if (st > 8) st = 8;
         if (st < 2 || st * KS < 3 || (long)st * stage < (long)WT_EPI_TOK * WT_ROWS * 4) continue;
-        if (occ == 1 && (long)st * stage + 2048 <= 110 * 1024) continue;  // same as the occ == 2 case
         int cand[6] = {1, 0, 0, 0, 0, 0};
         int n_sp = 1;
         if (allow_split) {
@@ -727,24 +685,18 @@ void gemm_wt_auto(int T, int row_blocks, int K, bool allow_split, WtConfig* best
           if (split > 1 && (long)split * T * row_blocks * 128 * 4 > (40L << 20)) continue;  // partial-tile budget
           const long ctas = base * split;
           const int kbs = cdiv(kb_total, split);
-          const double t_mma = 4.0 * (TN / 2.0) / 1900.0;                          // us per k-block
+          const double t_mma = 2.0 * WT_ROWS * TN * WT_BK / (989e6 / 132);   // us per k-block
           const double t_fill = (WT_WBLK + TN * 128) / 130e3 * (KS == 1 ? 1.15 : 1.0);
           const double t_kb = t_mma > t_fill ? t_mma : t_fill;
           const double t_fix = 5.2;                                  // first wave, prologue hidden by PDL
           const long per_sm = (ctas + sm_count - 1) / sm_count;      // CTAs an SM has to run
-          double t;
-          if (occ == 2) {
-            const long waves = (ctas + 2L * sm_count - 1) / (2L * sm_count);
-            t = t_fix + per_sm * kbs * t_kb + (waves - 1) * 4.0;
-          } else {
-            t = t_fix + kbs * t_kb + (per_sm - 1) * (9.5 + kbs * t_kb);  // serialised waves pay the full CTA latency
-          }
+          double t = t_fix + kbs * t_kb + (per_sm - 1) * (9.5 + kbs * t_kb);  // serialised waves pay the full CTA latency
           if (st * KS < 4) t *= 1.08;
           const double fill_total = (double)ctas * kbs * (WT_WBLK + TN * 128);
           if (t < t_fix + fill_total / 12e6) t = t_fix + fill_total / 12e6;   // chip-wide L2 -> SM fill rate
-          const double hbm = (double)row_blocks * 128 * K * 2 / 6e6 + 3.0;   // weights stream from HBM once
+          const double hbm = (double)row_blocks * 128 * K * 2 / 3.35e6 + 3.0;   // weights stream from HBM once
           if (t < hbm) t = hbm + 0.01 * kbs * t_kb;
-          if (split > 1) t += (double)split * T * row_blocks * 128 * 4 / 6e6 + 0.2 * split;
+          if (split > 1) t += (double)split * T * row_blocks * 128 * 4 / 3.35e6 + 0.2 * split;
           if (t < best_t) {
             best_t = t;
             best->TN = TN; best->KS = KS; best->stages = st; best->split = split;
@@ -802,18 +754,17 @@ int gemm_wt(const void* X, long ldx, const void* W, const void* bias, const void
   int dev = 0;
   B200_CUDA(cudaGetDevice(&dev));
   if (!(set_mask >> (dev & 63) & 1ull)) {
-    B200_CUDA(cudaFuncSetAttribute(gemm_wt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024));
-    B200_CUDA(cudaFuncSetAttribute(gemm_wt_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                   cudaSharedmemCarveoutMaxShared));
-    B200_CUDA(cudaFuncSetAttribute(gemm_wt_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024));
-    B200_CUDA(cudaFuncSetAttribute(gemm_wt_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                   cudaSharedmemCarveoutMaxShared));
+    for (auto* k : {gemm_wt_kernel<false, 8>, gemm_wt_kernel<false, 16>, gemm_wt_kernel<true, 8>,
+                    gemm_wt_kernel<true, 16>}) {
+      B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024));
+      B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    }
     set_mask |= 1ull << (dev & 63);
   }
   const int row_blocks = mode == B200_WT_SWIGLU ? cdiv(inter, 64) : cdiv(N, WT_ROWS);
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3(row_blocks, cdiv(T, cfg.TN), splits);
-  lc.blockDim = dim3(256);
+  lc.blockDim = dim3(WT_THREADS);
   lc.dynamicSmemBytes = smem;
   lc.stream = st;
   cudaLaunchAttribute at[1];
@@ -821,10 +772,11 @@ int gemm_wt(const void* X, long ldx, const void* W, const void* bias, const void
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at;
   lc.numAttrs = g_wt_pdl ? 1 : 0;
-  if (mode == B200_WT_F32 || mode == B200_WT_SPLIT) {
-    B200_CUDA(cudaLaunchKernelEx(&lc, gemm_wt_kernel<true>, tw, tx, p));
+  const bool tower = mode == B200_WT_F32 || mode == B200_WT_SPLIT, wide = cfg.TN > 128;
+  if (tower) {
+    B200_CUDA(cudaLaunchKernelEx(&lc, wide ? gemm_wt_kernel<true, 16> : gemm_wt_kernel<true, 8>, tw, tx, p));
   } else {
-    B200_CUDA(cudaLaunchKernelEx(&lc, gemm_wt_kernel<false>, tw, tx, p));
+    B200_CUDA(cudaLaunchKernelEx(&lc, wide ? gemm_wt_kernel<false, 16> : gemm_wt_kernel<false, 8>, tw, tx, p));
   }
   return B200_OK;
 }
@@ -833,9 +785,9 @@ int gemm_wt(const void* X, long ldx, const void* W, const void* bias, const void
 // Measured configuration choice ("measure, don't guess"): the first call for a problem class
 // (tokens rounded up to 64, N, K, mode) times a short list of candidate configurations on the
 // caller's stream with the call's own operands (CUDA events, one warm-up + two timed launches
-// each) and caches the winner; later calls cost one hash lookup.  Candidates follow what the
-// round-2 sweep showed matters: token tile {96,128,144,192,256}, one CTA per SM with 2 k-blocks
-// per stage vs two CTAs per SM with 1, and split-K to one or two waves.  The list is ordered and
+// each) and caches the winner; later calls cost one hash lookup.  Candidates: token tile
+// {64,96,112,128}, 2 k-blocks per stage with a deep ring vs 1 with a short one, and split-K to one
+// or two waves.  The list is ordered and
 // the first candidate within 3 % of the best wins, so the choice is stable run to run.
 // B200_WT_TUNE=0 uses the cost model (gemm_wt_auto) instead.
 // ---------------------------------------------------------------------------------------------
@@ -918,7 +870,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
     std::vector<WtConfig> cand;
     auto add = [&](int tn, int ks, int budget, int split) {
       if (tn > round16(T)) tn = round16(T);
-      if (tn > 256) tn = 256;
+      if (tn > WT_TN_AUTO) tn = WT_TN_AUTO;
       const int stage = ks * (WT_WBLK + tn * 128);
       int stg = budget / stage;
       if (stg > 6) stg = 6;
@@ -938,8 +890,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
       tns[n_tn++] = round16(T);
       if (T > 48) tns[n_tn++] = round16(cdiv(T, 2));
     } else {
-      for (int tn : {144, 96, 192, 128}) tns[n_tn++] = tn;
-      if (T > 512) tns[n_tn++] = 256;
+      for (int tn : {128, 96, 112, 64}) tns[n_tn++] = tn;
     }
     for (int i = 0; i < n_tn; ++i) {
       const int tn = tns[i];
@@ -954,8 +905,8 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
       // (measured and discarded: restricting the list to <= 110 KB configurations so that the NEXT kernel's prologue
       // can always co-reside under PDL made the C2 prefill 2-5 % slower)
       for (int sp : sps) {
-        add(tn, 2, 208 * 1024, sp);  // one CTA per SM, 256-byte weight-row bursts
-        add(tn, 1, 110 * 1024, sp);  // two CTAs per SM
+        add(tn, 2, 208 * 1024, sp);  // 256-byte weight-row bursts
+        add(tn, 1, 110 * 1024, sp);  // one k-block per stage, shorter ring
       }
     }
     if (cand.empty()) {
@@ -1101,7 +1052,7 @@ int b200_gemm_wt(const void* X, long ldx, const void* W, const void* bias, const
     c.TN = cfg4[0]; c.KS = cfg4[1]; c.stages = cfg4[2]; c.split = cfg4[3];
   } else {
     const int rbs = mode == B200_WT_SWIGLU ? cdiv(inter, 64) : cdiv(N, 128);
-    gemm_wt_auto(T, rbs, K, mode == B200_WT_PARTIAL, &c, 148);
+    gemm_wt_auto(T, rbs, K, mode == B200_WT_PARTIAL, &c, 132);
   }
   return gemm_wt(X, ldx, W, bias, residual, ldr, C, ldc, partial, T, N, K, epilogue, mode, inter, c,
                  flags, (cudaStream_t)stream);
@@ -1117,7 +1068,7 @@ int b200_finish_rows(const float* P, int S, const void* bias, const void* resid,
 int b200_gemm_wt_auto_config(int T, int N, int K, int mode, int inter, int* cfg4_out) {
   WtConfig c;
   const int rbs = mode == B200_WT_SWIGLU ? cdiv(inter, 64) : cdiv(N, 128);
-  gemm_wt_auto(T, rbs, K, mode == B200_WT_PARTIAL, &c, 148);
+  gemm_wt_auto(T, rbs, K, mode == B200_WT_PARTIAL, &c, 132);
   cfg4_out[0] = c.TN; cfg4_out[1] = c.KS; cfg4_out[2] = c.stages; cfg4_out[3] = c.split;
   return B200_OK;
 }

@@ -1,5 +1,5 @@
 // Device pieces shared by the two persistent decode kernels (k_mega: CUDA-core consumers,
-// decode_mega.cu; k_mega_tc: tcgen05 consumers, decode_mega_tc.cu): mbarrier / bulk-copy
+// decode_mega.cu; k_mega_tc: wgmma consumers, decode_mega_tc.cu): mbarrier / bulk-copy
 // wrappers, the software grid barrier, the distributed attention phase and the sampler.
 #pragma once
 #include "common.cuh"
@@ -104,13 +104,10 @@ __device__ __forceinline__ uint32_t bf_bits(float x) {
 __device__ __forceinline__ float ldcg_bf(const bf16* p) {
   return __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const unsigned short*>(p)) << 16);
 }
-// packed fp32 FMA (Blackwell FFMA2): (d0,d1) += (a0,a1) * (b0,b1), two IEEE fp32 FMAs per issue
+// (d0,d1) += (a0,a1) * (b0,b1): two IEEE fp32 FMAs (Hopper has no packed fp32 FMA)
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rc;\n\t"
-      "mov.b64 ra, {%2,%3};\n\tmov.b64 rb, {%4,%5};\n\tmov.b64 rc, {%0,%1};\n\t"
-      "fma.rn.f32x2 rc, ra, rb, rc;\n\tmov.b64 {%0,%1}, rc;\n\t}"
-      : "+f"(d0), "+f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fmaf_rn(a0, b0, d0);
+  d1 = __fmaf_rn(a1, b1, d1);
 }
 __device__ __forceinline__ void cbar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 

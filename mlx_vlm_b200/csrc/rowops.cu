@@ -216,8 +216,7 @@ __global__ void mrope_kv_write_kernel(bf16* __restrict__ qkv, const int* __restr
 // chunk of 8 rotary pairs) computes its 8 cos / sin ONCE and re-uses them for every head of the group, all loads and
 // stores are 16-byte vectors, and V^T goes through a shared-memory tile so that its stores are contiguous along the
 // token axis.  Identical arithmetic, element for element, to the scalar kernel above (which evaluated cosf / sinf per
-// element and wrote V^T with 2-byte stores a row apart: 329 us per layer at T = 4864 on the Llama-7B geometry = 13 % of
-// the batched C3 prefill, profiles/r2_launches_c3_prefill_ncu.txt).  grid (ceil(T / 32), slot groups), 256 threads.
+// element and wrote V^T with 2-byte stores a row apart).  grid (ceil(T / 32), slot groups), 256 threads.
 __global__ void __launch_bounds__(256)
 mrope_kv_write_tiled_kernel(bf16* __restrict__ qkv, const int* __restrict__ pos3, const float* __restrict__ inv_freq,
                             const int* __restrict__ axis_sel, bf16* __restrict__ kc, bf16* __restrict__ vc, int T, int ctx0,
@@ -418,7 +417,7 @@ __global__ void __launch_bounds__(512) embed_merge_kernel(const int* __restrict_
 // ---------------------------------------------------------------------------
 static inline int grid_for(long work, int block) {
   long g = (work + block - 1) / block;
-  if (g > 148L * 16) g = 148L * 16;
+  if (g > 132L * 16) g = 132L * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -467,7 +466,7 @@ int mrope_kv_write(void* qkv, const int* pos3, const float* inv_freq, const int*
   static const bool scalar_only = getenv("B200_MROPE_SCALAR") != nullptr;   // A/B and fallback
   if (!scalar_only && (hd % 16) == 0 && hd <= 128 && (!vt || (t_ld % 8) == 0)) {
     const int slots = n_heads + 2 * n_kv, tiles = (T + 31) / 32;
-    int groups = (4 * 148 + tiles - 1) / tiles;          // about four waves of CTAs
+    int groups = (4 * 132 + tiles - 1) / tiles;          // about four waves of CTAs
     if (groups > slots) groups = slots;
     if (groups < 1) groups = 1;
     const int per = (slots + groups - 1) / groups;
@@ -627,7 +626,7 @@ int embed_merge(const int* ids, int B, int T, const void* table, int hidden, con
                                    T * 4));
   }
   int per_row = (T + 7) / 8;  // >= 8 positions per CTA
-  const int cap_ctas = (2 * 148 + B - 1) / B;
+  const int cap_ctas = (2 * 132 + B - 1) / B;
   if (per_row > cap_ctas) per_row = cap_ctas;
   embed_merge_kernel<<<dim3(per_row, B), 512, (size_t)T * 4, st>>>(ids, B, T, (const bf16*)table, hidden,
                                                    (const bf16*)feats, n_feats, image_token,

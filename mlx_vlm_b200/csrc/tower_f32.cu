@@ -467,7 +467,7 @@ static int attn_f32_launch(const AttnF32P& p, dim3 grid, cudaStream_t st) {
 
 static inline int t_grid(long work, int block) {
   long g = (work + block - 1) / block;
-  if (g > 148L * 16) g = 148L * 16;
+  if (g > 132L * 16) g = 132L * 16;
   return (int)(g < 1 ? 1 : g);
 }
 
@@ -647,6 +647,6 @@ int b200_gemm_wt_f32(const void* X, long ldx, const void* W, long ldw, const voi
   ext.kb_w = kbw; ext.k_w = K_w; ext.ldw = ldw; ext.C32 = C32; ext.res32 = res32; ext.ldc32 = ldc32;
   ext.ldr32 = ldr32; ext.Csplit = (bf16*)Csplit; ext.ld_split = ld_split; ext.n_pad = n_pad;
   return gemm_wt_tuned(X, ldx, W, bias, nullptr, 0, nullptr, 0, nullptr, 0, T, N, n_parts * kbw * 64, epilogue, mode, 0,
-                       false, 148, nullptr, (cudaStream_t)stream, &ext);
+                       false, 132, nullptr, (cudaStream_t)stream, &ext);
 }
 }

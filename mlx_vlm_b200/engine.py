@@ -25,7 +25,7 @@ def _inv_freq(dim: int, base: float) -> np.ndarray:
 class Engine:
     def __init__(self, cfg: N.Qwen2VLConfig, device: torch.device):
         if device.type != "cuda":
-            raise N.B200Error("the b200vlm engine needs a CUDA (sm_100a) device; no CPU fallback")
+            raise N.B200Error("the b200vlm engine needs a CUDA (sm_90a) device; no CPU fallback")
         self.lib = N.lib()
         self.cfg = cfg
         self.device = device
@@ -238,7 +238,7 @@ class Engine:
 
     def set_mega(self, enabled):
         """0/False: one kernel per phase; 1/True: k_mega (CUDA-core consumers); 2: k_mega_tc
-        (tcgen05 consumers); 3: k_mega_tc with a full 16-row activation operand; 4: k_mega in
+        (wgmma consumers); 3: k_mega_tc with a full 16-row activation operand; 4: k_mega in
         dataflow mode (polled self-validating activation words instead of 3 of the 5 barriers)."""
         N.check(self.lib.b200_engine_set_mega(self.h, int(enabled)), "set_mega")
 

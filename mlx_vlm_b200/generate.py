@@ -104,7 +104,7 @@ def generate_step(
     """Yields (token id, logprobs (vocab,) bf16 device tensor) like ar.py:151-515."""
     for k in _UNSUPPORTED:
         if kwargs.pop(k, None) is not None:
-            raise NotImplementedError(f"generate_step: `{k}` is outside the B200 hot-path scope")
+            raise NotImplementedError(f"generate_step: `{k}` is outside this engine's hot-path scope")
     for k in ("kv_group_size", "kv_quant_scheme", "quantized_kv_start", "kv_key_scheme",
               "kv_value_scheme", "draft_kind", "draft_block_size", "prompt_cache_checkpoint",
               "prompt_cache_checkpoint_len", "thinking_budget_criteria"):
@@ -221,7 +221,7 @@ def stream_generate(model, processor, prompt: str, image: Union[str, List[str], 
     """generate/dispatch.py:694-1105 (vision/text requests; audio/video out of scope)."""
     from .utils import StoppingCriteria, prepare_inputs
     if audio is not None or video is not None:
-        raise NotImplementedError("audio / video inputs are outside the B200 hot-path scope")
+        raise NotImplementedError("audio / video inputs are outside this engine's hot-path scope")
     tokenizer = processor.tokenizer if hasattr(processor, "tokenizer") else processor
     skip_special_token_ids = (set(getattr(tokenizer, "all_special_ids", []))
                               if kwargs.pop("skip_special_tokens", False) else set())

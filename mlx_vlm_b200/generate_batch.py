@@ -3,10 +3,10 @@
 `BatchGenerationResult` :519-545, `_left_pad_prompts` / `_right_pad_prompts` :548-560,
 `batch_generate` :2890-3097).
 
-How the rows run on the B200 engine: LOCK STEP on the device (csrc/decode_batch.cu).  All active
+How the rows run on the CUDA engine: LOCK STEP on the device (csrc/decode_batch.cu).  All active
 rows live in ONE batched KV pool (layers, 2, rows, kv heads, capacity, head_dim), each with its own
 length (no left padding); a decode step is one captured CUDA graph that streams the weights ONCE
-for all rows (weight-major tcgen05 GEMMs with the rows as a 16-wide token tile), so B rows cost
+for all rows (weight-major wgmma GEMMs with the rows as a 16-wide token tile), so B rows cost
 about one batch-1 step.  Admission of a request = a batch-1 prefill straight into a free row of
 the pool; a finished row is replaced by the last row (one row copy); the device state is re-armed
 only when the set of rows changes.  Tokens are produced in slices of `decode_slice` steps and
@@ -175,7 +175,7 @@ class BatchGenerator:
                  decode_slice: int = 16, batched_prefill: bool = True, **unsupported):
         for k in ("kv_bits", "kv_key_bits", "kv_value_bits", "draft_model", "apc_manager", "prompt_cache"):
             if unsupported.pop(k, None) is not None:
-                raise NotImplementedError(f"BatchGenerator: `{k}` is outside the B200 hot-path scope")
+                raise NotImplementedError(f"BatchGenerator: `{k}` is outside this engine's hot-path scope")
         if logits_processors:
             raise NotImplementedError("BatchGenerator: logits processors run on the single-request path only")
         if top_logprobs_k:

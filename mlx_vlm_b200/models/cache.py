@@ -1,7 +1,7 @@
 """KV cache objects with the reference's Python-visible behaviour
 (mlx_vlm/models/cache.py:337-439 `KVCache`, :45-70 `make_prompt_cache`).
 
-Storage is B200-first: ONE device pool per request (`KVPool`, laid out
+Storage is device-first: ONE device pool per request (`KVPool`, laid out
 (n_layers, 2, batch, n_kv_heads, capacity, head_dim) bf16) that the CUDA engine
 writes directly (K is rotated and appended inside the QKV kernels), instead of
 per-layer arrays grown by concatenation.  Each layer's `KVCache` is a view of the
@@ -202,7 +202,7 @@ class BatchKVCache(_BaseCache):
     row b are dead, `offset[b] = _idx - left_padding[b]` is the row's real length.
 
     Host-side container with the reference's observable behaviour (merge / extract / filter /
-    extend / trim / state); the B200 engine decodes each row from its own `KVCache` pool
+    extend / trim / state); the CUDA engine decodes each row from its own `KVCache` pool
     (`generate_batch.BatchGenerator`), this class is the interchange format."""
     step = 256
 

@@ -1,4 +1,4 @@
-"""Idefics3 (and, through models/smolvlm, SmolVLM) on the B200 engine: tower + pixel-shuffle connector + Llama LM."""
+"""Idefics3 (and, through models/smolvlm, SmolVLM) on the CUDA engine: tower + pixel-shuffle connector + Llama LM."""
 from .idefics3 import Connector, Model
 from .vision import VisionModel, position_ids
 from .language import LanguageModel

@@ -130,7 +130,7 @@ class Model:
         B = x.shape[0]
         _, _, states = self.vision_tower(x, output_hidden_states=True, feature_layer=self.vision_feature_layer)
         if not isinstance(self.vision_feature_layer, int):
-            raise NotImplementedError("a list of vision feature layers is outside the B200 hot-path scope")
+            raise NotImplementedError("a list of vision feature layers is outside this engine's hot-path scope")
         sel = states[self.vision_feature_layer]
         P = (x.shape[1] // v.patch_size) * (x.shape[2] // v.patch_size)
         L = P + 1

@@ -1,6 +1,6 @@
 """Chat-template helpers of the reference's public surface (mlx_vlm/prompt_utils.py:
 `get_message_json` :555-591, `get_chat_template` :594-826, `apply_chat_template` :829-995) for the
-model families on the B200 generate path — qwen2_vl, llava, llava_next, idefics2 ("list with image"
+model families on the CUDA generate path — qwen2_vl, llava, llava_next, idefics2 ("list with image"
 messages, prompt_utils.py:37,45,77,78) and qwen2_5_vl / idefics3 / smolvlm ("list with image first", :46,38,76) — plus the reference's text-only fallback for unknown types.
 Behaviour is pinned against the reference's own module, executed, in tests/golden
 (`chat_template_cases`).  Video / audio message kinds are outside the hot-path scope.
@@ -75,7 +75,7 @@ def get_message_json(model_name: str, prompt: str, role: str = "user", skip_imag
     if num_images > 1 and name in _SINGLE_IMAGE_ONLY:
         raise ValueError(f"Model {name} does not support multi-image chat. Please only use 1 image.")
     if kwargs.get("video"):
-        raise NotImplementedError("video messages are outside the B200 hot-path scope")
+        raise NotImplementedError("video messages are outside this engine's hot-path scope")
     entries: List[Dict[str, Any]] = [{"type": "text", "text": prompt, "content": prompt}]
     if role == "user" and not skip_image_token and num_images > 0:
         images = [{"type": "image"}] * num_images

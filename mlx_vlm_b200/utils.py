@@ -3,7 +3,7 @@
 `prepare_inputs` :1918-2136, `load_image`/`process_image` :1503-1567,
 `StoppingCriteria` :2191-2249).
 
-B200-first differences: safetensors shards are memory-mapped on the host and every tensor is
+Device-first differences: safetensors shards are memory-mapped on the host and every tensor is
 packed (q/k/v and gate/up fused, conv layout fixed) straight into ONE device arena
 (`Model.packed_weights`, bf16) — which is also what a multi-GPU start-up broadcasts with a single
 NCCL call; inputs are moved to the device with one pinned-memory H2D copy per tensor on the
@@ -30,7 +30,7 @@ def get_model_and_args(config: dict):
     try:
         arch = importlib.import_module(f"mlx_vlm_b200.models.{model_type}")
     except ImportError as e:
-        raise ValueError(f"Model type {model_type} not supported by the B200 engine yet.") from e
+        raise ValueError(f"Model type {model_type} not supported by the CUDA engine yet.") from e
     return arch, model_type
 
 
@@ -90,7 +90,7 @@ def load(path_or_hf_repo: str, adapter_path: Optional[str] = None, lazy: bool = 
     pseudo-path `synthetic:qwen2-vl-2b` / `synthetic:qwen2-vl-7b` builds a seeded
     random-init model with a SyntheticProcessor (benchmarks, no checkpoint)."""
     if adapter_path is not None:
-        raise NotImplementedError("adapters (LoRA) are outside the B200 hot-path scope")
+        raise NotImplementedError("adapters (LoRA) are outside this engine's hot-path scope")
     if revision is not None:
         raise NotImplementedError("`revision` needs the hub; only local model directories are supported")
     if path_or_hf_repo.startswith("synthetic:"):
@@ -156,7 +156,7 @@ def prepare_inputs(processor, images=None, audio=None, prompts=None, image_token
     attention_mask as host numpy (the rope-index / merge bookkeeping is host logic,
     like the reference's `.tolist()`), pixel_values as a device fp32 tensor."""
     if audio is not None:
-        raise NotImplementedError("audio inputs are outside the B200 hot-path scope")
+        raise NotImplementedError("audio inputs are outside this engine's hot-path scope")
     if images is not None and not isinstance(images, (list, tuple)):
         images = [images]
     if images is not None:

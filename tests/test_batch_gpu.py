@@ -1,7 +1,7 @@
 """Lock-step batched decode on the GPU (csrc/decode_batch.cu; SURVEY §8 a15, config C5): rows that
 share one weight stream must produce what each request produces alone.
 
-The batch-1 path (persistent k_mega) and the batched path (weight-major tcgen05 GEMMs + bd_attn)
+The batch-1 path (persistent k_mega) and the batched path (weight-major wgmma GEMMs + bd_attn)
 are different kernels: both are within the per-op bar of the oracle, so a row's tokens are required
 to be equal until the first near-tie (the batched token's logprob on the batch-1 path within two
 bf16 ulps of the maximum), exactly like the oracle comparisons of test_engine_gpu.py."""

@@ -1,4 +1,4 @@
-"""The config classes of every model family on the B200 path are generated from tables (models/config_schema.py); this pins
+"""The config classes of every model family on the CUDA path are generated from tables (models/config_schema.py); this pins
 them field by field — names, order, defaults — against the reference's dataclasses as recorded with `ast` by
 tests/golden/make_config_golden.py, and checks the behaviour attached to them."""
 import dataclasses

@@ -226,7 +226,7 @@ def test_multi_kernel_decode_equals_megakernel():
 
 @pytest.mark.parametrize("kind,mode", [("tiny", 2), ("wide2", 2), ("wide2", 3), ("tiny", 4), ("wide2", 4)])
 def test_tensor_core_megakernel_parity(kind, mode):
-    """Alternative decode-step kernels — k_mega_tc (modes 2/3; decode_mega_tc.cu: tcgen05 GEMV
+    """Alternative decode-step kernels — k_mega_tc (modes 2/3; decode_mega_tc.cu: wgmma GEMV
     phases on pre-packed weight tile images, exact fixed-point split-K accumulation) and k_mega
     in dataflow mode (mode 4: polled self-validating activation words) — against the oracle, teacher-forced, and against
     k_mega on the same cache; the appended K/V rows of layer 0 must be bit-identical (same
@@ -352,7 +352,7 @@ def test_two_images_of_different_size_in_one_prompt(sizes):
 
 
 def test_geometry_that_does_not_fit_the_persistent_kernel_falls_back_per_phase():
-    """32 kv heads x 8 key ranges > 148 SMs: k_mega cannot hold the step; the engine must run the
+    """32 kv heads x 8 key ranges > 132 SMs: k_mega cannot hold the step; the engine must run the
     same step as per-phase kernels (still the CUDA path) and stay in parity with the oracle."""
     from mlx_vlm_b200.models.cache import make_prompt_cache
     from oracle import qwen2vl as O
