@@ -180,6 +180,33 @@ int b200_engine_set_workspace(b200_engine* e, void* ptr, long bytes);
 /* KV pool laid out (n_layers, 2, batch, n_kv, cap, head_dim) bf16 — per layer the
  * reference KVCache layout (B, n_kv_heads, S, head_dim), cache.py:345-367. */
 int b200_engine_bind_kv(b200_engine* e, void* pool, int batch, int cap);
+/* 8-bit KV pool (kv_bits=8; format in csrc/kvq.cuh): codes (n_layers, 2, batch, n_kv, cap, head_dim) uint8,
+ * scales and biases (n_layers, 2, batch, n_kv, cap, head_dim / group_size) bf16, group_size 32 | 64 | 128.
+ * Replaces the bf16 binding: decode steps quantize the new K/V row, append it and attend over the dequantized
+ * cache with the per-phase kernels (the persistent k_mega kernels read bf16 pools only).  Prefill calls need a
+ * bf16 pool (b200_engine_bind_kv) again. */
+int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases, int batch, int cap,
+                         int group_size);
+/* Prefill over an 8-bit cache: with the bf16 pool bound (its rows [0, ctx0) holding the dequantized prefix),
+ * every prefill layer quantizes the chunk's new K/V rows into this 8-bit pool (same batch and capacity as the
+ * bf16 one) and replaces them in the bf16 pool by their dequantized values before attending, so the chunk
+ * attends to its prefix and to itself in quantized form.  codes == NULL switches the write-through off;
+ * binding a pool switches it off too. */
+int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size);
+/* One 8-bit decode attention step (the kernel of the per-phase decode step) on caller buffers, synchronous:
+ * qbuf (n_heads, head_dim) bf16; K / V planes of one row and layer (n_kv, cap, ...); stage_k / stage_v bf16
+ * (n_kv, cap, head_dim) holding the new row at position ctx; out (n_heads, head_dim) bf16. */
+int b200_kvq_decode_attention(const void* qbuf, void* k_codes, void* k_scales, void* k_biases, void* v_codes,
+                              void* v_scales, void* v_biases, const void* stage_k, const void* stage_v, void* out,
+                              int n_heads, int n_kv, int head_dim, int cap, int ctx, int group_size, int cluster,
+                              void* stream);
+/* Bulk conversion between a bf16 pool and an 8-bit pool: the first n_tokens positions of `planes` planes
+ * (plane = one (layer, k/v, row, kv head) of cap positions x head_dim elements), each side with its own
+ * capacity.  Stream-ordered. */
+int b200_kvq_quantize(const void* src, int src_cap, void* codes, void* scales, void* biases, int dst_cap,
+                      long planes, int n_tokens, int head_dim, int group_size, void* stream);
+int b200_kvq_dequantize(const void* codes, const void* scales, const void* biases, int src_cap, void* dst,
+                        int dst_cap, long planes, int n_tokens, int head_dim, int group_size, void* stream);
 /* rotary inverse-frequency tables, HOST fp32: lm (head_dim/2) =
  * compute_inv_freq (rope_utils.py:1042-1044), vision (v_head_dim/4) =
  * VisionRotaryEmbedding (vision.py:53-65).  Either may be NULL (keep default).

@@ -100,6 +100,11 @@ SIGNATURES = {
     "b200_batch_logprobs": (_P, [_P]),
     "b200_batch_token_log": (_P, [_P]),
     "b200_kv_copy_row": (_I, [_P, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_engine_bind_kvq": (_I, [_P, _P, _P, _P, _I, _I, _I]),
+    "b200_engine_set_prefill_kvq": (_I, [_P, _P, _P, _P, _I]),
+    "b200_kvq_decode_attention": (_I, [_P] * 10 + [_I] * 7 + [_P]),
+    "b200_kvq_quantize": (_I, [_P, _I, _P, _P, _P, _I, _L, _I, _I, _I, _P]),
+    "b200_kvq_dequantize": (_I, [_P, _P, _P, _I, _P, _I, _L, _I, _I, _I, _P]),
     "b200_memcpy_d2d": (_I, [_P, _P, _L, _P]),
     "b200_memcpy_h2d": (_I, [_P, _P, _L, _P]),
     "b200_engine_last_decode_ms": (_F, [_P]),

@@ -10,6 +10,7 @@
 
 #include "common.cuh"
 #include "decode.cuh"
+#include "kvq.cuh"
 
 namespace b200 {
 
@@ -53,6 +54,12 @@ struct b200_engine {
   bf16* kv = nullptr;
   int kv_batch = 0, kv_cap = 0;
   int kv_row = 0;        // row of the pool that prefill / single-row decode read and write
+  // 8-bit pool (b200_engine_bind_kvq; replaces `kv` while bound) and the engine-owned bf16 staging planes
+  // [2][n_kv][cap][hd] where the decode QKV kernel leaves the new K/V row before it is quantized
+  KvqPlanes q8 = {};
+  KvqPlanes pre_q8 = {};  // b200_engine_set_prefill_kvq: prefill writes its rows through to this 8-bit pool
+  bf16* q8_stage = nullptr;
+  long q8_stage_elems = 0;
   void* batch = nullptr; // lock-step batched decoder (decode_batch.cu)
   std::vector<int> b_ctx, b_active;  // host mirrors of the batched rows' lengths
   // engine-owned small device buffers
@@ -139,6 +146,14 @@ struct b200_engine {
   bf16* vptr(int layer, int row) const {
     return kv + (((long)layer * 2 + 1) * kv_batch + row) * cfg.n_kv_heads * (long)kv_cap * cfg.head_dim;
   }
+  KvqPlanes q8_plane(int layer, int side, int row, const KvqPlanes& pool) const {
+    const long plane = (((long)layer * 2 + side) * kv_batch + row) * cfg.n_kv_heads;
+    KvqPlanes p = pool;
+    p.codes += plane * kv_cap * cfg.head_dim;
+    p.scales += plane * kv_cap * (cfg.head_dim / pool.gs);
+    p.biases += plane * kv_cap * (cfg.head_dim / pool.gs);
+    return p;
+  }
 };
 
 static const bf16* need(b200_engine* e, const std::string& name, long n_expected, bool* ok) {
@@ -221,6 +236,7 @@ static void invalidate_graph(b200_engine* e) {
 static int mega_prepare(b200_engine* e, cudaStream_t s) {
   const auto& c = e->cfg;
   B200_REQUIRE(c.n_layers <= MEGA_MAX_LAYERS, "mega: %d layers > %d", c.n_layers, MEGA_MAX_LAYERS);
+  B200_REQUIRE(!e->q8.codes, "mega: the persistent kernels read a bf16 KV pool; an 8-bit pool runs the per-phase kernels");
   if (!e->bar) {
     B200_CUDA(cudaMalloc(&e->bar, sizeof(unsigned long long)));
     B200_CUDA(cudaMemset(e->bar, 0, sizeof(unsigned long long)));
@@ -333,6 +349,20 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
   int rc;
   if (e->active_mega() == 2) return mega_tc_launch(e->tp, e->sm_count, s);
   if (e->active_mega()) return mega_launch(e->mp, e->sm_count, s);
+  if (e->q8.codes) {
+    bf16* sk = e->q8_stage;
+    bf16* sv = sk + (long)c.n_kv_heads * e->kv_cap * c.head_dim;
+    for (int l = 0; l < c.n_layers; ++l) {
+      const LayerW& lw = e->layers[l];
+      if ((rc = launch_qkv(d, lw, e->h, e->qbuf, sk, sv, e->st, e->lm_inv_freq, s))) return rc;
+      if ((rc = launch_attn_q8(d, e->qbuf, e->q8_plane(l, 0, e->kv_row, e->q8), e->q8_plane(l, 1, e->kv_row, e->q8), sk, sv,
+                               e->attn, e->st, e->attn_cluster, s)))
+        return rc;
+      if ((rc = launch_res(lw.wo, e->attn, e->h, c.hidden, c.n_heads * c.head_dim, s))) return rc;
+      if ((rc = launch_gateup(d, lw, e->h, e->act, s))) return rc;
+      if ((rc = launch_res(lw.wd, e->act, e->h, c.hidden, c.inter, s))) return rc;
+    }
+  } else {
   for (int l = 0; l < c.n_layers; ++l) {
     const LayerW& lw = e->layers[l];
     bf16* kc = e->kptr(l, e->kv_row);
@@ -342,6 +372,7 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
     if ((rc = launch_res(lw.wo, e->attn, e->h, c.hidden, c.n_heads * c.head_dim, s))) return rc;
     if ((rc = launch_gateup(d, lw, e->h, e->act, s))) return rc;
     if ((rc = launch_res(lw.wd, e->act, e->h, c.hidden, c.inter, s))) return rc;
+  }
   }
   if ((rc = launch_head(d, e->norm, e->head, e->h, e->logits, e->partials, s))) return rc;
   if ((rc = launch_sample(d, e->logits, e->partials, e->logprobs, e->embed, e->h, e->st,
@@ -657,7 +688,7 @@ static int prefill_layers_v2(b200_engine* e, const void* embeds, const int* pos3
   e->kvref_host->cap = e->kv_cap;
   B200_CUDA(cudaMemcpyAsync(e->kvref, e->kvref_host, sizeof(KvRef), cudaMemcpyHostToDevice, s));
   B200_CUDA(cudaEventRecord(e->kvref_ev, s));
-  if (all_logits_out || ctx0 != 0)  // all-row logits into a caller buffer / a later chunk: plain launches
+  if (all_logits_out || ctx0 != 0 || e->pre_q8.codes)  // all-row logits / a later chunk / 8-bit write-through: plain launches
     return prefill_layers_v2_body(e, pos_stage, T, ctx0, all_logits_out, s);
   const std::vector<long> key = {(long)(uintptr_t)e->ws, (long)e->ws_bytes, (long)T};
   return seq_run(e, e->pre_graphs, key, s, [&]() { return prefill_layers_v2_body(e, pos_stage, T, 0, nullptr, s); });
@@ -698,7 +729,7 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
     // the pipelined kernel needs V^T of EVERY key: available for a fresh prompt (ctx0 == 0).  It then
     // reads the chunk's own rotated K copy and V^T from the workspace, and the cache is addressed through
     // e->kvref: nothing about the KV pool is baked into the captured graph.
-    const bool fa = ctx0 == 0 && attention_fa_supported(qkv, QKV, hd, kws, hd, (long)T * hd, vt, (long)hd * t_ld,
+    const bool fa = ctx0 == 0 && !e->pre_q8.codes && attention_fa_supported(qkv, QKV, hd, kws, hd, (long)T * hd, vt, (long)hd * t_ld,
                                                         t_ld, att, QH, hd);
     if (segs) {
       B200_REQUIRE(fa, "prefill_batch: the pipelined attention kernel does not support this geometry");
@@ -718,6 +749,14 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
                              c.n_kv_heads, hd, s, fa ? scale_bf : 0.f, fa ? vt : nullptr, t_ld,
                              fa ? e->kvref : nullptr, l, fa ? kws : nullptr)))
       return rc;
+    if (e->pre_q8.codes) {  // an 8-bit cache: the chunk's rows are quantized before they are attended
+      if ((rc = kvq_quantize_rows(kc, e->kv_cap, e->q8_plane(l, 0, e->kv_row, e->pre_q8), c.n_kv_heads, ctx0, T, hd,
+                                  true, s)) ||
+          (rc = kvq_quantize_rows(vc, e->kv_cap, e->q8_plane(l, 1, e->kv_row, e->pre_q8), c.n_kv_heads, ctx0, T, hd,
+                                  true, s)))
+        return rc;
+      e->launches += 2;
+    }
     if (fa) {
       rc = attention_fa(qkv, QKV, hd, kws, hd, (long)T * hd, vt, (long)hd * t_ld, t_ld, att, QH, c.n_heads,
                         c.n_kv_heads, hd, T, S, 1, s, 0, T, 0, S);
@@ -860,6 +899,7 @@ int b200_engine_destroy(b200_engine* e) {
   if (e->packed) cudaFree(e->packed);
   if (e->tc_acc) cudaFree(e->tc_acc);
   if (e->flow_words) cudaFree(e->flow_words);
+  if (e->q8_stage) cudaFree(e->q8_stage);
   if (e->batch) batch_decoder_destroy(e->batch);
   if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
   if (e->ev0) cudaEventDestroy(e->ev0);
@@ -926,10 +966,56 @@ int b200_engine_set_workspace(b200_engine* e, void* ptr, long bytes) {
 int b200_engine_bind_kv(b200_engine* e, void* pool, int batch, int cap) {
   B200_REQUIRE(e && pool && batch >= 1 && cap >= 1 && ((uintptr_t)pool & 15) == 0,
                "bind_kv: bad arguments");
-  if (pool != e->kv || batch != e->kv_batch || cap != e->kv_cap) invalidate_graph(e);
+  if (pool != e->kv || batch != e->kv_batch || cap != e->kv_cap || e->q8.codes) invalidate_graph(e);
+  if (e->q8_stage) {  // the 8-bit decode staging planes are not needed while a bf16 pool is bound
+    B200_CUDA(cudaFree(e->q8_stage));
+    e->q8_stage = nullptr;
+    e->q8_stage_elems = 0;
+  }
   e->kv = (bf16*)pool;
   e->kv_batch = batch;
   e->kv_cap = cap;
+  e->q8 = KvqPlanes{};
+  e->pre_q8 = KvqPlanes{};
+  return B200_OK;
+}
+
+int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size) {
+  B200_REQUIRE(e, "set_prefill_kvq: null engine");
+  if (!codes) {
+    e->pre_q8 = KvqPlanes{};
+    return B200_OK;
+  }
+  B200_REQUIRE(e->kv && scales && biases && e->v2, "set_prefill_kvq: bind the bf16 pool first / round-1 prefill selected");
+  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && e->cfg.head_dim % group_size == 0,
+               "set_prefill_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size,
+               e->cfg.head_dim);
+  e->pre_q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
+  return B200_OK;
+}
+
+int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases, int batch, int cap,
+                         int group_size) {
+  B200_REQUIRE(e && codes && scales && biases && batch >= 1 && cap >= 1 && ((uintptr_t)codes & 15) == 0,
+               "bind_kvq: bad arguments");
+  const auto& c = e->cfg;
+  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && c.head_dim % group_size == 0,
+               "bind_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size, c.head_dim);
+  B200_REQUIRE(e->kv_row < batch, "bind_kvq: bound row %d of %d", e->kv_row, batch);
+  const long stage = 2L * c.n_kv_heads * cap * c.head_dim;
+  if (stage > e->q8_stage_elems) {
+    if (e->q8_stage) B200_CUDA(cudaFree(e->q8_stage));
+    e->q8_stage = nullptr;
+    e->q8_stage_elems = 0;
+    B200_CUDA(cudaMalloc(&e->q8_stage, (size_t)stage * sizeof(bf16)));
+    e->q8_stage_elems = stage;
+  }
+  if (codes != e->q8.codes || batch != e->kv_batch || cap != e->kv_cap || group_size != e->q8.gs)
+    invalidate_graph(e);
+  e->kv = nullptr;
+  e->kv_batch = batch;
+  e->kv_cap = cap;
+  e->q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
   return B200_OK;
 }
 
@@ -1122,6 +1208,7 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   int rc = resolve(e);
   if (rc) return rc;
   B200_REQUIRE(e->kv && e->v2, "engine_prefill_batch: KV pool not bound / round-1 prefill kernels selected");
+  B200_REQUIRE(!e->pre_q8.codes, "engine_prefill_batch: no 8-bit write-through in the batched prefill");
   long T = 0;
   std::vector<PreSeg> segs(n_seq);
   for (int g = 0; g < n_seq; ++g) {
@@ -1194,7 +1281,7 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   B200_REQUIRE(e && n_steps > 0, "engine_decode: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv, "engine_decode: KV pool not bound");
+  B200_REQUIRE(e->kv || e->q8.codes, "engine_decode: KV pool not bound");
   B200_REQUIRE(e->ctx_host + n_steps <= e->kv_cap,
                "engine_decode: %d cached + %d steps exceeds cache capacity %d", e->ctx_host,
                n_steps, e->kv_cap);
@@ -1225,6 +1312,8 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
       e->mega_fits = false;
     }
   }
+  if (e->q8.codes && !(e->use_graph && e->gexec))
+    if ((rc = kvq_decode_prepare(e->dims(), e->attn_cluster))) return rc;
   if (e->use_graph && !e->gexec) {
     // capture one step on the engine's own stream (capture does not execute)
     cudaGraph_t graph = nullptr;

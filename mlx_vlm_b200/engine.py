@@ -98,6 +98,25 @@ class Engine:
             self._bound = key
             self._bound_buf = pool.buf
 
+    def bind_kvq(self, pool):
+        """bind an 8-bit pool (models/cache.py QuantizedKVPool) in place of the bf16 one: decode steps then run
+        the per-phase kernels with the 8-bit attention (csrc/kvq.cu)"""
+        key = ("q8", pool.codes.data_ptr(), pool.batch, pool.capacity, pool.group_size)
+        if key != self._bound:
+            N.check(self.lib.b200_engine_bind_kvq(self.h, pool.codes.data_ptr(), pool.scales.data_ptr(),
+                                                  pool.biases.data_ptr(), pool.batch, pool.capacity,
+                                                  pool.group_size), "bind_kvq")
+            self._bound = key
+            self._bound_buf = (pool.codes, pool.scales, pool.biases)
+
+    def set_prefill_kvq(self, pool):
+        """prefill calls write their K/V rows through to this 8-bit pool (None: off); see b200_engine_set_prefill_kvq"""
+        if pool is None:
+            N.check(self.lib.b200_engine_set_prefill_kvq(self.h, None, None, None, 0), "set_prefill_kvq")
+            return
+        N.check(self.lib.b200_engine_set_prefill_kvq(self.h, pool.codes.data_ptr(), pool.scales.data_ptr(),
+                                                     pool.biases.data_ptr(), pool.group_size), "set_prefill_kvq")
+
     # -- calls ---------------------------------------------------------------
     def vision(self, pixel_values: torch.Tensor, grid_thw: np.ndarray) -> torch.Tensor:
         grid = np.ascontiguousarray(np.asarray(grid_thw, dtype=np.int32).reshape(-1, 3))

@@ -30,6 +30,8 @@ DEFAULT_TOP_N_SIGMA = 0.0
 DEFAULT_REPETITION_CONTEXT_SIZE = 20
 DEFAULT_PREFILL_STEP_SIZE = 2048
 DEFAULT_SEED = 0
+DEFAULT_KV_GROUP_SIZE = 64
+DEFAULT_QUANTIZED_KV_START = 5000
 
 
 @dataclass
@@ -68,7 +70,43 @@ class PromptCacheState:
         self.cache = kv_cache
 
 
-_UNSUPPORTED = ("max_kv_size", "kv_bits", "kv_key_bits", "kv_value_bits", "draft_model")
+_UNSUPPORTED = ("max_kv_size", "kv_key_bits", "kv_value_bits", "draft_model")
+
+
+def kv_quant_args(kv_bits, kv_group_size, kv_quant_scheme, head_dim: int):
+    """Validate the KV-quantization kwargs: returns the bit width (None: bf16 cache).  Only the uniform 8-bit
+    scheme is built; other widths and schemes raise NotImplementedError, a bad group size ValueError."""
+    if kv_bits is None:
+        return None
+    if kv_bits != 8:
+        raise NotImplementedError(f"kv_bits={kv_bits}: only the uniform 8-bit KV cache is built")
+    if kv_quant_scheme not in (None, "uniform"):
+        raise NotImplementedError(f"kv_quant_scheme={kv_quant_scheme!r}: only the uniform scheme is built")
+    if kv_group_size not in (32, 64, 128) or head_dim % kv_group_size:
+        raise ValueError(f"kv_group_size={kv_group_size}: must be 32, 64 or 128 and divide head_dim={head_dim}")
+    return 8
+
+
+def maybe_quantize_kv_cache(prompt_cache, quantized_kv_start, kv_group_size, kv_bits,
+                            kv_quant_scheme: str = "uniform", kv_key_bits=None, kv_value_bits=None,
+                            kv_key_scheme=None, kv_value_scheme=None):
+    """generate/common.py:77-183, uniform branch: every layer whose offset reached `quantized_kv_start` is
+    replaced by its 8-bit form.  The layers of a request share one pool: once all of them are converted the
+    bf16 pool is released (the replaced bf16 views are empty afterwards)."""
+    if kv_bits is None:
+        return
+    if kv_key_bits is not None or kv_value_bits is not None or kv_key_scheme is not None or \
+            kv_value_scheme is not None:
+        raise NotImplementedError("per-side KV quantization (kv_key_bits / kv_value_bits / schemes) is not built")
+    pools = set()
+    for index, layer_cache in enumerate(prompt_cache):
+        if hasattr(layer_cache, "to_quantized") and layer_cache.offset >= quantized_kv_start:
+            prompt_cache[index] = layer_cache.to_quantized(group_size=kv_group_size, bits=int(kv_bits))
+            pools.add(layer_cache._pool)
+    for pool in pools:
+        if pool is not None and not any(getattr(c, "_pool", None) is pool for c in prompt_cache):
+            pool.buf = None
+            pool.__dict__.pop("_q8", None)
 
 
 def generate_step(
@@ -105,8 +143,13 @@ def generate_step(
     for k in _UNSUPPORTED:
         if kwargs.pop(k, None) is not None:
             raise NotImplementedError(f"generate_step: `{k}` is outside this engine's hot-path scope")
-    for k in ("kv_group_size", "kv_quant_scheme", "quantized_kv_start", "kv_key_scheme",
-              "kv_value_scheme", "draft_kind", "draft_block_size", "prompt_cache_checkpoint",
+    kv_bits = kwargs.pop("kv_bits", None)
+    kv_group_size = kwargs.pop("kv_group_size", DEFAULT_KV_GROUP_SIZE)
+    kv_quant_scheme = kwargs.pop("kv_quant_scheme", None)
+    quantized_kv_start = kwargs.pop("quantized_kv_start", DEFAULT_QUANTIZED_KV_START)
+    if kv_bits is not None:
+        kv_bits = kv_quant_args(kv_bits, kv_group_size, kv_quant_scheme, model.language_model.head_dim)
+    for k in ("kv_key_scheme", "kv_value_scheme", "draft_kind", "draft_block_size", "prompt_cache_checkpoint",
               "prompt_cache_checkpoint_len", "thinking_budget_criteria"):
         kwargs.pop(k, None)
     if seed is not None:
@@ -140,21 +183,28 @@ def generate_step(
     if getattr(lm, "supports_logits_to_keep", False):
         step_kwargs["logits_to_keep"] = 1
 
+    def quantize_policy():
+        # ar.py:366,457: after every forward
+        maybe_quantize_kv_cache(prompt_cache, quantized_kv_start, kv_group_size, kv_bits)
+
     # ---- prefill (chunked above prefill_step_size, ar.py:426-472) ----
     if prefill_step_size is not None and T > prefill_step_size:
         while inputs_embeds.shape[1] > 1:
             n = min(prefill_step_size, inputs_embeds.shape[1] - 1)
             lm(ids_host[:, :n], inputs_embeds=inputs_embeds[:, :n], cache=prompt_cache,
                n_to_process=n, reserve_tokens=reserve, **step_kwargs)
+            quantize_policy()
             inputs_embeds = inputs_embeds[:, n:]
             ids_host = ids_host[:, n:]
         ids_host = ids_host[:, -1:]
     outputs = lm(ids_host, inputs_embeds=inputs_embeds, cache=prompt_cache,
                  reserve_tokens=reserve, **step_kwargs)
+    quantize_policy()
 
     fast = sampler_is_greedy and not processors
     if fast:
-        yield from _greedy_device_loop(eng, lm, prompt_cache, max_tokens, reserve, return_logprobs)
+        yield from _greedy_device_loop(eng, lm, prompt_cache, max_tokens, reserve, return_logprobs,
+                                       quantize_policy if kv_bits is not None else None)
         return
 
     # ---- general path: torch samplers / logits processors on the ENGINE's stream ----
@@ -187,11 +237,13 @@ def generate_step(
         if processors:
             tokens.append(tok)
         outputs = lm(np.asarray([[tok]]), cache=prompt_cache, reserve_tokens=reserve)
+        quantize_policy()
         logits = outputs.logits[:, -1, :]
 
 
-def _greedy_device_loop(eng, lm, prompt_cache, max_tokens, reserve, return_logprobs):
-    """Decode loop with device-resident token feedback, one step ahead of the host."""
+def _greedy_device_loop(eng, lm, prompt_cache, max_tokens, reserve, return_logprobs, after_step=None):
+    """Decode loop with device-resident token feedback, one step ahead of the host.  `after_step` runs after
+    every enqueued step (the KV quantization policy: stream-ordered, no host synchronisation)."""
     if max_tokens <= 0:
         return
     host = torch.empty(max_tokens + 2, dtype=torch.int32).pin_memory()
@@ -205,6 +257,8 @@ def _greedy_device_loop(eng, lm, prompt_cache, max_tokens, reserve, return_logpr
         next_lp = None
         if n != max_tokens:
             lm.fused_greedy_decode_n(1, prompt_cache, reserve_tokens=reserve)
+            if after_step is not None:
+                after_step()
             next_lp = eng.snapshot("logprobs") if return_logprobs else None
             eng.fetch_tokens(base + n + 1, 1, host[n + 1:n + 2])
             events[n + 1].record(eng.stream)

@@ -8,9 +8,13 @@ per-layer arrays grown by concatenation.  Each layer's `KVCache` is a view of th
 pool that keeps `offset / keys / values / state / trim / update_and_fetch /
 is_trimmable / size / empty / nbytes` semantics; capacity still grows in
 `step = 256` multiples (cache.py:338).
+
+`kv_bits=8` swaps the request's pool for a `QuantizedKVPool` (codes + bf16 scales / biases, the format of
+csrc/kvq.cuh) viewed per layer by `QuantizedKVCache` (cache.py:233-335).
 """
 from __future__ import annotations
 
+from contextlib import nullcontext
 from typing import Any, List, Optional
 
 import torch
@@ -20,11 +24,12 @@ class KVPool:
     step = 256
 
     def __init__(self, n_layers: int, n_kv_heads: int, head_dim: int, device, batch: int = 1,
-                 capacity: int = 0, dtype=torch.bfloat16):
+                 capacity: int = 0, dtype=torch.bfloat16, stream=None):
         self.n_layers, self.n_kv, self.hd = n_layers, n_kv_heads, head_dim
         self.batch = batch
         self.device = device
         self.dtype = dtype
+        self.stream = stream  # the stream the engine writes this pool on (None: the current stream)
         self.buf: Optional[torch.Tensor] = None
         self.capacity = 0
         self.generation = 0  # bumped whenever the buffer moves (engine must re-bind)
@@ -44,6 +49,95 @@ class KVPool:
         self.capacity = cap
         self.generation += 1
         return True
+
+
+def _kvq_check(group_size: int, bits, head_dim: Optional[int] = None):
+    if bits != 8:
+        raise NotImplementedError(f"{bits}-bit KV cache: only kv_bits=8 is built")
+    if group_size not in (32, 64, 128) or (head_dim is not None and head_dim % group_size):
+        raise ValueError(f"kv_group_size={group_size}: must be 32, 64 or 128 and divide head_dim={head_dim}")
+
+
+class QuantizedKVPool:
+    """8-bit twin of `KVPool` (format and arithmetic: csrc/kvq.cuh): codes (n_layers, 2, batch, n_kv, capacity,
+    head_dim) uint8 plus scales and biases (..., capacity, head_dim / group_size) bf16.  The one owner of the
+    allocation, growth and bulk conversion of 8-bit pools."""
+    step = 256
+    bits = 8
+
+    def __init__(self, n_layers: int, n_kv_heads: int, head_dim: int, device, group_size: int = 64,
+                 batch: int = 1, capacity: int = 0, stream=None):
+        _kvq_check(group_size, 8, head_dim)
+        self.n_layers, self.n_kv, self.hd = n_layers, n_kv_heads, head_dim
+        self.group_size = group_size
+        self.batch = batch
+        self.device = device
+        self.stream = stream
+        self.codes: Optional[torch.Tensor] = None
+        self.scales: Optional[torch.Tensor] = None
+        self.biases: Optional[torch.Tensor] = None
+        self.capacity = 0
+        self.generation = 0
+        if capacity:
+            self.reserve(capacity)
+
+    @property
+    def planes(self) -> int:
+        return self.n_layers * 2 * self.batch * self.n_kv
+
+    def bytes_per_position(self) -> int:
+        """bytes of one position of one row over all layers: codes + bf16 scales and biases"""
+        return self.n_layers * 2 * self.n_kv * (self.hd + 2 * 2 * (self.hd // self.group_size))
+
+    def reserve(self, n_tokens: int, live_tokens: int = 0) -> bool:
+        if n_tokens <= self.capacity:
+            return False
+        cap = ((max(n_tokens, 2 * self.capacity) + self.step - 1) // self.step) * self.step
+        lead = (self.n_layers, 2, self.batch, self.n_kv, cap)
+        ng = self.hd // self.group_size
+        with torch.cuda.stream(self.stream) if self.stream is not None else nullcontext():
+            new = (torch.zeros(lead + (self.hd,), dtype=torch.uint8, device=self.device),
+                   torch.zeros(lead + (ng,), dtype=torch.bfloat16, device=self.device),
+                   torch.zeros(lead + (ng,), dtype=torch.bfloat16, device=self.device))
+            if self.codes is not None and live_tokens > 0:
+                for n_, o_ in zip(new, (self.codes, self.scales, self.biases)):
+                    n_[..., :live_tokens, :].copy_(o_[..., :live_tokens, :])
+        self.codes, self.scales, self.biases = new
+        self.capacity = cap
+        self.generation += 1
+        return True
+
+    @classmethod
+    def from_pool(cls, pool: KVPool, n_tokens: int, group_size: int) -> "QuantizedKVPool":
+        """Quantize the first n_tokens positions of every plane of a bf16 pool (same capacity)."""
+        from .. import _native as N
+        q = cls(pool.n_layers, pool.n_kv, pool.hd, pool.device, group_size=group_size, batch=pool.batch,
+                capacity=max(pool.capacity, 1), stream=pool.stream)
+        if pool.buf is not None and n_tokens > 0:
+            N.check(N.lib().b200_kvq_quantize(pool.buf.data_ptr(), pool.capacity, q.codes.data_ptr(),
+                                              q.scales.data_ptr(), q.biases.data_ptr(), q.capacity, q.planes,
+                                              int(n_tokens), q.hd, group_size, _stream_handle(q)), "kvq_quantize")
+        return q
+
+    def to_bf16_pool(self, n_tokens: int) -> KVPool:
+        """A bf16 pool of the same capacity holding the dequantized first n_tokens positions (the prefix a
+        prefill chunk over this cache attends to)."""
+        from .. import _native as N
+        with torch.cuda.stream(self.stream) if self.stream is not None else nullcontext():
+            out = KVPool(self.n_layers, self.n_kv, self.hd, self.device, batch=self.batch, capacity=self.capacity,
+                         stream=self.stream)
+        assert out.capacity == self.capacity
+        if n_tokens > 0:
+            N.check(N.lib().b200_kvq_dequantize(self.codes.data_ptr(), self.scales.data_ptr(),
+                                                self.biases.data_ptr(), self.capacity, out.buf.data_ptr(),
+                                                out.capacity, self.planes, int(n_tokens), self.hd, self.group_size,
+                                                _stream_handle(self)), "kvq_dequantize")
+        return out
+
+
+def _stream_handle(pool) -> int:
+    s = pool.stream if pool.stream is not None else torch.cuda.current_stream(pool.device)
+    return s.cuda_stream
 
 
 class _BaseCache:
@@ -159,6 +253,22 @@ class KVCache(_BaseCache):
             return None
         return "causal"
 
+    def to_quantized(self, group_size: int = 64, bits: int = 4) -> "QuantizedKVCache":
+        """cache.py:415-423.  The layers of one request share a pool, so the first layer converted quantizes
+        the whole pool (one kernel) and the other layers of the same pool become views of that 8-bit pool."""
+        hd = self._pool.hd if self._pool is not None else (None if self._own is None else self._own.shape[-1])
+        _kvq_check(group_size, bits, hd)
+        if self._pool is None or self._pool.buf is None:
+            raise NotImplementedError("to_quantized: only engine (pool-backed) caches with content are converted")
+        pool = self._pool
+        q = getattr(pool, "_q8", None)
+        if q is None or q[0] != (pool.generation, self.offset, group_size):
+            q = ((pool.generation, self.offset, group_size), QuantizedKVPool.from_pool(pool, self.offset, group_size))
+            pool._q8 = q
+        out = QuantizedKVCache(group_size=group_size, bits=bits, pool=q[1], layer=self._layer, row=self._row)
+        out.offset = self.offset
+        return out
+
     def empty(self):
         return self.keys is None or self.offset == 0 and self._pool is None and self._own is None
 
@@ -168,6 +278,90 @@ class KVCache(_BaseCache):
         if k is None:
             return 0
         return 2 * k.numel() * k.element_size()
+
+
+class QuantizedKVCache(_BaseCache):
+    """One layer's view of a `QuantizedKVPool` with the reference surface (cache.py:233-335): `keys` / `values`
+    are (codes as uint32 (B, n_kv, S, head_dim / 4), scales, biases) with mx.quantize's packing (element 4i+j in
+    bits 8j of word i).  The engine appends to the pool in its decode kernels."""
+    step = 256
+
+    def __init__(self, group_size: int = 64, bits: int = 8, pool: Optional[QuantizedKVPool] = None,
+                 layer: int = 0, row: Optional[int] = None):
+        _kvq_check(group_size, bits)
+        self.group_size, self.bits = group_size, bits
+        self._pool = pool
+        self._layer = layer
+        self._row = row
+        self.offset = 0
+
+    def _side(self, side: int):
+        p = self._pool
+        if p is None or p.codes is None:
+            return None
+        sl = slice(None) if self._row is None else slice(self._row, self._row + 1)
+        return (p.codes[self._layer, side, sl].view(torch.uint32), p.scales[self._layer, side, sl],
+                p.biases[self._layer, side, sl])
+
+    @property
+    def keys(self):
+        return self._side(0)
+
+    @property
+    def values(self):
+        return self._side(1)
+
+    @property
+    def state(self):
+        k, v = self.keys, self.values
+        if self.offset == k[0].shape[2]:
+            return k, v
+        return tuple(x[..., :self.offset, :] for x in k), tuple(x[..., :self.offset, :] for x in v)
+
+    @state.setter
+    def state(self, v):
+        """(keys, values) triples of one row; written into this layer's planes of the pool (grown if needed)"""
+        k, vv = v
+        n = int(k[0].shape[2])
+        if self._pool is None:
+            raise NotImplementedError("QuantizedKVCache.state: only pool-backed caches are assigned")
+        self._pool.reserve(n, live_tokens=self.offset)
+        for side, trip in ((0, k), (1, vv)):
+            for dst, src in zip(self._side(side), trip):
+                dst[..., :n, :].copy_(src.view(dst.dtype))
+        self.offset = n
+
+    @property
+    def meta_state(self):
+        return tuple(map(str, (self.offset, self.group_size, self.bits)))
+
+    @meta_state.setter
+    def meta_state(self, v):
+        self.offset, self.group_size, self.bits = map(int, v)
+
+    def is_trimmable(self):
+        return True
+
+    def trim(self, n):
+        n = min(self.offset, n)
+        self.offset -= n
+        return n
+
+    def size(self):
+        return self.offset
+
+    def make_mask(self, N: int, return_array: bool = False, window_size=None):
+        return None if N == 1 else "causal"
+
+    def empty(self):
+        return self.keys is None
+
+    @property
+    def nbytes(self):
+        k, v = self.keys, self.values
+        if k is None:
+            return 0
+        return sum(x.numel() * x.element_size() for x in (*k, *v))
 
 
 def make_prompt_cache(model: Any, max_kv_size: Optional[int] = None) -> List[Any]:

@@ -15,7 +15,7 @@ import numpy as np
 import torch
 
 from ..base import LanguageModelOutput
-from ..cache import BatchRows, KVCache, KVPool, RowBatchKVCache
+from ..cache import BatchRows, KVCache, KVPool, QuantizedKVCache, QuantizedKVPool, RowBatchKVCache
 from .config import ModelConfig, TextConfig
 
 
@@ -112,7 +112,7 @@ class LanguageModel:
         """One device pool per request; per-layer KVCache views (models/cache.py)."""
         eng = self._engine()
         pool = KVPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim,
-                      eng.device, batch=1)
+                      eng.device, batch=1, stream=eng.stream)
         self._pool = pool
         return [KVCache(pool, l) for l in range(self.args.num_hidden_layers)]
 
@@ -128,12 +128,14 @@ class LanguageModel:
         r = BatchRows(pool, eng)
         return r, r.layer_caches()
 
-    def _bind(self, cache, need_tokens: int) -> KVPool:
+    def _bind(self, cache, need_tokens: int, decode: bool = False) -> KVPool:
         c0 = cache[0]
         pool = getattr(c0, "_pool", None)
         if pool is None:
             raise ValueError("b200 LanguageModel needs caches from make_prompt_cache(language_model)")
         eng = self._engine()
+        if any(isinstance(c, QuantizedKVCache) for c in cache):
+            return self._bind_q8(cache, need_tokens, decode)
         if pool.capacity < need_tokens:
             eng.stream.synchronize()
             with torch.cuda.stream(eng.stream):
@@ -143,6 +145,28 @@ class LanguageModel:
         eng.bind_pool(pool)
         eng.set_kv_row(c0._row or 0)
         return pool
+
+    def _bind_q8(self, cache, need_tokens: int, decode: bool):
+        """an 8-bit cache: every layer a view of ONE QuantizedKVPool.  Decode steps bind it directly.  A prefill
+        call gets a bf16 pool holding the dequantized prefix and writes its own rows through to the 8-bit pool
+        (quantized before they are attended); that bf16 pool lives until the next bind."""
+        c0 = cache[0]
+        pool = c0._pool
+        if not all(isinstance(c, QuantizedKVCache) and c._pool is pool for c in cache):
+            raise NotImplementedError("a cache that mixes 8-bit and bf16 layers is not built for single requests")
+        eng = self._engine()
+        if pool.capacity < need_tokens:
+            eng.stream.synchronize()
+            pool.reserve(need_tokens, live_tokens=c0.offset)
+        if decode:
+            eng.bind_kvq(pool)
+            eng.set_kv_row(c0._row or 0)
+            return pool
+        prefix = pool.to_bf16_pool(int(c0.offset))
+        eng.bind_pool(prefix)
+        eng.set_kv_row(c0._row or 0)
+        eng.set_prefill_kvq(pool)
+        return prefix
 
     # ------------------------------------------------------------------ call
     def __call__(self, inputs, inputs_embeds=None, mask=None, cache=None, **kwargs):
@@ -176,7 +200,7 @@ class LanguageModel:
                                                          image_grid_thw, video_grid_thw, rope_deltas_kw)
 
         need = max(cache_offset + L, reserve_tokens)
-        self._bind(cache, need)
+        self._bind(cache, need, decode=(L == 1 and inputs_embeds is None))
         V = self.args.vocab_size
         if L == 1 and inputs_embeds is None:
             # ---- decode step through the captured graph ----
@@ -197,6 +221,8 @@ class LanguageModel:
             Vp = (V + 7) // 8 * 8     # device rows are 16-byte aligned for any vocabulary
             all_logits = eng.empty((L, Vp)) if keep_all else None
             eng.prefill(emb.contiguous(), pos3, cache_offset, delta0, all_logits)
+            if isinstance(cache[0], QuantizedKVCache):
+                eng.set_prefill_kvq(None)
             logits = (all_logits[:, :V].unsqueeze(0) if keep_all
                       else eng.snapshot("logits").view(1, 1, V))
         for c in cache:
@@ -327,7 +353,7 @@ class LanguageModel:
         if rd is not None:
             self._rope_deltas = _np(rd)
         off = int(cache[0].offset)
-        self._bind(cache, max(off + 1, int(kwargs.get("reserve_tokens", 0))))
+        self._bind(cache, max(off + 1, int(kwargs.get("reserve_tokens", 0))), decode=True)
         if not chained:
             delta = int(np.asarray(self._rope_deltas).reshape(-1)[0]) if self._rope_deltas is not None else 0
             eng.set_next(int(ids[0, 0]), off, off + delta)
@@ -432,7 +458,7 @@ class LanguageModel:
         memory, no host round trip between steps).  Tokens land in the engine's token log."""
         eng = self._engine()
         off = int(cache[0].offset)
-        self._bind(cache, max(off + n_steps, reserve_tokens))
+        self._bind(cache, max(off + n_steps, reserve_tokens), decode=True)
         eng.decode(n_steps)
         self._fused_last = None
         for c in cache:
