@@ -113,6 +113,12 @@ int b200_mrope_kv_write(void* qkv, const int* pos3, const float* inv_freq,
                         int T, int ctx0, int cap, int n_heads, int n_kv,
                         int head_dim, void* stream);
 
+/* Qwen3-VL Attention.q_norm / k_norm (qwen3_vl/language.py:59-60,84-89): mx.fast.rms_norm over each q and k head of
+ * qkv (T, (n_heads + 2 n_kv) * head_dim) in place, weights (head_dim) bf16; the v heads are left alone.  Runs
+ * before b200_mrope_kv_write.  head_dim 64 or 128. */
+int b200_qk_norm(void* qkv, int T, int n_heads, int n_kv, int head_dim, const void* q_norm_w, const void* k_norm_w,
+                 float eps, void* stream);
+
 /* mx.fast.scaled_dot_product_attention as executed on the mlx CPU device
  * (fallback graph; base.py:366-373, vision.py:154): q*scale, scores, softmax and
  * output each rounded to bf16.  Strides in elements.  causal!=0: bottom-right
@@ -172,7 +178,10 @@ int b200_engine_destroy(b200_engine* e);
 /* Weight registration by name (packed names, see DESIGN.md §layout):
  *   v.patch_embed.w | v.blk.<i>.{ln1.w,ln1.b,ln2.w,ln2.b,qkv.w,qkv.b,proj.w,proj.b,
  *   fc1.w,fc1.b,fc2.w,fc2.b} | v.merger.{ln.w,ln.b,fc1.w,fc1.b,fc2.w,fc2.b} |
- *   lm.embed | lm.head (untied only) | lm.norm | lm.<i>.{ln1,ln2,wqkv,bqkv,wo,wgu,wd} */
+ *   lm.embed | lm.head (untied only) | lm.norm | lm.<i>.{ln1,ln2,wqkv,bqkv,wo,wgu,wd}
+ *   | lm.<i>.{qn,kn} (head_dim each: Qwen3-VL's q_norm / k_norm, qwen3_vl/language.py:59-60; set for every
+ *   layer or for none.  With them every path that writes K normalises q and k per head before the rotary;
+ *   the persistent k_mega / k_mega_tc kernels refuse such a model, so its steps run the per-phase kernels) */
 int b200_engine_set_weight(b200_engine* e, const char* name, const void* ptr, long n_elems);
 /* scratch for activations; must be >= b200_engine_workspace_bytes(max tokens) */
 long b200_engine_workspace_bytes(const b200_engine* e, int max_tokens, int max_patches);
@@ -214,6 +223,11 @@ int b200_kvq_dequantize(const void* codes, const void* scales, const void* biase
  * that host and device use bit-identical tables. */
 int b200_engine_set_rope_tables(b200_engine* e, const float* lm_inv_freq_host,
                                 const float* v_inv_freq_host);
+/* M-RoPE frequency-to-axis table, HOST int32 (head_dim/2 entries in {0,1,2}: which of the t / h / w position ids
+ * rotates frequency i).  The default is Qwen2-VL's chunked table (_chunked_position_selector, rope_utils.py:519-526);
+ * Qwen3-VL passes _interleaved_position_selector's (rope_utils.py:511-516).  Prefill reads it; decode positions
+ * are equal on all three axes. */
+int b200_engine_set_axis_sel(b200_engine* e, const int* axis_sel_host);
 
 /* VisionModel.__call__ (vision.py:257-290): pixel_values (n_patches, v_patch_dim)
  * f32, grid_thw_host (n_images,3) -> feats (n_patches / merge^2, v_out) bf16. */

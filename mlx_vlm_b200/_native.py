@@ -47,6 +47,7 @@ SIGNATURES = {
     "b200_rms_norm": (_I, [_P, _P, _P, _I, _I, _F, _P]),
     "b200_vision_rope": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "b200_mrope_kv_write": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_qk_norm": (_I, [_P, _I, _I, _I, _I, _P, _P, _F, _P]),
     "b200_attention": (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _I, _I, _I, _I, _I, _I,
                             _F, _P]),
     "b200_attention_fa": (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _I, _I, _I, _I, _I, _I, _P]),
@@ -60,6 +61,7 @@ SIGNATURES = {
     "b200_engine_set_workspace": (_I, [_P, _P, _L]),
     "b200_engine_bind_kv": (_I, [_P, _P, _I, _I]),
     "b200_engine_set_rope_tables": (_I, [_P, _P, _P]),
+    "b200_engine_set_axis_sel": (_I, [_P, _P]),
     "b200_engine_vision": (_I, [_P, _P, _P, _I, _P, _P]),
     "b200_engine_prefill": (_I, [_P, _P, _P, _I, _I, _I, _P, _P]),
     "b200_engine_prefill_batch": (_I, [_P, _P, _P, _I, _P, _P, _P]),

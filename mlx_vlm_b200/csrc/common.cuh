@@ -80,6 +80,36 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// ---- Qwen3-VL q/k norm (qwen3_vl/language.py:59-60,84-89) ------------------
+// One attention head of hd = 32 * NU elements held by a warp, lane l owning elements l + 32 u.  mx.fast.rms_norm
+// (oracle/mlx_semantics.py): bf16(x * rsqrt(mean(x^2) + eps)) then * w, two roundings.  Every kernel that writes a
+// normalised K row (prefill, per-phase decode, lock-step batch) calls this helper, so their rows agree bit for bit.
+template <int NU>
+__device__ __forceinline__ void warp_head_rms(float (&x)[NU], const bf16* __restrict__ w, float eps) {
+  const int lane = threadIdx.x & 31;
+  float s = 0.f;
+#pragma unroll
+  for (int u = 0; u < NU; ++u) s = fmaf(x[u], x[u], s);
+  s = warp_sum(s);
+  const float rs = 1.0f / sqrtf(s / (float)(32 * NU) + eps);
+#pragma unroll
+  for (int u = 0; u < NU; ++u) x[u] = rbf(rbf(x[u] * rs) * bf2f(w[lane + 32 * u]));
+}
+// The rotate_half rotary of the same warp-held head at one position (decode: the three M-RoPE axes agree), three
+// roundings like the M-RoPE kernels; element j pairs with j + hd/2, which the same lane holds (hd % 64 == 0).
+template <int NU>
+__device__ __forceinline__ void warp_head_rope(float (&x)[NU], int pos, const float* __restrict__ inv_freq) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int u = 0; u < NU / 2; ++u) {
+    const float ang = (float)pos * inv_freq[lane + 32 * u];
+    const float c = rbf(cosf(ang)), sn = rbf(sinf(ang));
+    const float y1 = x[u], y2 = x[u + NU / 2];
+    x[u] = rbf(rbf(y1 * c) + rbf((-y2) * sn));
+    x[u + NU / 2] = rbf(rbf(y2 * c) + rbf(y1 * sn));
+  }
+}
+
 // ---- activation restatements (oracle/mlx_semantics.py) --------------------
 // 1 / (1 + e^-x) with the SFU exponential and reciprocal (branch-free, ~3 ulp): far below the bf16 rounding every
 // bf16 caller applies next and below the 2^-17 of the split-operand GEMMs on the fp32 paths (the libm expf + IEEE

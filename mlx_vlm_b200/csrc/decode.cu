@@ -112,6 +112,7 @@ struct StreamP {
   // QKV geometry
   int n_heads, n_kv, hd, cap;
   float eps;
+  int raw_qk;        // QKV: q / k rows left unrotated (Qwen3-VL: k_qk_norm_rope normalises and rotates them)
 };
 
 constexpr int STREAM_CONSUMERS = 256;            // 8 warps
@@ -323,6 +324,11 @@ __global__ void __launch_bounds__(STREAM_THREADS, 2) k_stream(const StreamP p) {
           bf16* dst = p.vc + ((long)(slot - p.n_heads - p.n_kv) * p.cap + ctx) * p.hd;
           dst[j] = f2bf(y1);
           dst[j + half] = f2bf(y2);
+        } else if (p.raw_qk) {
+          bf16* dst = (slot < p.n_heads) ? p.out + (long)slot * p.hd
+                                         : p.kc + ((long)(slot - p.n_heads) * p.cap + ctx) * p.hd;
+          dst[j] = f2bf(y1);
+          dst[j + half] = f2bf(y2);
         } else {
           // M-RoPE, identical t/h/w position on decode (language.py:476-509)
           const float ang = (float)pos * p.inv_freq[j];
@@ -362,6 +368,30 @@ __global__ void __launch_bounds__(STREAM_THREADS, 2) k_stream(const StreamP p) {
       p.partials[blockIdx.x] = make_float2(M, L);
     }
   }
+}
+
+// ---------------------------------------------------------------------------
+// k_qk_norm_rope (Qwen3-VL, language.py:84-89 then the M-RoPE of :113-119): after a raw_qk QKV kernel, q_norm /
+// k_norm and the rotary of one decode position on the q heads (qbuf, in place) and the new K row (the cache at
+// ctx, in place).  One warp per head.
+template <int NU>
+__global__ void __launch_bounds__(256) k_qk_norm_rope(const DecodeDims d, bf16* __restrict__ qbuf,
+                                                      bf16* __restrict__ kc, const DecState* __restrict__ st,
+                                                      const float* __restrict__ inv_freq,
+                                                      const bf16* __restrict__ qn, const bf16* __restrict__ kn) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int slot = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (slot >= d.n_heads + d.n_kv) return;
+  const int ctx = st->ctx, pos = st->pos;
+  bf16* base = slot < d.n_heads ? qbuf + (long)slot * d.hd : kc + ((long)(slot - d.n_heads) * d.cap + ctx) * d.hd;
+  float x[NU];
+#pragma unroll
+  for (int u = 0; u < NU; ++u) x[u] = bf2f(base[lane + 32 * u]);
+  warp_head_rms<NU>(x, slot < d.n_heads ? qn : kn, d.eps);
+  warp_head_rope<NU>(x, pos, inv_freq);
+#pragma unroll
+  for (int u = 0; u < NU; ++u) base[lane + 32 * u] = f2bf(x[u]);
 }
 
 // ---------------------------------------------------------------------------
@@ -839,6 +869,9 @@ static int stream_geometry(StreamP& p, bool pair, int units /*rows or pairs avai
   const long unit = (long)p.K * 2 * (pair ? 2 : 1);
   int R = 8;
   while (R > 1 && (R * unit > 50 * 1024 || R > units)) R >>= 1;
+  // fewer rows per tile -> more K slices: keep the activation slice within the 10 chunks per lane of the largest
+  // k_stream instantiation (e.g. K = 6144: 4 rows would need 12)
+  while (R > 1 && cdiv(cdiv(p.K >> 3, 8 / R), 32) > 10) R >>= 1;
   B200_REQUIRE(R * unit <= STREAM_SMEM_BUDGET / 2, "decode: K=%d too large for the weight ring", p.K);
   p.R = R;
   p.S = 8 / R;
@@ -915,22 +948,30 @@ int decode_prepare(const DecodeDims& d, int cluster) {
     B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
     if ((rc = set_carveout(k_attn, (int)smem))) return rc;
   }
-  if ((rc = set_carveout(k_sample, 0)) || (rc = set_carveout(k_set_state, 0))) return rc;
+  if ((rc = set_carveout(k_sample, 0)) || (rc = set_carveout(k_set_state, 0)) ||
+      (rc = set_carveout(k_qk_norm_rope<4>, 0)) || (rc = set_carveout(k_qk_norm_rope<2>, 0)))
+    return rc;
   return B200_OK;
 }
 
 int launch_qkv(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* qbuf, bf16* kc,
-               bf16* vc, const DecState* st, const float* inv_freq, cudaStream_t s) {
+               bf16* vc, const DecState* st, const float* inv_freq, cudaStream_t s, const bf16* qn,
+               const bf16* kn) {
   StreamP p = {};
   p.W = lw.wqkv; p.bias = lw.bqkv; p.x = h; p.lnw = lw.ln1; p.out = qbuf; p.kc = kc; p.vc = vc;
   p.st = st; p.inv_freq = inv_freq; p.K = d.hidden; p.N = 0;
   p.n_heads = d.n_heads; p.n_kv = d.n_kv; p.hd = d.hd; p.cap = d.cap; p.eps = d.eps;
+  p.raw_qk = qn != nullptr;
   const int half = d.hd / 2;
   int rc = stream_geometry(p, true, half);
   if (rc) return rc;
   B200_REQUIRE(half % p.R == 0, "decode qkv: head_dim/2=%d not a multiple of tile rows %d", half, p.R);
   p.tiles = (d.n_heads + 2 * d.n_kv) * (half / p.R);
-  return launch_stream<SM_QKV>(p, g_sm_count, s);
+  if ((rc = launch_stream<SM_QKV>(p, g_sm_count, s)) || !qn) return rc;
+  B200_REQUIRE(kn && (d.hd == 64 || d.hd == 128), "decode q/k norm: head_dim=%d (64 | 128)", d.hd);
+  const dim3 grid(cdiv(d.n_heads + d.n_kv, 8));
+  if (d.hd == 128) return launch_ex(k_qk_norm_rope<4>, grid, dim3(256), 0, s, 1, d, qbuf, kc, st, inv_freq, qn, kn);
+  return launch_ex(k_qk_norm_rope<2>, grid, dim3(256), 0, s, 1, d, qbuf, kc, st, inv_freq, qn, kn);
 }
 
 int launch_attn(const DecodeDims& d, const bf16* qbuf, const bf16* kc, const bf16* vc, bf16* out,

@@ -69,6 +69,11 @@ struct MegaP {
   float* att_part;  // [groups][8 units][4*hd] fp32 partial attention outputs
   float* att_stats; // [groups][8 units][4 heads] x 2 words {float bits << 32 | epoch}: (max, sum exp)
   long long* dbg;  // optional [2][1024][2] globaltimer stamps (arrive, release) per barrier
+  // Qwen3-VL q_norm / k_norm (qk_norm != 0): the QKV phase leaves q / k unrotated and a q/k-norm phase between two
+  // grid barriers normalises and rotates them (the per-phase step's arithmetic, common.cuh::warp_head_rms / _rope)
+  int qk_norm;
+  const bf16* qn[MEGA_MAX_LAYERS];
+  const bf16* kn[MEGA_MAX_LAYERS];
 };
 int mega_fill(MegaP& p, int sm_count);
 int mega_launch(const MegaP& p, int sm_count, cudaStream_t s);
@@ -112,6 +117,8 @@ struct BdModel {
   bf16* kv;            // layer 0 K plane of row 0
   long layer_stride, v_off, row_stride;
   int kv_batch, sm_count;
+  const bf16* const* qn;  // per layer q_norm / k_norm weights (Qwen3-VL), or nullptr
+  const bf16* const* kn;
 };
 int batch_decoder_begin(void** handle, const BdModel& m, int B, const int* tok, const int* ctx, const int* pos,
                         const int* active, cudaStream_t s);
@@ -126,8 +133,11 @@ void decode_set_pdl(bool on);
 int decode_prepare(const DecodeDims& d, int cluster);
 int head_grid();
 size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap);
+// qn / kn (Qwen3-VL q_norm / k_norm weights, both or neither): the QKV kernel leaves q / k unrotated and a second
+// kernel (k_qk_norm_rope) normalises and rotates the q heads and the new K row
 int launch_qkv(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* qbuf, bf16* kc,
-               bf16* vc, const DecState* st, const float* inv_freq, cudaStream_t s);
+               bf16* vc, const DecState* st, const float* inv_freq, cudaStream_t s, const bf16* qn = nullptr,
+               const bf16* kn = nullptr);
 int launch_attn(const DecodeDims& d, const bf16* qbuf, const bf16* kc, const bf16* vc, bf16* out,
                 const DecState* st, int cluster, cudaStream_t s);
 int launch_res(const bf16* W, const bf16* x, bf16* h, int N, int K, cudaStream_t s);
@@ -160,6 +170,9 @@ int mrope_kv_write(void* qkv, const int* pos3, const float* inv_freq, const int*
                    cudaStream_t st, float q_scale = 0.f, void* vt = nullptr, int t_ld = 0,
                    const KvRef* ref = nullptr, int layer = 0, void* kws = nullptr, const void* tok_loc = nullptr,
                    long row_stride = 0);
+// Qwen3-VL q/k RMSNorm per head, in place on the q and k heads of qkv (before mrope_kv_write)
+int qk_norm(void* qkv, int T, int n_heads, int n_kv, int hd, const void* qn, const void* kn, float eps,
+            cudaStream_t st);
 int vision_qkv_post(void* qkv, const int* pos_hw, const float* inv_freq, int n_tok, int n_heads, int hd,
                     float scale, void* vt, int t_ld, cudaStream_t st, const void* cs = nullptr);
 // cos / sin table [n_tok][hd / 2] float2 for vision_qkv_post (computed once per tower call)

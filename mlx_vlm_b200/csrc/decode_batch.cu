@@ -90,6 +90,8 @@ struct BdAttnP {
   bf16* out;          // [B][n_heads*hd]
   int n_heads, n_kv, cap, hsplit;
   float scale_bf;
+  const bf16 *qn, *kn;  // Qwen3-VL q_norm / k_norm weights of the layer (nullptr: no q/k norm)
+  float eps;
   // weights of the GEMMs that follow (o_proj, gate/up, down): this kernel is a chain of dependent round trips that
   // leaves HBM idle, so its CTAs ask the L2 for them up front (l2_prefetch_span; weights are static during a step)
   const void* pf[3];
@@ -156,6 +158,18 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
     (slot < G ? qs + slot * HD : (slot == G ? kn : vn))[j] = a;
   }
   __syncthreads();
+  if (p.qn) {  // q_norm / k_norm (qwen3_vl/language.py:84-89) before the rotary, one warp per head
+    for (int slot = warp; slot <= G; slot += 8) {
+      float* v = slot < G ? qs + slot * HD : kn;
+      float x[HD / 32];
+#pragma unroll
+      for (int u = 0; u < HD / 32; ++u) x[u] = v[lane + 32 * u];
+      warp_head_rms<HD / 32>(x, slot < G ? p.qn : p.kn, p.eps);
+#pragma unroll
+      for (int u = 0; u < HD / 32; ++u) v[lane + 32 * u] = x[u];
+    }
+    __syncthreads();
+  }
   // M-RoPE at a decode position: the three axes carry the same position (language.py:476-509)
   for (int i = threadIdx.x; i < (G + 1) * half; i += 256) {
     const int slot = i / half, j = i % half;
@@ -588,6 +602,7 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
     ap.ctx = d->ctx; ap.pos = d->pos; ap.kv = m.kv + (long)l * m.layer_stride; ap.v_off = m.v_off;
     ap.row_stride = m.row_stride; ap.out = d->att; ap.n_heads = dd.n_heads; ap.n_kv = dd.n_kv; ap.cap = dd.cap;
     ap.hsplit = hs; ap.scale_bf = dd.scale_bf;
+    ap.qn = m.qn ? m.qn[l] : nullptr; ap.kn = m.kn ? m.kn[l] : nullptr; ap.eps = dd.eps;
     {  // o_proj, then gate/up, then down, as far as the budget goes
       long left = bd_prefetch_budget();
       const void* w[3] = {lw.wo, lw.wgu, lw.wd};

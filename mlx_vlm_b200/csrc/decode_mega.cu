@@ -82,6 +82,25 @@ __device__ __forceinline__ void l2_prefetch_phase(const MegaPhase& g, const bf16
   }
 }
 
+// ---- q/k-norm phase (Qwen3-VL, language.py:84-89 then the rotary): one consumer warp per q head / new K row,
+// in place in qbuf and the cache at ctx.  Loads and stores bypass L1 (the rows were written by other CTAs in the
+// QKV phase, and the attention phase of other CTAs reads them after the next grid barrier).
+template <int NU>
+__device__ __forceinline__ void qk_norm_phase(const MegaP& p, int l, bf16* qbuf, bf16* kc, int ctx, int pos) {
+  const DecodeDims& d = p.d;
+  const int lane = threadIdx.x & 31;
+  for (int slot = blockIdx.x * 8 + (threadIdx.x >> 5); slot < d.n_heads + d.n_kv; slot += gridDim.x * 8) {
+    bf16* base = slot < d.n_heads ? qbuf + (long)slot * d.hd : kc + ((long)(slot - d.n_heads) * d.cap + ctx) * d.hd;
+    float x[NU];
+#pragma unroll
+    for (int u = 0; u < NU; ++u) x[u] = bf2f(__ldcg(base + lane + 32 * u));
+    warp_head_rms<NU>(x, slot < d.n_heads ? p.qn[l] : p.kn[l], d.eps);
+    warp_head_rope<NU>(x, pos, p.inv_freq);
+#pragma unroll
+    for (int u = 0; u < NU; ++u) __stcg(base + lane + 32 * u, f2bf(x[u]));
+  }
+}
+
 // ---- consumers: one GEMV phase ----------------------------------------------
 struct PhaseIO {
   const bf16* x;     // activation vector (cross-CTA: read with ld.cg)
@@ -226,6 +245,11 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
           dst[j] = f2bf(y1);
           dst[j + half] = f2bf(y2);
           if (FLOW) st_word(io.qkvw + (long)slot * half + j, bf_bits(y1) | (bf_bits(y2) << 16), io.epoch);
+        } else if (!FLOW && p.qk_norm) {  // raw q / k: the q/k-norm phase normalises and rotates them
+          bf16* dst = (slot < p.d.n_heads) ? io.out + (long)slot * hd
+                                           : io.kc + ((long)(slot - p.d.n_heads) * p.d.cap + ctx) * hd;
+          dst[j] = f2bf(y1);
+          dst[j + half] = f2bf(y2);
         } else {
           const float ang = (float)pos * (ti == 0 ? pc : p.inv_freq[j]);
           const float c = rbf(cosf(ang)), sn = rbf(sinf(ang));
@@ -449,6 +473,11 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega(const MegaP p) {
       consume_phase<PH_QKV, CHH, FLOW>(p, p.ph[PH_QKV], io, ring, xs, &sh, rg, ctx, pos);
     }
     if (!FLOW) grid_barrier(p, &sh, bidx);
+    if (!FLOW && p.qk_norm) {
+      if (d.hd == 128) qk_norm_phase<4>(p, l, p.qbuf, kc, ctx, pos);
+      else qk_norm_phase<2>(p, l, p.qbuf, kc, ctx, pos);
+      grid_barrier(p, &sh, bidx);
+    }
     if ((int)blockIdx.x < p.attn_ctas) {
       const AttnParts ap = {nullptr, nullptr, 0, p.qkv_w, ep};
       constexpr int AM = FLOW ? ATT_FLOW : ATT_PLAIN;
@@ -499,6 +528,9 @@ static int mega_geometry(MegaPhase& g, int K, int N, bool pair, int units) {
   const long unit = (long)K * 2 * (pair ? 2 : 1);
   int R = 8;
   while (R > 1 && (R * unit > MEGA_STAGE || R > units)) R >>= 1;
+  // as decode.cu::stream_geometry: more K slices when a slice would exceed the 10 chunks per lane of the largest
+  // instantiation (K = 6144, Qwen3-VL-2B's down projection)
+  while (R > 1 && cdiv(cdiv(K >> 3, 8 / R), 32) > 10) R >>= 1;
   B200_REQUIRE(R * unit <= MEGA_STAGE, "mega: K=%d does not fit a %d-byte ring stage", K, MEGA_STAGE);
   g.R = R;
   g.S = 8 / R;
@@ -516,6 +548,8 @@ static size_t mega_attn_scratch(const DecodeDims& d) {
 int mega_fill(MegaP& p, int sm_count) {
   const DecodeDims& d = p.d;
   int rc;
+  B200_REQUIRE(!p.qk_norm || (!p.flow && (d.hd == 64 || d.hd == 128)),
+               "mega: q/k norm needs the barrier mode (not dataflow) and head_dim 64 | 128");
   const int half = d.hd / 2;
   if ((rc = mega_geometry(p.ph[PH_QKV], d.hidden, 0, true, half))) return rc;
   B200_REQUIRE(half % p.ph[PH_QKV].R == 0, "mega: head_dim/2 %% tile rows != 0");

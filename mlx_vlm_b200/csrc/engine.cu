@@ -47,6 +47,9 @@ struct b200_engine {
              *m_fc2w = nullptr, *m_fc2b = nullptr;
   const bf16 *embed = nullptr, *head = nullptr, *norm = nullptr;
   std::vector<LayerW> layers;
+  // Qwen3-VL q_norm / k_norm weights per layer (lm.<i>.qn / lm.<i>.kn): registered for every layer or for none
+  bool qk_norm = false;
+  std::vector<const bf16*> qn, kn;
   // workspace (caller-owned)
   uint8_t* ws = nullptr;
   long ws_bytes = 0;
@@ -211,6 +214,14 @@ static int resolve(b200_engine* e) {
     l.wo = need(e, p + "wo", H * (long)c.n_heads * c.head_dim, &ok);
     l.wgu = need(e, p + "wgu", 2 * I * H, &ok); l.wd = need(e, p + "wd", H * I, &ok);
   }
+  e->qk_norm = ok && c.n_layers > 0 && e->w.count("lm.0.qn");
+  e->qn.assign(e->qk_norm ? c.n_layers : 0, nullptr);
+  e->kn.assign(e->qk_norm ? c.n_layers : 0, nullptr);
+  for (int i = 0; e->qk_norm && i < c.n_layers && ok; ++i) {
+    const std::string p = "lm." + std::to_string(i) + ".";
+    e->qn[i] = need(e, p + "qn", c.head_dim, &ok);
+    e->kn[i] = need(e, p + "kn", c.head_dim, &ok);
+  }
   if (!ok) return B200_ERR_STATE;
   e->resolved = true;
   return B200_OK;
@@ -237,6 +248,8 @@ static int mega_prepare(b200_engine* e, cudaStream_t s) {
   const auto& c = e->cfg;
   B200_REQUIRE(c.n_layers <= MEGA_MAX_LAYERS, "mega: %d layers > %d", c.n_layers, MEGA_MAX_LAYERS);
   B200_REQUIRE(!e->q8.codes, "mega: the persistent kernels read a bf16 KV pool; an 8-bit pool runs the per-phase kernels");
+  B200_REQUIRE(!e->qk_norm || e->use_mega == 1,
+               "mega: k_mega_tc has no q/k norm (Qwen3-VL); such a model runs k_mega or the per-phase kernels");
   if (!e->bar) {
     B200_CUDA(cudaMalloc(&e->bar, sizeof(unsigned long long)));
     B200_CUDA(cudaMemset(e->bar, 0, sizeof(unsigned long long)));
@@ -261,6 +274,11 @@ static int mega_prepare(b200_engine* e, cudaStream_t s) {
   p.partials = e->partials; p.st = e->st; p.token_log = e->token_log; p.log_cap = e->log_cap;
   p.force = e->force; p.inv_freq = e->lm_inv_freq; p.bar = e->bar; p.advance = 1;
   p.dbg = e->dbg;
+  p.qk_norm = e->qk_norm;
+  for (int l = 0; e->qk_norm && l < c.n_layers; ++l) {
+    p.qn[l] = e->qn[l];
+    p.kn[l] = e->kn[l];
+  }
   // tuning aids
   p.max_inflight = e->fma_inflight;
   p.flow = e->flow;
@@ -354,7 +372,9 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
     bf16* sv = sk + (long)c.n_kv_heads * e->kv_cap * c.head_dim;
     for (int l = 0; l < c.n_layers; ++l) {
       const LayerW& lw = e->layers[l];
-      if ((rc = launch_qkv(d, lw, e->h, e->qbuf, sk, sv, e->st, e->lm_inv_freq, s))) return rc;
+      if ((rc = launch_qkv(d, lw, e->h, e->qbuf, sk, sv, e->st, e->lm_inv_freq, s, e->qk_norm ? e->qn[l] : nullptr,
+                           e->qk_norm ? e->kn[l] : nullptr)))
+        return rc;
       if ((rc = launch_attn_q8(d, e->qbuf, e->q8_plane(l, 0, e->kv_row, e->q8), e->q8_plane(l, 1, e->kv_row, e->q8), sk, sv,
                                e->attn, e->st, e->attn_cluster, s)))
         return rc;
@@ -367,7 +387,9 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
     const LayerW& lw = e->layers[l];
     bf16* kc = e->kptr(l, e->kv_row);
     bf16* vc = e->vptr(l, e->kv_row);
-    if ((rc = launch_qkv(d, lw, e->h, e->qbuf, kc, vc, e->st, e->lm_inv_freq, s))) return rc;
+    if ((rc = launch_qkv(d, lw, e->h, e->qbuf, kc, vc, e->st, e->lm_inv_freq, s, e->qk_norm ? e->qn[l] : nullptr,
+                         e->qk_norm ? e->kn[l] : nullptr)))
+      return rc;
     if ((rc = launch_attn(d, e->qbuf, kc, vc, e->attn, e->st, e->attn_cluster, s))) return rc;
     if ((rc = launch_res(lw.wo, e->attn, e->h, c.hidden, c.n_heads * c.head_dim, s))) return rc;
     if ((rc = launch_gateup(d, lw, e->h, e->act, s))) return rc;
@@ -382,7 +404,7 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
 }
 
 static int kernels_per_step(const b200_engine* e) {
-  return e->active_mega() ? 1 : e->cfg.n_layers * 5 + 2;
+  return e->active_mega() ? 1 : e->cfg.n_layers * (e->qk_norm ? 6 : 5) + 2;
 }
 
 
@@ -726,6 +748,10 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
     bf16* kc = e->kptr(l, e->kv_row);
     bf16* vc = e->vptr(l, e->kv_row);
     if ((rc = v2_linear(e, xn, H, lw.wqkv, lw.bqkv, qkv, QKV, T, (int)QKV, (int)H, B200_EPI_NONE, s))) return rc;
+    if (e->qk_norm) {
+      if ((rc = qk_norm(qkv, T, c.n_heads, c.n_kv_heads, hd, e->qn[l], e->kn[l], c.rms_eps, s))) return rc;
+      e->launches += 1;
+    }
     // the pipelined kernel needs V^T of EVERY key: available for a fresh prompt (ctx0 == 0).  It then
     // reads the chunk's own rotated K copy and V^T from the workspace, and the cache is addressed through
     // e->kvref: nothing about the KV pool is baked into the captured graph.
@@ -935,6 +961,15 @@ int b200_engine_set_rope_tables(b200_engine* e, const float* lm_inv_freq_host,
   return B200_OK;
 }
 
+int b200_engine_set_axis_sel(b200_engine* e, const int* axis_sel_host) {
+  B200_REQUIRE(e && axis_sel_host, "set_axis_sel: null argument");
+  const int n = e->cfg.head_dim / 2;
+  for (int i = 0; i < n; ++i)
+    B200_REQUIRE(axis_sel_host[i] >= 0 && axis_sel_host[i] <= 2, "set_axis_sel: entry %d is %d (0, 1 or 2)", i,
+                 axis_sel_host[i]);
+  B200_CUDA(cudaMemcpy(e->axis_sel, axis_sel_host, (size_t)n * 4, cudaMemcpyHostToDevice));
+  return B200_OK;
+}
 
 long b200_engine_workspace_bytes(const b200_engine* e, int max_tokens, int max_patches) {
   const auto& c = e->cfg;
@@ -1146,6 +1181,8 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
     if ((rc = rms_norm(h, lw.ln1, xn, T, (int)H, c.rms_eps, s))) return rc;
     if ((rc = gemm_bf16_tn(xn, H, lw.wqkv, lw.bqkv, nullptr, 0, qkv, QKV, T, (int)QKV, (int)H,
                            B200_EPI_NONE, s)))
+      return rc;
+    if (e->qk_norm && (rc = qk_norm(qkv, T, c.n_heads, c.n_kv_heads, c.head_dim, e->qn[l], e->kn[l], c.rms_eps, s)))
       return rc;
     if ((rc = mrope_kv_write(qkv, pos3, e->lm_inv_freq, e->axis_sel, kc, vc, T, ctx0, e->kv_cap,
                              c.n_heads, c.n_kv_heads, c.head_dim, s)))
@@ -1452,6 +1489,8 @@ static void bd_model(b200_engine* e, BdModel* m) {
   m->layer_stride = 2L * m->v_off;
   m->kv_batch = e->kv_batch;
   m->sm_count = e->sm_count;
+  m->qn = e->qk_norm ? e->qn.data() : nullptr;
+  m->kn = e->qk_norm ? e->kn.data() : nullptr;
 }
 
 int b200_batch_begin(b200_engine* e, int B, const int* tok, const int* ctx, const int* pos, const int* active,

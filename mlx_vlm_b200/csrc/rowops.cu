@@ -321,6 +321,42 @@ mrope_kv_write_tiled_kernel(bf16* __restrict__ qkv, const int* __restrict__ pos3
 }
 
 // ---------------------------------------------------------------------------
+// Qwen3-VL q_norm / k_norm (language.py:84-89) in place on the q and k heads of qkv (T, (n_heads + 2 n_kv) * hd),
+// before mrope_kv_write rotates and appends them.  One warp per (token, q or k head).
+template <int NU>
+__global__ void __launch_bounds__(256) qk_norm_kernel(bf16* __restrict__ qkv, int T, int n_heads, int n_kv,
+                                                      const bf16* __restrict__ qn, const bf16* __restrict__ kn,
+                                                      float eps) {
+  pdl_prologue();
+  const int hd = 32 * NU, lane = threadIdx.x & 31;
+  const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int qk = n_heads + n_kv;
+  if (warp >= (long)T * qk) return;
+  const int t = (int)(warp / qk), slot = (int)(warp % qk);
+  bf16* base = qkv + (long)t * (qk + n_kv) * hd + (long)slot * hd;
+  float x[NU];
+#pragma unroll
+  for (int u = 0; u < NU; ++u) x[u] = bf2f(base[lane + 32 * u]);
+  warp_head_rms<NU>(x, slot < n_heads ? qn : kn, eps);
+#pragma unroll
+  for (int u = 0; u < NU; ++u) base[lane + 32 * u] = f2bf(x[u]);
+}
+
+int qk_norm(void* qkv, int T, int n_heads, int n_kv, int hd, const void* qn, const void* kn, float eps,
+            cudaStream_t st) {
+  B200_REQUIRE(T > 0 && qn && kn && (hd == 64 || hd == 128), "qk_norm: T=%d head_dim=%d (64 | 128)", T, hd);
+  const long warps = (long)T * (n_heads + n_kv);
+  const dim3 grid(cdiv(warps, 8));
+  if (hd == 128)
+    B200_CUDA(launch_pdl(qk_norm_kernel<4>, grid, dim3(256), 0, st, (bf16*)qkv, T, n_heads, n_kv, (const bf16*)qn,
+                         (const bf16*)kn, eps));
+  else
+    B200_CUDA(launch_pdl(qk_norm_kernel<2>, grid, dim3(256), 0, st, (bf16*)qkv, T, n_heads, n_kv, (const bf16*)qn,
+                         (const bf16*)kn, eps));
+  return B200_OK;
+}
+
+// ---------------------------------------------------------------------------
 __global__ void swiglu_kernel(const bf16* __restrict__ gu, bf16* __restrict__ out, int rows,
                               int inter) {
   const int nvec = inter >> 3;
@@ -658,6 +694,10 @@ int b200_mrope_kv_write(void* qkv, const int* pos3, const float* inv_freq, const
                         int hd, void* st) {
   return mrope_kv_write(qkv, pos3, inv_freq, axis_sel, kc, vc, T, ctx0, cap, n_heads, n_kv, hd,
                         (cudaStream_t)st, 0.f, nullptr, 0, nullptr, 0, nullptr, nullptr, 0);
+}
+int b200_qk_norm(void* qkv, int T, int n_heads, int n_kv, int hd, const void* q_norm_w, const void* k_norm_w,
+                 float eps, void* st) {
+  return qk_norm(qkv, T, n_heads, n_kv, hd, q_norm_w, k_norm_w, eps, (cudaStream_t)st);
 }
 int b200_vision_qkv_post(void* qkv, const int* pos_hw, const float* inv_freq, int n_tok, int n_heads,
                          int hd, float scale, void* vt, int t_ld, void* st) {

@@ -88,9 +88,18 @@ class Engine:
         self._ws_tokens, self._ws_patches = tokens, patches
 
     # -- kv ------------------------------------------------------------------
+    def _check_pool_shape(self, pool):
+        # the C ABI takes no pool size: a pool laid out for other head counts / widths than the engine's would be
+        # indexed past its end by the kernels
+        c = self.cfg
+        if (pool.n_layers, pool.n_kv, pool.hd) != (c.n_layers, c.n_kv_heads, c.head_dim):
+            raise N.B200Error(f"KV pool (layers, kv heads, head_dim) = {(pool.n_layers, pool.n_kv, pool.hd)} does not "
+                              f"match the engine's {(c.n_layers, c.n_kv_heads, c.head_dim)}")
+
     def bind_pool(self, pool: KVPool):
         # keyed on the device buffer itself (not id(pool): CPython reuses ids of collected pools);
         # the engine keeps a strong reference to the bound buffer so its address cannot be recycled
+        self._check_pool_shape(pool)
         key = (pool.buf.data_ptr(), pool.batch, pool.capacity)
         if key != self._bound:
             N.check(self.lib.b200_engine_bind_kv(self.h, pool.buf.data_ptr(), pool.batch,
@@ -101,6 +110,7 @@ class Engine:
     def bind_kvq(self, pool):
         """bind an 8-bit pool (models/cache.py QuantizedKVPool) in place of the bf16 one: decode steps then run
         the per-phase kernels with the 8-bit attention (csrc/kvq.cu)"""
+        self._check_pool_shape(pool)
         key = ("q8", pool.codes.data_ptr(), pool.batch, pool.capacity, pool.group_size)
         if key != self._bound:
             N.check(self.lib.b200_engine_bind_kvq(self.h, pool.codes.data_ptr(), pool.scales.data_ptr(),

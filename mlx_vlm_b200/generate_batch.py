@@ -201,6 +201,7 @@ class BatchGenerator:
         lm = getattr(model, "language_model", None)
         # lock-step batched decode needs the native batched decoder (<= 16 rows per weight stream)
         self._lockstep = (hasattr(eng, "batch_begin") and hasattr(lm, "make_cache_row")
+                          and getattr(lm, "lockstep_supported", True)
                           and not unsupported.pop("time_multiplex", False))
         if self._lockstep:
             self.completion_batch_size = min(self.completion_batch_size, 16)
