@@ -202,6 +202,22 @@ int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases
  * attends to its prefix and to itself in quantized form.  codes == NULL switches the write-through off;
  * binding a pool switches it off too. */
 int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size);
+/* Lock-step batch pool of kv_bits=8, the reference's batch rule (generate/ar.py:751-859 `_make_cache`: a
+ * BatchQuantizedKVCache for every layer where models/cache.py:8-21 `should_quantize_kv_layer` holds, a BatchKVCache
+ * for the others).  Layers 0 .. n_q8_layers-1 live in the 8-bit pool (n_q8_layers, 2, batch, n_kv, cap, ...) of the
+ * b200_engine_bind_kvq format, layers n_q8_layers .. n_layers-1 in the bf16 pool (n_layers - n_q8_layers, 2, batch,
+ * n_kv, cap, head_dim) — NULL when every layer is 8-bit.  Both share batch and cap.  b200_batch_begin /
+ * b200_batch_decode then quantize each row's new K/V on the 8-bit layers before they are attended
+ * (BatchQuantizedKVCache.update_and_fetch, models/cache.py:1747-1960).  Such a binding serves the batched decoder
+ * only: prefill and single-row decode calls refuse it. */
+int b200_engine_bind_batch_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int n_q8_layers,
+                               void* bf16_pool, int batch, int cap);
+/* b200_engine_set_prefill_kvq into ROW `row` of an 8-bit batch pool of `rows` rows and capacity `cap` holding layers
+ * 0 .. n_q8_layers-1 (the layout of b200_engine_bind_batch_kvq): the prefill of one admitted row writes its K/V rows
+ * of those layers through to the batch pool (quantized before they are attended, BatchQuantizedKVCache.update_and_fetch
+ * on a prefill chunk); the other layers stay bf16 in the bound pool.  Reset like b200_engine_set_prefill_kvq. */
+int b200_engine_set_prefill_kvq_row(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int rows,
+                                    int cap, int row, int n_q8_layers);
 /* One 8-bit decode attention step (the kernel of the per-phase decode step) on caller buffers, synchronous:
  * qbuf (n_heads, head_dim) bf16; K / V planes of one row and layer (n_kv, cap, ...); stage_k / stage_v bf16
  * (n_kv, cap, head_dim) holding the new row at position ctx; out (n_heads, head_dim) bf16. */
@@ -387,6 +403,23 @@ int b200_batch_fetch(b200_engine* e, long first_step, int n_steps, int* tok_host
 const void* b200_batch_logits(b200_engine* e);
 const void* b200_batch_logprobs(b200_engine* e); /* same layout (want_logprobs) */
 const int* b200_batch_token_log(b200_engine* e); /* device int32 [4096 steps][16 rows]        */
+/* One lock-step attention of an 8-bit layer (the kv_bits=8 variant of the batched decoder's attention kernel) on
+ * caller buffers, stream-ordered.  Replaces, for one decode step of a batch, BatchQuantizedKVCache.update_and_fetch
+ * (models/cache.py:1805-1857) followed by quantized_scaled_dot_product_attention (models/base.py:260-356, the
+ * quantized branch of scaled_dot_product_attention).  Arguments: qkv (B, (n_heads + 2 n_kv) head_dim) fp32 rows before bias; bias (n_heads + 2 n_kv)
+ * head_dim bf16; inv_freq (head_dim / 2) fp32; ctx / pos (B) int32 device; codes / scales / biases the layer's planes
+ * (2, pool_rows, n_kv, cap, ...) in the b200_engine_bind_kvq format; q_norm / k_norm (head_dim) bf16 or NULL.  Row b
+ * quantizes its new K/V row, appends it at ctx[b] and attends over positions 0 .. ctx[b]; out (B, n_heads, head_dim). */
+int b200_batch_kvq_attention(const float* qkv, const void* bias, const float* inv_freq, const int* ctx, const int* pos,
+                             void* codes, void* scales, void* biases, int group_size, int pool_rows, int cap, void* out,
+                             int B, int n_heads, int n_kv, int head_dim, const void* q_norm, const void* k_norm, float eps,
+                             void* stream);
+/* BatchQuantizedKVCache.filter / extend / extract (models/cache.py:1747-1960) on 8-bit pools: b200_kv_copy_row for
+ * any per-position plane set — bytes_per_position = head_dim (codes), 2 * head_dim / group_size (scales, biases) or
+ * 2 * head_dim (bf16 K/V).  The bytes move unchanged. */
+int b200_pool_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool, int src_batch,
+                       int src_cap, int src_row, int n_layers, int n_kv, int bytes_per_position, int n_tokens,
+                       void* stream);
 /* BatchKVCache.filter / extend / extract (cache.py:1077-1201) on device pools: copy the first
  * n_tokens positions of one row of a pool into a row of another (or the same) pool */
 int b200_kv_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool,

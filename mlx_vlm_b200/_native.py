@@ -104,6 +104,10 @@ SIGNATURES = {
     "b200_kv_copy_row": (_I, [_P, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "b200_engine_bind_kvq": (_I, [_P, _P, _P, _P, _I, _I, _I]),
     "b200_engine_set_prefill_kvq": (_I, [_P, _P, _P, _P, _I]),
+    "b200_engine_bind_batch_kvq": (_I, [_P, _P, _P, _P, _I, _I, _P, _I, _I]),
+    "b200_engine_set_prefill_kvq_row": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I]),
+    "b200_batch_kvq_attention": (_I, [_P] * 8 + [_I, _I, _I, _P, _I, _I, _I, _I, _P, _P, _F, _P]),
+    "b200_pool_copy_row": (_I, [_P, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "b200_kvq_decode_attention": (_I, [_P] * 10 + [_I] * 7 + [_P]),
     "b200_kvq_quantize": (_I, [_P, _I, _P, _P, _P, _I, _L, _I, _I, _I, _P]),
     "b200_kvq_dequantize": (_I, [_P, _P, _P, _I, _P, _I, _L, _I, _I, _I, _P]),

@@ -114,12 +114,23 @@ struct BdModel {
   const LayerW* layers;
   const bf16 *embed, *head, *final_norm;
   const float* inv_freq;
-  bf16* kv;            // layer 0 K plane of row 0
+  bf16* kv;            // K plane of row 0 of the first bf16 layer (layer q8_layers), or nullptr
   long layer_stride, v_off, row_stride;
   int kv_batch, sm_count;
   const bf16* const* qn;  // per layer q_norm / k_norm weights (Qwen3-VL), or nullptr
   const bf16* const* kn;
+  // kv_bits=8 (b200_engine_bind_batch_kvq): layers 0 .. q8_layers-1 live in an 8-bit pool (format kvq.cuh) of the
+  // same rows and capacity, layers q8_layers .. n_layers-1 in the bf16 pool `kv`.  q8_layers = 0: all bf16.
+  uint8_t* q8_codes;
+  bf16 *q8_scales, *q8_biases;
+  int q8_gs, q8_layers;
 };
+// one 8-bit lock-step attention on caller buffers (b200_batch_kvq_attention): qkv (B, (n_heads + 2 n_kv) hd) fp32
+// finished-but-unbiased rows, the layer's 8-bit planes (2, pool_rows, n_kv, cap, ...) and per-row ctx / pos (device)
+int batch_kvq_attention(const float* qkv, const bf16* bias, const float* inv_freq, const int* ctx, const int* pos,
+                        uint8_t* codes, bf16* scales, bf16* biases, int gs, int pool_rows, int cap, bf16* out, int B,
+                        int n_heads, int n_kv, int hd, const bf16* qn, const bf16* kn, float eps, int sm_count,
+                        cudaStream_t s);
 int batch_decoder_begin(void** handle, const BdModel& m, int B, const int* tok, const int* ctx, const int* pos,
                         const int* active, cudaStream_t s);
 int batch_decoder_step(void* handle, const BdModel& m, int n_steps, bool want_logprobs, cudaStream_t s,

@@ -8,7 +8,10 @@
 // replays unchanged while rows join and leave:
 //   per layer   qkv      gemm_wt (weight-major wgmma GEMM, token tile 16, split-K partials)
 //               bd_attn  finishes q/k/v from the partials (+bias, M-RoPE at the row's position,
-//                        KV append at the row's length) and attends over the row's keys
+//                        KV append at the row's length) and attends over the row's keys; on a layer
+//                        whose pool is 8-bit (kv_bits=8, format kvq.cuh) the same kernel quantizes the
+//                        new row, appends its codes / scales / biases and attends over the dequantized
+//                        keys and values, the new row included
 //               o_proj   gemm_wt partials -> finish_rows (+residual, RMSNorm)
 //               gate/up  gemm_wt with the SwiGLU epilogue
 //               down     gemm_wt partials -> finish_rows (+residual, next RMSNorm)
@@ -20,6 +23,7 @@
 
 #include "common.cuh"
 #include "decode.cuh"
+#include "kvq.cuh"
 
 namespace b200 {
 
@@ -96,9 +100,67 @@ struct BdAttnP {
   // leaves HBM idle, so its CTAs ask the L2 for them up front (l2_prefetch_span; weights are static during a step)
   const void* pf[3];
   long pf_bytes[3];
+  // 8-bit layer (Q8 variant): the layer's K codes / scales / biases of row 0.  Codes sit at the same element
+  // offsets as the bf16 planes (row_stride, v_off); scales and biases at those offsets / gs.
+  uint8_t* q8c;
+  bf16 *q8s, *q8b;
+  int gs;
 };
 
-template <int HD, int AG>
+// 8 codes -> their dequantized values (bf16 exactly: kvq_dequant rounds), packed as 8 bf16
+__device__ __forceinline__ uint4 bd_q8_unpack8(uint2 w, float s, float b) {
+  float f[8];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    f[e] = kvq_dequant((w.x >> (8 * e)) & 0xffu, s, b);
+    f[4 + e] = kvq_dequant((w.y >> (8 * e)) & 0xffu, s, b);
+  }
+  uint4 o;
+  o.x = pack2(f[0], f[1]); o.y = pack2(f[2], f[3]); o.z = pack2(f[4], f[5]); o.w = pack2(f[6], f[7]);
+  return o;
+}
+
+// key j of an 8-bit K plane (HD codes, HD / gs scales per position), dequantized into the bf16 layout of a key row
+template <int HD>
+__device__ __forceinline__ void bd_q8_key(const uint8_t* codes, const bf16* sc, const bf16* bi, int gs, long j,
+                                          uint4 (&kv)[HD / 8]) {
+  constexpr int NG = HD / 32;   // most groups per position (gs = 32)
+  const int ng = HD / gs;
+  float s[NG], b[NG];
+#pragma unroll
+  for (int g = 0; g < NG; ++g) {
+    s[g] = g < ng ? bf2f(__ldcg(sc + j * ng + g)) : 0.f;
+    b[g] = g < ng ? bf2f(__ldcg(bi + j * ng + g)) : 0.f;
+  }
+  const uint2* c = reinterpret_cast<const uint2*>(codes + j * HD);
+#pragma unroll
+  for (int ch = 0; ch < HD / 8; ++ch) {
+    const int g = ch * 8 / gs;
+    float sg = s[0], bg = b[0];
+#pragma unroll
+    for (int t = 1; t < NG; ++t)
+      if (g == t) { sg = s[t]; bg = b[t]; }
+    kv[ch] = bd_q8_unpack8(__ldcg(c + ch), sg, bg);
+  }
+}
+
+// the 8 * NV codes of dims [d0, d0 + 8 * NV) of value j of an 8-bit V plane (NV = 1: in .x / .y) and the scale / bias
+// of their quantization group (8 * NV divides gs); dequantized where they are used
+template <int HD, int NV>
+__device__ __forceinline__ void bd_q8_val(const uint8_t* codes, const bf16* sc, const bf16* bi, int gs, long j, int d0,
+                                          uint4& c, float& s, float& b) {
+  const long si = j * (HD / gs) + d0 / gs;
+  s = bf2f(__ldcg(sc + si));
+  b = bf2f(__ldcg(bi + si));
+  if constexpr (NV == 2) {
+    c = __ldcg(reinterpret_cast<const uint4*>(codes + j * HD + d0));
+  } else {
+    const uint2 w = __ldcg(reinterpret_cast<const uint2*>(codes + j * HD + d0));
+    c = make_uint4(w.x, w.y, 0u, 0u);
+  }
+}
+
+template <int HD, int AG, bool Q8>
 __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   bd_pdl_launch();
   if (threadIdx.x == 0) {
@@ -126,8 +188,16 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   const int kvh = blockIdx.x / p.hsplit, part = blockIdx.x % p.hsplit;
   const int G = min(Gc, Gall - part * Gc);
   const int h0 = kvh * Gall + part * Gc;
-  bf16* kb = p.kv + (long)row * p.row_stride + (long)kvh * p.cap * HD;
-  bf16* vb = kb + p.v_off;
+  const long plane0 = (long)row * p.row_stride + (long)kvh * p.cap * HD;   // element offset of this row's K plane
+  bf16* kb = Q8 ? nullptr : p.kv + plane0;
+  bf16* vb = Q8 ? nullptr : kb + p.v_off;
+  // Q8: codes at the same element offsets, scales / biases at offsets / gs
+  const uint8_t* kq = Q8 ? p.q8c + plane0 : nullptr;
+  const uint8_t* vq = Q8 ? kq + p.v_off : nullptr;
+  const bf16* kqs = Q8 ? p.q8s + plane0 / p.gs : nullptr;
+  const bf16* kqb = Q8 ? p.q8b + plane0 / p.gs : nullptr;
+  const bf16* vqs = Q8 ? kqs + p.v_off / p.gs : nullptr;
+  const bf16* vqb = Q8 ? kqb + p.v_off / p.gs : nullptr;
   bd_pdl_wait();
   const int ctx = p.ctx[row], pos = p.pos[row];
   const int nkeys = ctx + 1;
@@ -136,10 +206,13 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   // split-K partials of q/k/v are summed, the first block of values before the softmax.
   uint4 kfirst[NCH];
   {
-    const int j = warp * 32 + lane;
-    const uint4* kr = reinterpret_cast<const uint4*>(kb + (long)j * HD);
+    // (the 8-bit variant loads its first keys in the score loop: holding them dequantized across the sums spills)
+    if constexpr (!Q8) {
+      const int j = warp * 32 + lane;
+      const uint4* kr = reinterpret_cast<const uint4*>(kb + (long)j * HD);
 #pragma unroll
-    for (int c = 0; c < NCH; ++c) kfirst[c] = (j < ctx) ? __ldcg(kr + c) : make_uint4(0, 0, 0, 0);
+      for (int c = 0; c < NCH; ++c) kfirst[c] = (j < ctx) ? __ldcg(kr + c) : make_uint4(0, 0, 0, 0);
+    }
   }
   // ---- finish q (G heads), k, v of this step: sum of the split-K partials + bias, one rounding ----
   for (int i = threadIdx.x; i < (G + 2) * HD; i += 256) {
@@ -188,7 +261,37 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   }
   for (int i = threadIdx.x + G * HD; i < AG * HD; i += 256) qs[i] = 0.f;
   __syncthreads();
-  if (part == 0) {  // append the new position to the row's cache (one CTA per kv head)
+  if constexpr (Q8) {
+    // quantize the new K and V row (warp w < 2 * ng: group w % ng of K, then of V) with the format's own
+    // arithmetic, append it (one CTA per kv head), and attend to its dequantized values from here on
+    const int ng = HD / p.gs, E = p.gs >> 5;
+    if (warp < 2 * ng) {
+      const int side = warp / ng, g = warp % ng;
+      float* src = (side ? vn : kn) + g * p.gs + lane * E;
+      float w[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) w[e] = e < E ? src[e] : 0.f;
+      uint32_t code[4];
+      float scale, bias;
+      kvq_quantize_group(w, E, code, &scale, &bias);
+      const float sb = rbf(scale), bb = rbf(bias);
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (e < E) src[e] = kvq_dequant(code[e], sb, bb);
+      if (part == 0) {
+        const long at = plane0 + (side ? p.v_off : 0) + (long)ctx * HD;
+        uint8_t* c = p.q8c + at + g * p.gs + lane * E;
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (e < E) c[e] = (uint8_t)code[e];
+        if (lane == 0) {
+          p.q8s[at / p.gs + g] = f2bf(scale);
+          p.q8b[at / p.gs + g] = f2bf(bias);
+        }
+      }
+    }
+    __syncthreads();
+  } else if (part == 0) {  // append the new position to the row's cache (one CTA per kv head)
     for (int i = threadIdx.x; i < HD; i += 256) {
       kb[(long)ctx * HD + i] = f2bf(kn[i]);
       vb[(long)ctx * HD + i] = f2bf(vn[i]);
@@ -201,13 +304,17 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   for (int j0 = warp * 32; j0 < nkeys; j0 += 256) {
     const int j = j0 + lane;
     uint4 kv[NCH];
-    if (j0 == warp * 32) {
+    if (!Q8 && j0 == warp * 32) {
 #pragma unroll
       for (int c = 0; c < NCH; ++c) kv[c] = kfirst[c];
     } else if (j < ctx) {
-      const uint4* kr = reinterpret_cast<const uint4*>(kb + (long)j * HD);
+      if constexpr (Q8) {
+        bd_q8_key<HD>(kq, kqs, kqb, p.gs, j, kv);
+      } else {
+        const uint4* kr = reinterpret_cast<const uint4*>(kb + (long)j * HD);
 #pragma unroll
-      for (int c = 0; c < NCH; ++c) kv[c] = __ldcg(kr + c);
+        for (int c = 0; c < NCH; ++c) kv[c] = __ldcg(kr + c);
+      }
     }
     if (j < nkeys) {
       if (j == ctx) {
@@ -242,14 +349,21 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   }
   // first block of values: warp w, trip q, key = 32 * w + 4 * q + ksub; lane = (ksub, dim segment)
   const int seg = lane & 7, ksub = lane >> 3;
+  static_assert(NV <= 2, "one 16-byte code word per lane and key");
   uint4 vfirst[VU][NV];
+  uint4 vfc[VU];            // 8-bit variant: codes and group scale / bias of the first block of values
+  float vfs[VU], vfb[VU];
 #pragma unroll
   for (int q = 0; q < VU; ++q) {
     const int j = warp * 32 + q * 4 + ksub;
+    if constexpr (Q8) {
+      if (j < ctx) bd_q8_val<HD, NV>(vq, vqs, vqb, p.gs, j, seg * SEG, vfc[q], vfs[q], vfb[q]);
+    } else {
 #pragma unroll
-    for (int v = 0; v < NV; ++v)
-      vfirst[q][v] = (j < ctx) ? __ldcg(reinterpret_cast<const uint4*>(vb + (long)j * HD + seg * SEG + v * 8))
-                               : make_uint4(0, 0, 0, 0);
+      for (int v = 0; v < NV; ++v)
+        vfirst[q][v] = (j < ctx) ? __ldcg(reinterpret_cast<const uint4*>(vb + (long)j * HD + seg * SEG + v * 8))
+                                 : make_uint4(0, 0, 0, 0);
+    }
   }
 #pragma unroll
   for (int g = 0; g < AG; ++g) {
@@ -301,14 +415,24 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
     for (int e = 0; e < SEG; ++e) acc[g][e] = 0.f;
   for (int j0 = 0; j0 < nkeys; j0 += 256) {
     uint4 vv[VU][NV];
+    uint4 vc[VU];
+    float vs[VU], vbi[VU];
 #pragma unroll
     for (int q = 0; q < VU; ++q) {
       const int j = j0 + warp * 32 + q * 4 + ksub;
+      if constexpr (Q8) {
+        if (j0 == 0) {
+          vc[q] = vfc[q]; vs[q] = vfs[q]; vbi[q] = vfb[q];
+        } else if (j < ctx) {
+          bd_q8_val<HD, NV>(vq, vqs, vqb, p.gs, j, seg * SEG, vc[q], vs[q], vbi[q]);
+        }
+      } else {
 #pragma unroll
-      for (int v = 0; v < NV; ++v) {
-        if (j0 == 0) vv[q][v] = vfirst[q][v];
-        else vv[q][v] = (j < ctx) ? __ldcg(reinterpret_cast<const uint4*>(vb + (long)j * HD + seg * SEG + v * 8))
-                                  : make_uint4(0, 0, 0, 0);
+        for (int v = 0; v < NV; ++v) {
+          if (j0 == 0) vv[q][v] = vfirst[q][v];
+          else vv[q][v] = (j < ctx) ? __ldcg(reinterpret_cast<const uint4*>(vb + (long)j * HD + seg * SEG + v * 8))
+                                    : make_uint4(0, 0, 0, 0);
+        }
       }
     }
 #pragma unroll
@@ -324,6 +448,13 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
           if (j == ctx) {
 #pragma unroll
             for (int e = 0; e < 8; ++e) vf[e] = rbf(vn[seg * SEG + v * 8 + e]);
+          } else if constexpr (Q8) {
+            const uint32_t w0 = v ? vc[q].z : vc[q].x, w1 = v ? vc[q].w : vc[q].y;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              vf[e] = kvq_dequant((w0 >> (8 * e)) & 0xffu, vs[q], vbi[q]);
+              vf[4 + e] = kvq_dequant((w1 >> (8 * e)) & 0xffu, vs[q], vbi[q]);
+            }
           } else {
             unpack8(vv[q][v], vf);
           }
@@ -484,6 +615,8 @@ struct BatchDecoder {
   int* stage_host = nullptr;  // pinned [4][max_b]
   cudaGraphExec_t gexec = nullptr;
   const void* graph_kv = nullptr;
+  const void* graph_q8 = nullptr;
+  int graph_q8_layers = 0, graph_gs = 0;
   int graph_B = 0, graph_cap = 0, graph_lp = 0;
   long steps_done = 0;
   bool want_logprobs = false;
@@ -558,13 +691,32 @@ static int bd_attn_heads_per_cta(const DecodeDims& d, int B, int sm_count) {
   return BD_AG_MAX;
 }
 
-template <int HD>
+template <int HD, bool Q8>
 static int bd_attn_launch(int ag, dim3 grid, size_t smem, cudaStream_t s, const BdAttnP& ap) {
   switch (ag) {
-    case 1: return bd_launch(bd_attn_kernel<HD, 1>, grid, dim3(256), smem, s, ap);
-    case 2: return bd_launch(bd_attn_kernel<HD, 2>, grid, dim3(256), smem, s, ap);
-    default: return bd_launch(bd_attn_kernel<HD, 4>, grid, dim3(256), smem, s, ap);
+    case 1: return bd_launch(bd_attn_kernel<HD, 1, Q8>, grid, dim3(256), smem, s, ap);
+    case 2: return bd_launch(bd_attn_kernel<HD, 2, Q8>, grid, dim3(256), smem, s, ap);
+    default: return bd_launch(bd_attn_kernel<HD, 4, Q8>, grid, dim3(256), smem, s, ap);
   }
+}
+
+static int bd_attn_dispatch(const DecodeDims& d, int ag, dim3 grid, cudaStream_t s, const BdAttnP& ap, bool q8) {
+  const size_t smem = bd_attn_smem(d, ag);
+  if (d.hd == 128) return q8 ? bd_attn_launch<128, true>(ag, grid, smem, s, ap) : bd_attn_launch<128, false>(ag, grid, smem, s, ap);
+  return q8 ? bd_attn_launch<64, true>(ag, grid, smem, s, ap) : bd_attn_launch<64, false>(ag, grid, smem, s, ap);
+}
+
+static int bd_set_smem_attrs() {
+  static unsigned long long attr_mask = 0ull;
+  if (!first_use_on_device(&attr_mask)) return B200_OK;
+  const void* ks[] = {(const void*)bd_attn_kernel<128, 1, false>, (const void*)bd_attn_kernel<128, 2, false>,
+                      (const void*)bd_attn_kernel<128, 4, false>, (const void*)bd_attn_kernel<64, 1, false>,
+                      (const void*)bd_attn_kernel<64, 2, false>,  (const void*)bd_attn_kernel<64, 4, false>,
+                      (const void*)bd_attn_kernel<128, 1, true>,  (const void*)bd_attn_kernel<128, 2, true>,
+                      (const void*)bd_attn_kernel<128, 4, true>,  (const void*)bd_attn_kernel<64, 1, true>,
+                      (const void*)bd_attn_kernel<64, 2, true>,   (const void*)bd_attn_kernel<64, 4, true>};
+  for (const void* k : ks) B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  return B200_OK;
 }
 
 // L2 prefetch budget of the latency-bound kernels of a step, in bytes (B200_BD_PREFETCH_MB).  DEFAULT 0 = off: the
@@ -599,7 +751,13 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
       return rc;
     BdAttnP ap;
     ap.P = d->partial; ap.S = split; ap.B = B; ap.QKV = QKV; ap.bias = lw.bqkv; ap.inv_freq = m.inv_freq;
-    ap.ctx = d->ctx; ap.pos = d->pos; ap.kv = m.kv + (long)l * m.layer_stride; ap.v_off = m.v_off;
+    const bool q8 = l < m.q8_layers;
+    ap.ctx = d->ctx; ap.pos = d->pos; ap.v_off = m.v_off;
+    ap.kv = q8 ? nullptr : m.kv + (long)(l - m.q8_layers) * m.layer_stride;
+    ap.q8c = q8 ? m.q8_codes + (long)l * m.layer_stride : nullptr;
+    ap.q8s = q8 ? m.q8_scales + (long)l * m.layer_stride / m.q8_gs : nullptr;
+    ap.q8b = q8 ? m.q8_biases + (long)l * m.layer_stride / m.q8_gs : nullptr;
+    ap.gs = q8 ? m.q8_gs : 0;
     ap.row_stride = m.row_stride; ap.out = d->att; ap.n_heads = dd.n_heads; ap.n_kv = dd.n_kv; ap.cap = dd.cap;
     ap.hsplit = hs; ap.scale_bf = dd.scale_bf;
     ap.qn = m.qn ? m.qn[l] : nullptr; ap.kn = m.kn ? m.kn[l] : nullptr; ap.eps = dd.eps;
@@ -613,10 +771,7 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
         left -= ap.pf_bytes[i];
       }
     }
-    const dim3 ag(dd.n_kv * hs, B);
-    if (dd.hd == 128) rc = bd_attn_launch<128>(ag_heads, ag, bd_attn_smem(dd, ag_heads), s, ap);
-    else rc = bd_attn_launch<64>(ag_heads, ag, bd_attn_smem(dd, ag_heads), s, ap);
-    if (rc) return rc;
+    if ((rc = bd_attn_dispatch(dd, ag_heads, dim3(dd.n_kv * hs, B), s, ap, q8))) return rc;
     if ((rc = gemm_wt_tuned(d->att, QH, lw.wo, nullptr, nullptr, 0, nullptr, 0, d->partial, d->partial_bytes, B, H, QH,
                             B200_EPI_NONE, B200_WT_PARTIAL, 0, true, m.sm_count, &split, s)))
       return rc;
@@ -666,15 +821,7 @@ int batch_decoder_begin(void** handle, const BdModel& m, int B, const int* tok, 
       return rc;
     }
     *handle = d;
-    static unsigned long long attr_mask = 0ull;
-    if (first_use_on_device(&attr_mask)) {
-      B200_CUDA(cudaFuncSetAttribute(bd_attn_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      B200_CUDA(cudaFuncSetAttribute(bd_attn_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      B200_CUDA(cudaFuncSetAttribute(bd_attn_kernel<128, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      B200_CUDA(cudaFuncSetAttribute(bd_attn_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      B200_CUDA(cudaFuncSetAttribute(bd_attn_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      B200_CUDA(cudaFuncSetAttribute(bd_attn_kernel<64, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    }
+    if ((rc = bd_set_smem_attrs())) return rc;
   }
   d->B = B;
   for (int b = 0; b < B; ++b) {
@@ -705,7 +852,8 @@ int batch_decoder_step(void* handle, const BdModel& m, int n_steps, bool want_lo
   int rc;
   int done = 0;
   const bool stale = !d->gexec || d->graph_kv != m.kv || d->graph_B != d->B || d->graph_cap != m.d.cap ||
-                     d->graph_lp != (int)want_logprobs;
+                     d->graph_lp != (int)want_logprobs || d->graph_q8 != m.q8_codes ||
+                     d->graph_q8_layers != m.q8_layers || d->graph_gs != m.q8_gs;
   if (stale) {
     if (d->gexec) {
       cudaGraphExecDestroy(d->gexec);
@@ -729,6 +877,7 @@ int batch_decoder_step(void* handle, const BdModel& m, int n_steps, bool want_lo
       cudaGraphDestroy(graph);
       if (ce != cudaSuccess) return cuda_fail(ce, "cudaGraphInstantiate(batch step)", __FILE__, __LINE__);
       d->graph_kv = m.kv; d->graph_B = d->B; d->graph_cap = m.d.cap; d->graph_lp = (int)want_logprobs;
+      d->graph_q8 = m.q8_codes; d->graph_q8_layers = m.q8_layers; d->graph_gs = m.q8_gs;
     }
   }
   for (int i = done; i < n_steps; ++i) B200_CUDA(cudaGraphLaunch(d->gexec, s));
@@ -747,6 +896,30 @@ int batch_decoder_fetch(void* handle, long first_step, int n_steps, int* tok_hos
     B200_CUDA(cudaMemcpy2DAsync(lp_host, (size_t)d->B * 4, d->lp_log + first_step * d->max_b, (size_t)d->max_b * 4,
                                 (size_t)d->B * 4, n_steps, cudaMemcpyDeviceToHost, s));
   return B200_OK;
+}
+
+int batch_kvq_attention(const float* qkv, const bf16* bias, const float* inv_freq, const int* ctx, const int* pos,
+                        uint8_t* codes, bf16* scales, bf16* biases, int gs, int pool_rows, int cap, bf16* out, int B,
+                        int n_heads, int n_kv, int hd, const bf16* qn, const bf16* kn, float eps, int sm_count,
+                        cudaStream_t s) {
+  B200_REQUIRE(hd == 64 || hd == 128, "batch kvq attention: head_dim %d (64|128)", hd);
+  B200_REQUIRE((gs == 32 || gs == 64 || gs == 128) && hd % gs == 0, "batch kvq attention: group size %d", gs);
+  B200_REQUIRE(B >= 1 && B <= pool_rows && n_kv > 0 && n_heads % n_kv == 0, "batch kvq attention: bad arguments");
+  DecodeDims d = {};
+  d.n_heads = n_heads; d.n_kv = n_kv; d.hd = hd; d.cap = cap; d.eps = eps;
+  d.scale_bf = __bfloat162float(__float2bfloat16_rn(1.0f / sqrtf((float)hd)));
+  B200_REQUIRE(bd_attn_smem(d, BD_AG_MAX) <= 200 * 1024, "batch kvq attention: capacity %d too large", cap);
+  int rc = bd_set_smem_attrs();
+  if (rc) return rc;
+  const int ag_heads = bd_attn_heads_per_cta(d, B, sm_count);
+  const int hs = (n_heads / n_kv + ag_heads - 1) / ag_heads;
+  BdAttnP ap = {};
+  ap.P = qkv; ap.S = 1; ap.B = B; ap.QKV = (n_heads + 2 * n_kv) * hd; ap.bias = bias; ap.inv_freq = inv_freq;
+  ap.ctx = ctx; ap.pos = pos; ap.row_stride = (long)n_kv * cap * hd; ap.v_off = (long)pool_rows * ap.row_stride;
+  ap.out = out; ap.n_heads = n_heads; ap.n_kv = n_kv; ap.cap = cap; ap.hsplit = hs; ap.scale_bf = d.scale_bf;
+  ap.qn = qn; ap.kn = kn; ap.eps = eps;
+  ap.q8c = codes; ap.q8s = scales; ap.q8b = biases; ap.gs = gs;
+  return bd_attn_dispatch(d, ag_heads, dim3(n_kv * hs, B), s, ap, true);
 }
 
 const void* batch_decoder_buffer(void* handle, int which) {

@@ -61,6 +61,13 @@ struct b200_engine {
   // [2][n_kv][cap][hd] where the decode QKV kernel leaves the new K/V row before it is quantized
   KvqPlanes q8 = {};
   KvqPlanes pre_q8 = {};  // b200_engine_set_prefill_kvq: prefill writes its rows through to this 8-bit pool
+  // b200_engine_set_prefill_kvq_row: the write-through pool is a batch pool of its own geometry (pre_rows x pre_cap,
+  // target row pre_row) holding layers 0 .. pre_layers-1 only; pre_layers = 0: the bound pool's geometry, every layer
+  int pre_rows = 0, pre_cap = 0, pre_row = 0, pre_layers = 0;
+  // b200_engine_bind_batch_kvq: the lock-step batch pool of kv_bits=8.  Layers 0 .. bq8_layers-1 in this 8-bit pool,
+  // the others in the bf16 pool `kv` (nullptr when every layer is 8-bit)
+  KvqPlanes bq8 = {};
+  int bq8_layers = 0;
   bf16* q8_stage = nullptr;
   long q8_stage_elems = 0;
   void* batch = nullptr; // lock-step batched decoder (decode_batch.cu)
@@ -148,6 +155,17 @@ struct b200_engine {
   }
   bf16* vptr(int layer, int row) const {
     return kv + (((long)layer * 2 + 1) * kv_batch + row) * cfg.n_kv_heads * (long)kv_cap * cfg.head_dim;
+  }
+  bool pre_q8_layer(int layer) const { return pre_q8.codes && (pre_layers == 0 || layer < pre_layers); }
+  int pre_q8_cap() const { return pre_layers ? pre_cap : kv_cap; }
+  KvqPlanes pre_q8_plane(int layer, int side) const {
+    if (!pre_layers) return q8_plane(layer, side, kv_row, pre_q8);
+    const long plane = (((long)layer * 2 + side) * pre_rows + pre_row) * cfg.n_kv_heads;
+    KvqPlanes p = pre_q8;
+    p.codes += plane * pre_cap * cfg.head_dim;
+    p.scales += plane * pre_cap * (cfg.head_dim / pre_q8.gs);
+    p.biases += plane * pre_cap * (cfg.head_dim / pre_q8.gs);
+    return p;
   }
   KvqPlanes q8_plane(int layer, int side, int row, const KvqPlanes& pool) const {
     const long plane = (((long)layer * 2 + side) * kv_batch + row) * cfg.n_kv_heads;
@@ -775,10 +793,10 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
                              c.n_kv_heads, hd, s, fa ? scale_bf : 0.f, fa ? vt : nullptr, t_ld,
                              fa ? e->kvref : nullptr, l, fa ? kws : nullptr)))
       return rc;
-    if (e->pre_q8.codes) {  // an 8-bit cache: the chunk's rows are quantized before they are attended
-      if ((rc = kvq_quantize_rows(kc, e->kv_cap, e->q8_plane(l, 0, e->kv_row, e->pre_q8), c.n_kv_heads, ctx0, T, hd,
+    if (e->pre_q8_layer(l)) {  // an 8-bit layer: the chunk's rows are quantized before they are attended
+      if ((rc = kvq_quantize_rows(kc, e->kv_cap, e->pre_q8_plane(l, 0), e->pre_q8_cap(), c.n_kv_heads, ctx0, T, hd,
                                   true, s)) ||
-          (rc = kvq_quantize_rows(vc, e->kv_cap, e->q8_plane(l, 1, e->kv_row, e->pre_q8), c.n_kv_heads, ctx0, T, hd,
+          (rc = kvq_quantize_rows(vc, e->kv_cap, e->pre_q8_plane(l, 1), e->pre_q8_cap(), c.n_kv_heads, ctx0, T, hd,
                                   true, s)))
         return rc;
       e->launches += 2;
@@ -1012,11 +1030,58 @@ int b200_engine_bind_kv(b200_engine* e, void* pool, int batch, int cap) {
   e->kv_cap = cap;
   e->q8 = KvqPlanes{};
   e->pre_q8 = KvqPlanes{};
+  e->pre_layers = 0;
+  e->bq8 = KvqPlanes{};
+  e->bq8_layers = 0;
+  return B200_OK;
+}
+
+int b200_engine_bind_batch_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int n_q8_layers,
+                               void* bf16_pool, int batch, int cap) {
+  B200_REQUIRE(e && codes && scales && biases && batch >= 1 && cap >= 1 && ((uintptr_t)codes & 15) == 0 &&
+                   ((uintptr_t)bf16_pool & 15) == 0,
+               "bind_batch_kvq: bad arguments");
+  const auto& c = e->cfg;
+  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && c.head_dim % group_size == 0,
+               "bind_batch_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size, c.head_dim);
+  B200_REQUIRE(n_q8_layers >= 1 && n_q8_layers <= c.n_layers && (bf16_pool != nullptr) == (n_q8_layers < c.n_layers),
+               "bind_batch_kvq: %d of %d layers 8-bit needs a bf16 pool for the rest (and only then)", n_q8_layers,
+               c.n_layers);
+  B200_REQUIRE(e->kv_row < batch, "bind_batch_kvq: bound row %d of %d", e->kv_row, batch);
+  if (bf16_pool != e->kv || batch != e->kv_batch || cap != e->kv_cap || e->q8.codes) invalidate_graph(e);
+  e->kv = (bf16*)bf16_pool;
+  e->kv_batch = batch;
+  e->kv_cap = cap;
+  e->q8 = KvqPlanes{};
+  e->pre_q8 = KvqPlanes{};
+  e->pre_layers = 0;
+  e->bq8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
+  e->bq8_layers = n_q8_layers;
+  return B200_OK;
+}
+
+int b200_engine_set_prefill_kvq_row(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int rows,
+                                    int cap, int row, int n_q8_layers) {
+  B200_REQUIRE(e && codes && scales && biases && rows >= 1 && cap >= 1 && row >= 0 && row < rows,
+               "set_prefill_kvq_row: bad arguments");
+  B200_REQUIRE(n_q8_layers >= 1 && n_q8_layers <= e->cfg.n_layers, "set_prefill_kvq_row: %d 8-bit layers of %d",
+               n_q8_layers, e->cfg.n_layers);
+  B200_REQUIRE(e->kv && e->v2, "set_prefill_kvq_row: bind the bf16 pool first / round-1 prefill selected");
+  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && e->cfg.head_dim % group_size == 0,
+               "set_prefill_kvq_row: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size,
+               e->cfg.head_dim);
+  // every argument is checked: only now does the engine state change
+  e->pre_q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
+  e->pre_rows = rows;
+  e->pre_cap = cap;
+  e->pre_row = row;
+  e->pre_layers = n_q8_layers;
   return B200_OK;
 }
 
 int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size) {
   B200_REQUIRE(e, "set_prefill_kvq: null engine");
+  e->pre_layers = 0;
   if (!codes) {
     e->pre_q8 = KvqPlanes{};
     return B200_OK;
@@ -1050,6 +1115,8 @@ int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases
   e->kv = nullptr;
   e->kv_batch = batch;
   e->kv_cap = cap;
+  e->bq8 = KvqPlanes{};
+  e->bq8_layers = 0;
   e->q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
   return B200_OK;
 }
@@ -1151,9 +1218,11 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   B200_REQUIRE(e && embeds && pos3 && T > 0 && ctx0 >= 0, "engine_prefill: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv, "engine_prefill: KV pool not bound");
+  B200_REQUIRE(e->kv && !e->bq8.codes, "engine_prefill: KV pool not bound (a lock-step 8-bit batch pool is decode-only)");
   B200_REQUIRE(ctx0 + T <= e->kv_cap, "engine_prefill: ctx0+T=%d exceeds cache capacity %d",
                ctx0 + T, e->kv_cap);
+  B200_REQUIRE(!e->pre_q8.codes || !e->pre_layers || ctx0 + T <= e->pre_cap,
+               "engine_prefill: ctx0+T=%d exceeds the capacity %d of the 8-bit write-through pool", ctx0 + T, e->pre_cap);
   B200_REQUIRE(e->ws && b200_engine_workspace_bytes(e, T, 1) <= e->ws_bytes,
                "engine_prefill: workspace too small for %d tokens", T);
   B200_CUDA(cudaSetDevice(e->device));
@@ -1244,7 +1313,8 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_REQUIRE(e && embeds && pos3 && n_seq > 0 && seq_len && rows, "engine_prefill_batch: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv && e->v2, "engine_prefill_batch: KV pool not bound / round-1 prefill kernels selected");
+  B200_REQUIRE(e->kv && !e->bq8.codes && e->v2,
+               "engine_prefill_batch: KV pool not bound / 8-bit batch pool bound / round-1 prefill kernels selected");
   B200_REQUIRE(!e->pre_q8.codes, "engine_prefill_batch: no 8-bit write-through in the batched prefill");
   long T = 0;
   std::vector<PreSeg> segs(n_seq);
@@ -1318,7 +1388,8 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   B200_REQUIRE(e && n_steps > 0, "engine_decode: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv || e->q8.codes, "engine_decode: KV pool not bound");
+  B200_REQUIRE((e->kv || e->q8.codes) && !e->bq8.codes, "engine_decode: KV pool not bound (a lock-step 8-bit batch pool "
+               "serves b200_batch_decode only)");
   B200_REQUIRE(e->ctx_host + n_steps <= e->kv_cap,
                "engine_decode: %d cached + %d steps exceeds cache capacity %d", e->ctx_host,
                n_steps, e->kv_cap);
@@ -1483,7 +1554,7 @@ static void bd_model(b200_engine* e, BdModel* m) {
   m->layers = e->layers.data();
   m->embed = e->embed; m->head = e->head; m->final_norm = e->norm;
   m->inv_freq = e->lm_inv_freq;
-  m->kv = e->kptr(0, 0);
+  m->kv = e->kv;
   m->row_stride = (long)c.n_kv_heads * e->kv_cap * c.head_dim;
   m->v_off = (long)e->kv_batch * m->row_stride;
   m->layer_stride = 2L * m->v_off;
@@ -1491,6 +1562,8 @@ static void bd_model(b200_engine* e, BdModel* m) {
   m->sm_count = e->sm_count;
   m->qn = e->qk_norm ? e->qn.data() : nullptr;
   m->kn = e->qk_norm ? e->kn.data() : nullptr;
+  m->q8_codes = e->bq8.codes; m->q8_scales = e->bq8.scales; m->q8_biases = e->bq8.biases;
+  m->q8_gs = e->bq8.gs; m->q8_layers = e->bq8_layers;
 }
 
 int b200_batch_begin(b200_engine* e, int B, const int* tok, const int* ctx, const int* pos, const int* active,
@@ -1498,7 +1571,7 @@ int b200_batch_begin(b200_engine* e, int B, const int* tok, const int* ctx, cons
   B200_REQUIRE(e && tok && ctx && pos && active, "batch_begin: null argument");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv, "batch_begin: KV pool not bound");
+  B200_REQUIRE(e->kv || e->bq8.codes, "batch_begin: KV pool not bound");
   B200_CUDA(cudaSetDevice(e->device));
   BdModel m;
   bd_model(e, &m);

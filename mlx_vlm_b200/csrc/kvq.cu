@@ -50,11 +50,11 @@ __global__ void __launch_bounds__(256) k_kvq_quantize(const bf16* src, int src_c
   }
 }
 
-int kvq_quantize_rows(bf16* src, int cap, const KvqPlanes& dst, long planes, int pos0, int n, int hd, bool writeback,
-                      cudaStream_t s) {
+int kvq_quantize_rows(bf16* src, int cap, const KvqPlanes& dst, int dst_cap, long planes, int pos0, int n, int hd,
+                      bool writeback, cudaStream_t s) {
   const long groups = planes * n * (hd / dst.gs);
   if (groups == 0) return B200_OK;
-  k_kvq_quantize<<<(unsigned)((groups + 7) / 8), 256, 0, s>>>(src, cap, dst, cap, planes, n, hd, pos0,
+  k_kvq_quantize<<<(unsigned)((groups + 7) / 8), 256, 0, s>>>(src, cap, dst, dst_cap, planes, n, hd, pos0,
                                                                 writeback ? src : nullptr);
   B200_CHECK_LAUNCH();
   return B200_OK;
@@ -380,4 +380,38 @@ int b200_kvq_decode_attention(const void* qbuf, void* k_codes, void* k_scales, v
   if (rc) return rc;
   return cudaStreamSynchronize(s) == cudaSuccess ? B200_OK : cuda_fail(cudaGetLastError(), "kvq_decode_attention",
                                                                          __FILE__, __LINE__);
+}
+
+/* one 8-bit lock-step attention (the Q8 variant of bd_attn_kernel) on caller buffers; see include/b200vlm.h */
+int b200_batch_kvq_attention(const float* qkv, const void* bias, const float* inv_freq, const int* ctx, const int* pos,
+                             void* codes, void* scales, void* biases, int group_size, int pool_rows, int cap, void* out,
+                             int B, int n_heads, int n_kv, int head_dim, const void* q_norm, const void* k_norm, float eps,
+                             void* stream) {
+  B200_REQUIRE(qkv && bias && inv_freq && ctx && pos && codes && scales && biases && out && ((uintptr_t)codes & 15) == 0,
+               "batch_kvq_attention: bad arguments");
+  int dev = 0, sms = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  return batch_kvq_attention(qkv, (const bf16*)bias, inv_freq, ctx, pos, (uint8_t*)codes, (bf16*)scales, (bf16*)biases,
+                             group_size, pool_rows, cap, (bf16*)out, B, n_heads, n_kv, head_dim, (const bf16*)q_norm,
+                             (const bf16*)k_norm, eps, sms, (cudaStream_t)stream);
+}
+
+/* row copy of any per-position plane set (bf16 K/V, 8-bit codes, scales or biases): byte-exact */
+int b200_pool_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool, int src_batch,
+                       int src_cap, int src_row, int n_layers, int n_kv, int bytes_per_position, int n_tokens,
+                       void* stream) {
+  B200_REQUIRE(dst_pool && src_pool && dst_row >= 0 && dst_row < dst_batch && src_row >= 0 && src_row < src_batch &&
+                   n_tokens >= 0 && n_tokens <= dst_cap && n_tokens <= src_cap && bytes_per_position > 0,
+               "pool_copy_row: bad arguments");
+  if (n_tokens == 0) return B200_OK;
+  const size_t bp = (size_t)bytes_per_position, w = (size_t)n_tokens * bp;
+  for (int l = 0; l < n_layers; ++l)
+    for (int kv = 0; kv < 2; ++kv) {
+      const char* sp = (const char*)src_pool + ((((size_t)l * 2 + kv) * src_batch + src_row) * n_kv) * (size_t)src_cap * bp;
+      char* dp = (char*)dst_pool + ((((size_t)l * 2 + kv) * dst_batch + dst_row) * n_kv) * (size_t)dst_cap * bp;
+      B200_CUDA(cudaMemcpy2DAsync(dp, (size_t)dst_cap * bp, sp, (size_t)src_cap * bp, w, n_kv, cudaMemcpyDeviceToDevice,
+                                  (cudaStream_t)stream));
+    }
+  return B200_OK;
 }

@@ -73,10 +73,10 @@ __device__ __forceinline__ float kvq_dequant(uint32_t code, float scale, float b
 // the QKV kernel left the new row at position ctx.  Quantizes the new row, appends it to the pool and attends
 // over positions 0..ctx, the new one in its quantized form.
 int kvq_decode_prepare(const DecodeDims& d, int cluster);
-// quantize positions [pos0, pos0 + n) of `planes` bf16 planes (capacity cap, same as dst) into dst; writeback:
+// quantize positions [pos0, pos0 + n) of `planes` bf16 planes (capacity cap) into dst (capacity dst_cap); writeback:
 // replace those bf16 rows by their dequantized values
-int kvq_quantize_rows(bf16* src, int cap, const KvqPlanes& dst, long planes, int pos0, int n, int hd, bool writeback,
-                      cudaStream_t s);
+int kvq_quantize_rows(bf16* src, int cap, const KvqPlanes& dst, int dst_cap, long planes, int pos0, int n, int hd,
+                      bool writeback, cudaStream_t s);
 int launch_attn_q8(const DecodeDims& d, const bf16* qbuf, const KvqPlanes& kc8, const KvqPlanes& vc8,
                    const bf16* stage_k, const bf16* stage_v, bf16* out, const DecState* st, int cluster,
                    cudaStream_t s);

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _native as N
-from .models.cache import KVPool
+from .models.cache import BatchKVQPool, KVPool
 
 
 def _inv_freq(dim: int, base: float) -> np.ndarray:
@@ -99,6 +99,8 @@ class Engine:
     def bind_pool(self, pool: KVPool):
         # keyed on the device buffer itself (not id(pool): CPython reuses ids of collected pools);
         # the engine keeps a strong reference to the bound buffer so its address cannot be recycled
+        if isinstance(pool, BatchKVQPool):
+            return self.bind_batch_kvq(pool)
         self._check_pool_shape(pool)
         key = (pool.buf.data_ptr(), pool.batch, pool.capacity)
         if key != self._bound:
@@ -118,6 +120,28 @@ class Engine:
                                                   pool.group_size), "bind_kvq")
             self._bound = key
             self._bound_buf = (pool.codes, pool.scales, pool.biases)
+
+    def bind_batch_kvq(self, pool: BatchKVQPool):
+        """bind the lock-step batch pool of kv_bits=8 (8-bit layers + a bf16 last layer, models/cache.py
+        BatchKVQPool); see b200_engine_bind_batch_kvq"""
+        self._check_pool_shape(pool)
+        q, bf = pool.q, pool.bf
+        key = ("bq8", q.codes.data_ptr(), N.ptr(None if bf is None else bf.buf), pool.batch, pool.capacity,
+               pool.group_size)
+        if key != self._bound:
+            N.check(self.lib.b200_engine_bind_batch_kvq(self.h, q.codes.data_ptr(), q.scales.data_ptr(),
+                                                        q.biases.data_ptr(), pool.group_size, pool.n_q,
+                                                        N.ptr(None if bf is None else bf.buf), pool.batch,
+                                                        pool.capacity), "bind_batch_kvq")
+            self._bound = key
+            self._bound_buf = (q.codes, q.scales, q.biases, None if bf is None else bf.buf)
+
+    def set_prefill_kvq_row(self, pool: BatchKVQPool, row: int):
+        """the next prefill calls write the 8-bit layers' K/V rows through to row `row` of the batch pool"""
+        q = pool.q
+        N.check(self.lib.b200_engine_set_prefill_kvq_row(self.h, q.codes.data_ptr(), q.scales.data_ptr(),
+                                                         q.biases.data_ptr(), pool.group_size, pool.batch,
+                                                         pool.capacity, int(row), pool.n_q), "set_prefill_kvq_row")
 
     def set_prefill_kvq(self, pool):
         """prefill calls write their K/V rows through to this 8-bit pool (None: off); see b200_engine_set_prefill_kvq"""
@@ -205,7 +229,20 @@ class Engine:
         return self._view(p, self.BATCH_LOG_STEPS * self.BATCH_LOG_ROWS, torch.int32).view(self.BATCH_LOG_STEPS,
                                                                                         self.BATCH_LOG_ROWS)
 
+    def kvq_copy_row(self, dst, dst_row: int, src, src_row: int, n_tokens: int):
+        """row copy between 8-bit pools (QuantizedKVPool): codes, scales and biases, byte for byte"""
+        ng = src.hd // src.group_size
+        for plane, bpp in (("codes", src.hd), ("scales", 2 * ng), ("biases", 2 * ng)):
+            N.check(self.lib.b200_pool_copy_row(getattr(dst, plane).data_ptr(), dst.batch, dst.capacity, int(dst_row),
+                                                getattr(src, plane).data_ptr(), src.batch, src.capacity, int(src_row),
+                                                src.n_layers, src.n_kv, bpp, int(n_tokens), self.s), "pool_copy_row")
+
     def kv_copy_row(self, dst: KVPool, dst_row: int, src: KVPool, src_row: int, n_tokens: int):
+        if isinstance(dst, BatchKVQPool):   # the 8-bit layers, then the bf16 ones
+            self.kvq_copy_row(dst.q, dst_row, src.q, src_row, n_tokens)
+            if dst.bf is not None:
+                self.kv_copy_row(dst.bf, dst_row, src.bf, src_row, n_tokens)
+            return
         N.check(self.lib.b200_kv_copy_row(dst.buf.data_ptr(), dst.batch, dst.capacity, int(dst_row), src.buf.data_ptr(),
                                           src.batch, src.capacity, int(src_row), dst.n_layers, dst.n_kv, dst.hd,
                                           int(n_tokens), self.s), "kv_copy_row")

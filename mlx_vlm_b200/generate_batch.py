@@ -3,6 +3,10 @@
 `BatchGenerationResult` :519-545, `_left_pad_prompts` / `_right_pad_prompts` :548-560,
 `batch_generate` :2890-3097).
 
+With `kv_bits=8` the pool follows the reference's batch rule (`_make_cache`, ar.py:751-859): the layers where
+`should_quantize_kv_layer` holds are 8-bit from the first prefill on (models/cache.py `BatchKVQPool`), the last
+layer of a deeper stack stays bf16.
+
 How the rows run on the CUDA engine: LOCK STEP on the device (csrc/decode_batch.cu).  All active
 rows live in ONE batched KV pool (layers, 2, rows, kv heads, capacity, head_dim), each with its own
 length (no left padding); a decode step is one captured CUDA graph that streams the weights ONCE
@@ -172,10 +176,18 @@ class BatchGenerator:
                  prefill_batch_size: int = DEFAULT_PREFILL_BATCH_SIZE,
                  prefill_step_size: Optional[int] = None, compute_logprobs: bool = False,
                  top_logprobs_k: int = 0, logits_processors=None, greedy_sampling: bool = False,
-                 decode_slice: int = 16, batched_prefill: bool = True, **unsupported):
-        for k in ("kv_bits", "kv_key_bits", "kv_value_bits", "draft_model", "apc_manager", "prompt_cache"):
+                 decode_slice: int = 16, batched_prefill: bool = True, kv_bits=None, kv_group_size: int = 64,
+                 kv_quant_scheme: Optional[str] = None, quantized_kv_start: int = 0, **unsupported):
+        for k in ("kv_key_bits", "kv_value_bits", "draft_model", "apc_manager", "prompt_cache"):
             if unsupported.pop(k, None) is not None:
                 raise NotImplementedError(f"BatchGenerator: `{k}` is outside this engine's hot-path scope")
+        # kv_bits=8: the reference's batch rule (ar.py:751-859 `_make_cache`): every layer where
+        # `should_quantize_kv_layer` holds keeps an 8-bit cache from the first prefill on; `quantized_kv_start`
+        # plays no part in it (accepted for the reference's signature)
+        from .generate import kv_quant_args
+        self.kv_bits = kv_quant_args(kv_bits, kv_group_size, kv_quant_scheme,
+                                     getattr(getattr(model, "language_model", None), "head_dim", None) or 128)
+        self.kv_group_size = int(kv_group_size)
         if logits_processors:
             raise NotImplementedError("BatchGenerator: logits processors run on the single-request path only")
         if top_logprobs_k:
@@ -203,6 +215,11 @@ class BatchGenerator:
         self._lockstep = (hasattr(eng, "batch_begin") and hasattr(lm, "make_cache_row")
                           and getattr(lm, "lockstep_supported", True)
                           and not unsupported.pop("time_multiplex", False))
+        if self.kv_bits is not None and not self._lockstep:
+            raise NotImplementedError(
+                "BatchGenerator(kv_bits=8) runs in the lock-step batch only; this model / engine runs its rows "
+                "time-multiplexed over the single-request path (no batched decoder, or a Qwen3-VL head_dim other "
+                "than hidden / heads), whose 8-bit policy is the single-request one")
         if self._lockstep:
             self.completion_batch_size = min(self.completion_batch_size, 16)
         self._pool = None          # the shared batched KV pool (lock-step mode)
@@ -330,6 +347,8 @@ class BatchGenerator:
         row.last_token, row.n_decoded = tok, 1
         row.ctx = int(row.cache[0].offset)
         row.buffer.append((tok, lp))
+        if self.kv_bits is not None and self._lockstep:
+            self._pool._admit = None   # the bf16 pool of the admission (csrc: prefill write-through) is done
         dt = time.perf_counter() - tic
         self._prompt_tokens_counter += len(row.ids)
         self._prompt_time_counter += dt
@@ -389,7 +408,11 @@ class BatchGenerator:
         lm, eng = self.model.language_model, self.model.engine
         step = cache_mod.KVPool.step
         cap = ((need_tokens + step - 1) // step) * step
-        if self._pool is None:
+        if self._pool is None and self.kv_bits is not None:
+            self._pool = cache_mod.BatchKVQPool(lm.args.num_hidden_layers, lm.n_kv_heads, lm.head_dim, eng.device,
+                                                group_size=self.kv_group_size, batch=self.completion_batch_size,
+                                                capacity=cap, stream=eng.stream)
+        elif self._pool is None:
             self._pool = cache_mod.KVPool(lm.args.num_hidden_layers, lm.n_kv_heads, lm.head_dim, eng.device,
                                           batch=self.completion_batch_size, capacity=cap)
         elif cap > self._pool.capacity:
@@ -528,7 +551,9 @@ class BatchGenerator:
         n_admit = min(room, self.prefill_batch_size, len(self._unprocessed_sequences))
         admitted = []
         self._admitting = 0
+        # kv_bits=8 rows are admitted one at a time (the grouped prefill has no 8-bit write-through)
         group = (self._lockstep and n_admit >= 2 and self.greedy_sampling and not self.compute_logprobs
+                 and self.kv_bits is None
                  and hasattr(self.model.language_model, "prefill_rows") and self.batched_prefill
                  and (self.prefill_step_size is None
                       or all(len(r.ids) <= self.prefill_step_size + 1 for r in self._unprocessed_sequences[:n_admit])))

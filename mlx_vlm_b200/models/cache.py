@@ -140,6 +140,69 @@ def _stream_handle(pool) -> int:
     return s.cuda_stream
 
 
+def should_quantize_kv_layer(layer_idx: int, num_layers: int) -> bool:
+    """models/cache.py:8-21: the lock-step batch rule of kv_bits.  Stacks of more than two layers keep the last
+    layer in bf16; shallower stacks quantize every layer."""
+    if num_layers <= 2:
+        return True
+    return layer_idx < num_layers - 1
+
+
+class BatchKVQPool:
+    """The lock-step batch pool of kv_bits=8 (DESIGN §3).  The layers where `should_quantize_kv_layer` holds are a
+    prefix 0 .. n_q-1; they live in a `QuantizedKVPool` of n_q layers, the remaining layers in a bf16 `KVPool` of
+    n_layers - n_q layers (None when every layer is 8-bit).  Both have the same rows and capacity and grow together,
+    so an 8-bit layer takes no bf16 storage."""
+    step = 256
+    bits = 8
+
+    def __init__(self, n_layers: int, n_kv_heads: int, head_dim: int, device, group_size: int = 64, batch: int = 1,
+                 capacity: int = 0, stream=None):
+        self.n_layers, self.n_kv, self.hd = n_layers, n_kv_heads, head_dim
+        self.n_q = sum(should_quantize_kv_layer(i, n_layers) for i in range(n_layers))
+        self.group_size, self.batch, self.device, self.stream = group_size, batch, device, stream
+        self.q = QuantizedKVPool(self.n_q, n_kv_heads, head_dim, device, group_size=group_size, batch=batch,
+                                 capacity=capacity, stream=stream)
+        self.bf = (KVPool(n_layers - self.n_q, n_kv_heads, head_dim, device, batch=batch, capacity=capacity,
+                          stream=stream) if self.n_q < n_layers else None)
+
+    @property
+    def capacity(self) -> int:
+        return self.q.capacity
+
+    @property
+    def generation(self) -> int:
+        return self.q.generation
+
+    @generation.setter
+    def generation(self, v):
+        self.q.generation = v
+
+    def reserve(self, n_tokens: int, live_tokens: int = 0) -> bool:
+        moved = self.q.reserve(n_tokens, live_tokens=live_tokens)
+        if self.bf is not None:
+            with torch.cuda.stream(self.stream) if self.stream is not None else nullcontext():
+                self.bf.reserve(n_tokens, live_tokens=live_tokens)
+            assert self.bf.capacity == self.q.capacity
+        return moved
+
+    def like(self, batch: int, capacity: int) -> "BatchKVQPool":
+        return BatchKVQPool(self.n_layers, self.n_kv, self.hd, self.device, group_size=self.group_size, batch=batch,
+                            capacity=capacity, stream=self.stream)
+
+    def bytes_per_position(self) -> int:
+        """bytes of one position of one row over all layers"""
+        return self.q.bytes_per_position() + (self.n_layers - self.n_q) * 2 * self.n_kv * self.hd * 2
+
+    def row_caches(self, row: int) -> list:
+        """per-layer views of row `row`: QuantizedKVCache on the 8-bit layers, KVCache on the bf16 one"""
+        out = [QuantizedKVCache(self.group_size, 8, pool=self.q, layer=l, row=row) for l in range(self.n_q)]
+        out += [KVCache(self.bf, l - self.n_q, row=row) for l in range(self.n_q, self.n_layers)]
+        for c in out:
+            c._batch_pool = self
+        return out
+
+
 class _BaseCache:
     @property
     def state(self):
@@ -609,8 +672,11 @@ class BatchRows:
         """room for `rows` rows of `tokens` positions (re-allocates and copies the live part)"""
         p = self.pool
         if rows > p.batch:
-            new = KVPool(p.n_layers, p.n_kv, p.hd, p.device, batch=rows, capacity=max(p.capacity, tokens),
-                         dtype=p.dtype)
+            if isinstance(p, BatchKVQPool):
+                new = p.like(rows, max(p.capacity, tokens))
+            else:
+                new = KVPool(p.n_layers, p.n_kv, p.hd, p.device, batch=rows, capacity=max(p.capacity, tokens),
+                             dtype=p.dtype)
             with torch.cuda.stream(self.eng.stream):
                 for b, n in enumerate(self.lengths):
                     self.eng.kv_copy_row(new, b, p, b, n)
@@ -653,8 +719,19 @@ class BatchRows:
         self._touch()
         return n
 
-    def layer_caches(self) -> List["RowBatchKVCache"]:
-        return [RowBatchKVCache(self, l) for l in range(self.pool.n_layers)]
+    def layer_caches(self) -> list:
+        p = self.pool
+        if isinstance(p, BatchKVQPool):   # the batch rule: BatchQuantizedKVCache where the layer is 8-bit
+            return ([BatchQuantizedKVCache(self, l) for l in range(p.n_q)] +
+                    [RowBatchKVCache(self, l) for l in range(p.n_q, p.n_layers)])
+        return [RowBatchKVCache(self, l) for l in range(p.n_layers)]
+
+    def key(self) -> tuple:
+        """identifies the device allocation behind the rows (changes whenever it moves)"""
+        p = self.pool
+        if isinstance(p, BatchKVQPool):
+            return (p.q.codes.data_ptr() if p.q.codes is not None else 0, p.capacity)
+        return (p.buf.data_ptr() if p.buf is not None else 0,)
 
 
 class RowBatchKVCache(_BaseCache):
@@ -678,13 +755,17 @@ class RowBatchKVCache(_BaseCache):
         import numpy as np
         return np.zeros(self._rows.B, dtype=np.int64)
 
+    def _planes(self):
+        p = self._rows.pool
+        return p.bf.buf[self._layer - p.n_q] if isinstance(p, BatchKVQPool) else p.buf[self._layer]
+
     @property
     def keys(self):
-        return self._rows.pool.buf[self._layer, 0][:self._rows.B]
+        return self._planes()[0][:self._rows.B]
 
     @property
     def values(self):
-        return self._rows.pool.buf[self._layer, 1][:self._rows.B]
+        return self._planes()[1][:self._rows.B]
 
     @property
     def state(self):
@@ -751,3 +832,106 @@ class RowBatchKVCache(_BaseCache):
                 for c in caches:
                     rows.append_row(c._pool, c._row or 0, int(c.offset))
         return cls(rows, c0._layer)
+
+
+class BatchQuantizedKVCache(_BaseCache):
+    """One 8-bit layer's view of a `BatchRows` over a `BatchKVQPool`, with the reference's observable surface
+    (models/cache.py:1747-1960): `keys` / `values` are (codes as uint32 (B, n_kv, S, head_dim / 4), scales, biases)
+    in mx.quantize's packing, `offset` the per-row lengths, `left_padding` zeros (rows here are not padded).  Rows
+    sit on the pool rows exactly as for `RowBatchKVCache`; `filter` / `extend` act on the whole pool from layer 0 and
+    move every plane byte for byte.  `extract` returns a single-request `QuantizedKVCache`."""
+
+    def __init__(self, rows: BatchRows, layer: int):
+        self._rows = rows
+        self._layer = layer
+        self.bits = 8
+
+    @property
+    def group_size(self) -> int:
+        return self._rows.pool.group_size
+
+    @property
+    def offset(self):
+        import numpy as np
+        return np.asarray(self._rows.lengths, dtype=np.int64)
+
+    @property
+    def left_padding(self):
+        import numpy as np
+        return np.zeros(self._rows.B, dtype=np.int64)
+
+    def _side(self, side: int):
+        q = self._rows.pool.q
+        B = self._rows.B
+        return (q.codes[self._layer, side, :B].view(torch.uint32), q.scales[self._layer, side, :B],
+                q.biases[self._layer, side, :B])
+
+    @property
+    def keys(self):
+        return self._side(0)
+
+    @property
+    def values(self):
+        return self._side(1)
+
+    @property
+    def state(self):
+        n = self.size()
+        k, v = self.keys, self.values
+        return (tuple(x[..., :n, :] for x in k), tuple(x[..., :n, :] for x in v), self.offset, self.left_padding)
+
+    def size(self):
+        return max(self._rows.lengths) if self._rows.lengths else 0
+
+    def empty(self):
+        return self._rows.B == 0
+
+    def is_trimmable(self):
+        return True
+
+    @property
+    def batch_size(self) -> int:
+        return self._rows.B
+
+    def trim(self, n):
+        if self._layer == 0:
+            return self._rows.trim(n)
+        return min([n] + [ln + n for ln in self._rows.lengths]) if self._rows.lengths else 0
+
+    def filter(self, batch_indices):
+        if self._layer == 0:
+            idx = batch_indices.tolist() if hasattr(batch_indices, "tolist") else list(batch_indices)
+            self._rows.filter(idx)
+
+    def extend(self, other: "BatchQuantizedKVCache"):
+        if self._layer == 0:
+            self._rows.extend(other._rows)
+
+    def extract(self, idx: int) -> QuantizedKVCache:
+        """row `idx` as a single-request QuantizedKVCache of this layer (a byte copy of its first offset[idx]
+        positions).  The reference calls extract on every layer in turn; as the layers of a request share one pool
+        here, the extract of layer 0 copies the row's 8-bit layers into a FRESH single-request pool and the extracts
+        of the other 8-bit layers of that same sweep (same rows state, row and length) view it.  Every sweep gets its
+        own pool, so caches extracted twice never share storage."""
+        rows = self._rows
+        key = (rows.version, rows.key(), idx, rows.lengths[idx])
+        cached = getattr(rows, "_extracted", None)
+        if self._layer == 0 or cached is None or cached[0] != key or self._layer in cached[2]:
+            bp, n = rows.pool, rows.lengths[idx]
+            one = QuantizedKVPool(bp.n_q, bp.n_kv, bp.hd, bp.device, group_size=bp.group_size, batch=1,
+                                  capacity=max(n, 1), stream=rows.eng.stream)
+            with torch.cuda.stream(rows.eng.stream) if rows.eng.stream is not None else nullcontext():
+                rows.eng.kvq_copy_row(one, 0, bp.q, idx, n)
+            cached = (key, one, set())
+            rows._extracted = cached
+        cached[2].add(self._layer)
+        out = QuantizedKVCache(self.group_size, 8, pool=cached[1], layer=self._layer)
+        out.offset = rows.lengths[idx]
+        return out
+
+    def make_mask(self, N: int, return_array: bool = False, **kwargs):
+        return None if N == 1 else "causal"
+
+    @property
+    def nbytes(self):
+        return sum(x.numel() * x.element_size() for x in (*self.keys, *self.values))

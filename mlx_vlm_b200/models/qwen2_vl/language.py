@@ -15,7 +15,8 @@ import numpy as np
 import torch
 
 from ..base import LanguageModelOutput
-from ..cache import BatchRows, KVCache, KVPool, QuantizedKVCache, QuantizedKVPool, RowBatchKVCache
+from ..cache import (BatchKVQPool, BatchQuantizedKVCache, BatchRows, KVCache, KVPool, QuantizedKVCache,
+                     QuantizedKVPool, RowBatchKVCache)
 from .config import ModelConfig, TextConfig
 
 
@@ -117,23 +118,36 @@ class LanguageModel:
         return [KVCache(pool, l) for l in range(self.args.num_hidden_layers)]
 
     def make_cache_row(self, pool: KVPool, row: int):
-        """per-layer KVCache views of ROW `row` of a batched pool (a request admitted to a batch)"""
+        """per-layer KVCache views of ROW `row` of a batched pool (a request admitted to a batch); on a kv_bits=8
+        batch pool (BatchKVQPool) QuantizedKVCache views on its 8-bit layers"""
+        if isinstance(pool, BatchKVQPool):
+            return pool.row_caches(row)
         return [KVCache(pool, l, row=row) for l in range(self.args.num_hidden_layers)]
 
-    def make_batch_cache(self, rows: int, capacity: int = 0):
-        """device-resident batch cache for `rows` requests: (BatchRows, per-layer RowBatchKVCache)"""
+    def make_batch_cache(self, rows: int, capacity: int = 0, kv_bits=None, kv_group_size: int = 64):
+        """device-resident batch cache for `rows` requests: (BatchRows, per-layer caches) — RowBatchKVCache, or with
+        kv_bits=8 the reference's batch rule (BatchQuantizedKVCache where `should_quantize_kv_layer` holds)"""
         eng = self._engine()
-        pool = KVPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
-                      batch=rows, capacity=max(capacity, KVPool.step))
+        if kv_bits is not None:
+            from ..cache import _kvq_check
+            _kvq_check(kv_group_size, kv_bits, self.head_dim)
+            pool = BatchKVQPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
+                                group_size=kv_group_size, batch=rows, capacity=max(capacity, KVPool.step),
+                                stream=eng.stream)
+        else:
+            pool = KVPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
+                          batch=rows, capacity=max(capacity, KVPool.step))
         r = BatchRows(pool, eng)
         return r, r.layer_caches()
 
-    def _bind(self, cache, need_tokens: int, decode: bool = False) -> KVPool:
+    def _bind(self, cache, need_tokens: int, decode: bool = False, chunk_end: Optional[int] = None) -> KVPool:
         c0 = cache[0]
         pool = getattr(c0, "_pool", None)
         if pool is None:
             raise ValueError("b200 LanguageModel needs caches from make_prompt_cache(language_model)")
         eng = self._engine()
+        if getattr(c0, "_batch_pool", None) is not None:
+            return self._bind_batch_row(cache, need_tokens, decode, chunk_end)
         if any(isinstance(c, QuantizedKVCache) for c in cache):
             return self._bind_q8(cache, need_tokens, decode)
         if pool.capacity < need_tokens:
@@ -168,6 +182,53 @@ class LanguageModel:
         eng.set_prefill_kvq(pool)
         return prefix
 
+    def _bind_batch_row(self, cache, need_tokens: int, decode: bool, chunk_end: Optional[int]):
+        """the prefill of a row admitted to a kv_bits=8 batch pool (BatchKVQPool): the chunks run on a batch-1 bf16
+        pool of this admission and write the 8-bit layers' rows through to the batch pool's row, quantized before
+        they are attended (their dequantized values stay in the bf16 pool as the prefix of the next chunk); the
+        bf16 layers are copied to the batch pool after each chunk (`_finish_batch_row`).  The transient pool holds
+        the prompt only (`chunk_end`: the end of this chunk), grown chunk by chunk; `need_tokens` (which includes
+        the tokens still to be generated) sizes the batch pool"""
+        c0 = cache[0]
+        bp, row, off = c0._batch_pool, c0._row, int(c0.offset)
+        if decode or chunk_end is None:
+            raise NotImplementedError("a row of a kv_bits=8 batch pool decodes in the lock-step batch only")
+        eng = self._engine()
+        adm = getattr(bp, "_admit", None)
+        if off == 0 or adm is None or adm[0] != row:
+            if off != 0:
+                raise NotImplementedError("a prefill chunk of a kv_bits=8 batch row must continue that row's admission")
+            with torch.cuda.stream(eng.stream):
+                tmp = KVPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
+                             batch=1, capacity=chunk_end, stream=eng.stream)
+            bp._admit = (row, tmp)
+        else:
+            tmp = adm[1]
+            if tmp.capacity < chunk_end:
+                eng.stream.synchronize()
+                with torch.cuda.stream(eng.stream):
+                    tmp.reserve(chunk_end, live_tokens=off)
+        if bp.capacity < need_tokens:
+            raise ValueError(f"kv_bits=8 batch pool holds {bp.capacity} positions per row, the row needs {need_tokens}")
+        eng.bind_pool(tmp)
+        eng.set_kv_row(0)
+        eng.set_prefill_kvq_row(bp, row)
+        return tmp
+
+    def _finish_batch_row(self, cache, n_tokens: int):
+        """after a prefill chunk of a kv_bits=8 batch row: its bf16 layers move to the batch pool's row"""
+        eng = self._engine()
+        bp = cache[0]._batch_pool
+        eng.set_prefill_kvq(None)
+        if bp.bf is None:
+            return
+        from ... import _native as Nn
+        tmp = bp._admit[1]
+        src = tmp.buf[bp.n_q:]
+        Nn.check(eng.lib.b200_pool_copy_row(bp.bf.buf.data_ptr(), bp.batch, bp.capacity, int(cache[0]._row),
+                                            src.data_ptr(), 1, tmp.capacity, 0, bp.n_layers - bp.n_q, bp.n_kv,
+                                            2 * bp.hd, int(n_tokens), eng.s), "pool_copy_row")
+
     # ------------------------------------------------------------------ call
     def __call__(self, inputs, inputs_embeds=None, mask=None, cache=None, **kwargs):
         position_ids = kwargs.pop("position_ids", None)
@@ -189,7 +250,7 @@ class LanguageModel:
         if ids_host.ndim == 1:
             ids_host = ids_host[None]
         B, L = ids_host.shape
-        if isinstance(cache[0], RowBatchKVCache):
+        if isinstance(cache[0], (RowBatchKVCache, BatchQuantizedKVCache)):
             return self._call_batch(ids_host, inputs_embeds, mask, cache, rope_deltas_kw, position_ids,
                                     reserve_tokens)
         cache_offset = int(cache[0].offset)
@@ -200,7 +261,7 @@ class LanguageModel:
                                                          image_grid_thw, video_grid_thw, rope_deltas_kw)
 
         need = max(cache_offset + L, reserve_tokens)
-        self._bind(cache, need, decode=(L == 1 and inputs_embeds is None))
+        self._bind(cache, need, decode=(L == 1 and inputs_embeds is None), chunk_end=cache_offset + L)
         V = self.args.vocab_size
         if L == 1 and inputs_embeds is None:
             # ---- decode step through the captured graph ----
@@ -221,7 +282,9 @@ class LanguageModel:
             Vp = (V + 7) // 8 * 8     # device rows are 16-byte aligned for any vocabulary
             all_logits = eng.empty((L, Vp)) if keep_all else None
             eng.prefill(emb.contiguous(), pos3, cache_offset, delta0, all_logits)
-            if isinstance(cache[0], QuantizedKVCache):
+            if getattr(cache[0], "_batch_pool", None) is not None:
+                self._finish_batch_row(cache, cache_offset + L)
+            elif isinstance(cache[0], QuantizedKVCache):
                 eng.set_prefill_kvq(None)
             logits = (all_logits[:, :V].unsqueeze(0) if keep_all
                       else eng.snapshot("logits").view(1, 1, V))
@@ -376,7 +439,7 @@ class LanguageModel:
         eng.bind_pool(rows.pool)
         ctx = np.asarray(rows.lengths, dtype=np.int64)
         eng.batch_begin(np.asarray(toks).reshape(-1)[:B], ctx, ctx + d, np.ones(B, dtype=np.int32))
-        self._batch_key = (id(rows), rows.version, rows.pool.buf.data_ptr())
+        self._batch_key = (id(rows), rows.version, rows.key())
         self._batch_step = 0
 
     def _fused_greedy_batch(self, ids, cache, **kwargs):
@@ -388,7 +451,7 @@ class LanguageModel:
         eng = self._engine()
         inputs = kwargs.get("_inputs_tensor", None)
         last = getattr(self, "_fused_last", None)
-        key = (id(rows), rows.version, rows.pool.buf.data_ptr() if rows.pool.buf is not None else 0)
+        key = (id(rows), rows.version, rows.key())
         chained = (last is not None and isinstance(inputs, torch.Tensor) and inputs.is_cuda and
                    inputs.data_ptr() == last.data_ptr() and getattr(self, "_batch_key", None) == key and
                    self._batch_step + 1 < eng.BATCH_LOG_STEPS and
