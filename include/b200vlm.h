@@ -180,8 +180,8 @@ int b200_engine_destroy(b200_engine* e);
  *   fc1.w,fc1.b,fc2.w,fc2.b} | v.merger.{ln.w,ln.b,fc1.w,fc1.b,fc2.w,fc2.b} |
  *   lm.embed | lm.head (untied only) | lm.norm | lm.<i>.{ln1,ln2,wqkv,bqkv,wo,wgu,wd}
  *   | lm.<i>.{qn,kn} (head_dim each: Qwen3-VL's q_norm / k_norm, qwen3_vl/language.py:59-60; set for every
- *   layer or for none.  With them every path that writes K normalises q and k per head before the rotary;
- *   the persistent k_mega / k_mega_tc kernels refuse such a model, so its steps run the per-phase kernels) */
+ *   layer or for none.  With them every path that writes K normalises q and k per head before the rotary,
+ *   the persistent k_mega kernel included) */
 int b200_engine_set_weight(b200_engine* e, const char* name, const void* ptr, long n_elems);
 /* scratch for activations; must be >= b200_engine_workspace_bytes(max tokens) */
 long b200_engine_workspace_bytes(const b200_engine* e, int max_tokens, int max_patches);
@@ -192,7 +192,7 @@ int b200_engine_bind_kv(b200_engine* e, void* pool, int batch, int cap);
 /* 8-bit KV pool (kv_bits=8; format in csrc/kvq.cuh): codes (n_layers, 2, batch, n_kv, cap, head_dim) uint8,
  * scales and biases (n_layers, 2, batch, n_kv, cap, head_dim / group_size) bf16, group_size 32 | 64 | 128.
  * Replaces the bf16 binding: decode steps quantize the new K/V row, append it and attend over the dequantized
- * cache with the per-phase kernels (the persistent k_mega kernels read bf16 pools only).  Prefill calls need a
+ * cache with the per-phase kernels (the persistent k_mega kernel reads bf16 pools only).  Prefill calls need a
  * bf16 pool (b200_engine_bind_kv) again. */
 int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases, int batch, int cap,
                          int group_size);
@@ -295,15 +295,11 @@ long b200_engine_launch_count(const b200_engine* e);
 /* 0: decode via plain launches, 1: CUDA-graph replay (default) */
 int b200_engine_set_graph(b200_engine* e, int enabled);
 /* decode-step implementation.  0: one kernel per phase (28 x 5 + 2 launches);
- * 1: ONE persistent kernel, CUDA-core GEMV consumers (k_mega: weight ring + software grid
- * barrier); 2: the same step with wgmma GEMV consumers on pre-packed tile images of
- * the weights (k_mega_tc; the engine allocates the packed copy on first use);
- * 3: as 2 with a full 16-row activation operand (debugging);
- * 4: k_mega in dataflow mode (three of the five per-layer grid barriers replaced by polling
- *    self-validating activation words; measured slower than 1, kept for A/B). */
+ * 1 (default): ONE persistent kernel, CUDA-core GEMV consumers (k_mega: weight ring + software
+ * grid barrier); a geometry it cannot hold runs the per-phase kernels.  Any other value is
+ * B200_ERR_INVALID and leaves the mode unchanged. */
 int b200_engine_set_mega(b200_engine* e, int enabled);
-/* debugging / test aid: device pointer and size of an internal buffer.  names: "h", "act",
- * "tc_acc" (k_mega_tc fixed-point split-K accumulators, 3 x rows int64). */
+/* debugging / test aid: device pointer and size of an internal buffer.  names: "h", "act". */
 int b200_engine_debug_buffer(b200_engine* e, const char* name, void** ptr, long* bytes);
 /* synchronous: reads the device-side error flag (0 = none; a bounded wait gave up) */
 int b200_engine_device_error(b200_engine* e, int* out);

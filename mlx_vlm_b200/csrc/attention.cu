@@ -138,21 +138,13 @@ int attention_tc(const void* q, long q_ts, long q_hs, const void* k, long k_ts, 
                  const void* v, long v_ts, long v_hs, void* out, long o_ts, int n_heads, int n_kv,
                  int hd, int Lq, int S, int causal, float scale, cudaStream_t st);
 
-static int g_attn_impl = -1;  // -1: read B200_ATTN_V1 once; 0: tensor cores; 1: CUDA-core v1
-void attention_set_impl(int v1) { g_attn_impl = v1 ? 1 : 0; }
-
 int attention(const void* q, long q_ts, long q_hs, const void* k, long k_ts, long k_hs,
               const void* v, long v_ts, long v_hs, void* out, long o_ts, int n_heads, int n_kv,
               int hd, int Lq, int S, int causal, float scale, cudaStream_t st) {
   B200_REQUIRE(Lq > 0 && S > 0 && n_heads > 0 && n_kv > 0 && n_heads % n_kv == 0,
                "attention: bad shape Lq=%d S=%d heads=%d kv=%d", Lq, S, n_heads, n_kv);
   B200_REQUIRE(!causal || S >= Lq, "attention: causal needs S >= Lq");
-  if (g_attn_impl < 0) {
-    const char* e = getenv("B200_ATTN_V1");
-    g_attn_impl = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (g_attn_impl == 0 &&
-      attention_tc_supported(q, q_ts, q_hs, k, k_ts, k_hs, v, v_ts, v_hs, out, o_ts, hd))
+  if (attention_tc_supported(q, q_ts, q_hs, k, k_ts, k_hs, v, v_ts, v_hs, out, o_ts, hd))
     return attention_tc(q, q_ts, q_hs, k, k_ts, k_hs, v, v_ts, v_hs, out, o_ts, n_heads, n_kv, hd,
                         Lq, S, causal, scale, st);
   B200_REQUIRE(hd % 8 == 0 && hd <= 128, "attention: head_dim %d unsupported (need %%8, <=128)", hd);

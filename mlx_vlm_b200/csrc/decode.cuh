@@ -59,13 +59,7 @@ struct MegaP {
   int attn_ctas, hsplit;
   unsigned long long* bar;  // monotonic grid-barrier counter
   int advance;
-  int l2_prefetch;   // 1: producer-issued (round 1), 2: consumer-issued gate/up, 3: + down
-  int l2_skip;       // gate/up tiles per CTA the consumer-issued prefetch leaves to the ring
-  int max_inflight;   // k_mega: weight tiles requested but not landed per SM (0: no limit)
-  int flow;           // k_mega dataflow mode: 3 of the 5 per-layer grid barriers become polled words
   int scratch_bytes;  // attention scratch / activation vector region after the ring
-  unsigned long long *hmid_w, *hout_w;  // residual stream after o_proj / after down, one word per element
-  unsigned long long* qkv_w;            // finished q/k/v pairs [head slot][hd/2]
   float* att_part;  // [groups][8 units][4*hd] fp32 partial attention outputs
   float* att_stats; // [groups][8 units][4 heads] x 2 words {float bits << 32 | epoch}: (max, sum exp)
   long long* dbg;  // optional [2][1024][2] globaltimer stamps (arrive, release) per barrier
@@ -77,35 +71,6 @@ struct MegaP {
 };
 int mega_fill(MegaP& p, int sm_count);
 int mega_launch(const MegaP& p, int sm_count, cudaStream_t s);
-
-// ---- k_mega_tc (decode_mega_tc.cu): the same step with wgmma GEMV phases -----------
-struct LayerWT {
-  const uint8_t *wqkv, *wo, *wgu, *wd;  // tile images (128 rows x 64 cols, 128B swizzle)
-};
-struct MegaTcPhase {
-  int K, N;    // reduction length, output rows (gate/up: intermediate channels)
-  int KB, RB;  // K blocks of 64, row blocks
-  int S;       // K splits (units = RB * S; split phases have at most one unit per CTA)
-  int units;
-};
-struct MegaTcP {
-  MegaP base;
-  LayerWT lt[MEGA_MAX_LAYERS];
-  const uint8_t* head_t;
-  long long *qkv_acc, *o_acc, *d_acc;  // fixed-point split-K sums, one per output row
-  MegaTcPhase ph[5];
-  int max_inflight;  // weight tiles requested but not yet landed, per SM
-  int sps;           // K blocks per ring stage
-  int x_kstride;     // bytes between K blocks of the activation operand (1024: 8 rows, 2048: 16)
-  int x_sbo;         // stride between its 8-row groups (0: rows 8..15 alias rows 0..7)
-  int region_bytes;  // operand / attention scratch region
-  size_t smem_bytes;
-};
-int mega_tc_fill(MegaTcP& P, int sm_count);
-int mega_tc_launch(const MegaTcP& P, int sm_count, cudaStream_t s);
-size_t mega_tc_packed_bytes(int N, int K, bool interleave);
-int mega_tc_pack(const bf16* src, const bf16* src2, int N, int K, bool interleave, void* dst,
-                 cudaStream_t s);
 
 // lock-step batched decode (decode_batch.cu)
 struct BdModel {

@@ -36,20 +36,12 @@ __device__ __forceinline__ const bf16* mega_tile_src(const MegaPhase& g, const b
 template <int MODE>
 __device__ __forceinline__ void produce_phase(const MegaPhase& g, const bf16* W, const bf16* W2,
                                               int hd, uint8_t* ring, MegaShared* sh, Ring& rg,
-                                              uint64_t pol, Ring& lag, int& issued, int max_inflight,
-                                              long long* tdbg = nullptr) {
+                                              uint64_t pol, long long* tdbg = nullptr) {
   using T = PhTraits<MODE>;
   const int rows_unit = g.K * 2;
   int tn = 0;
   for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
     const int s = rg.slot();
-    if (max_inflight > 0) {  // in-flight throttle (see decode_mega_tc.cu::Producer)
-      if (issued >= max_inflight) {
-        mb_wait(&sh->full_bar[lag.slot()], lag.parity(), &sh->err);
-        lag.advance();
-      }
-      ++issued;
-    }
     mb_wait(&sh->empty_bar[s], rg.parity() ^ 1u, &sh->err);
     if (tdbg && tn < 30) tdbg[tn++] = gtimer();
     int rows = g.R;
@@ -62,23 +54,6 @@ __device__ __forceinline__ void produce_phase(const MegaPhase& g, const bf16* W,
       bulk_g2s(dst + (long)g.R * rows_unit, mega_tile_src<MODE>(g, W, W2, hd, t, 1), bytes,
                &sh->full_bar[s], pol);
     rg.advance();
-  }
-}
-
-template <int MODE>
-__device__ __forceinline__ void l2_prefetch_phase(const MegaPhase& g, const bf16* W,
-                                                  const bf16* W2, int skip = 0) {
-  const int rows_unit = g.K * 2;
-  for (int t = blockIdx.x + skip * gridDim.x; t < g.tiles; t += gridDim.x) {
-    const int rows = min(g.R, g.N - t * g.R);
-    const uint32_t bytes = (uint32_t)rows * rows_unit;
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(W + (long)t * g.R * g.K),
-                 "r"(bytes)
-                 : "memory");
-    if (PhTraits<MODE>::PAIR)
-      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(W2 + (long)t * g.R * g.K),
-                   "r"(bytes)
-                   : "memory");
   }
 }
 
@@ -110,15 +85,9 @@ struct PhaseIO {
   bf16 *kc, *vc;     // QKV
   float2* partials;  // HEAD
   const float* xpart;  // ORES: partial attention outputs to be summed (instead of x)
-  // dataflow mode: activations cross CTAs as self-validating words (mega_common.cuh::st_word)
-  const unsigned long long* xw;  // input vector, one word per element (nullptr: plain io.x)
-  unsigned long long* outw;      // ORES / DRES: output h, one word per element
-  unsigned long long* qkvw;      // QKV: finished (dim j, dim j + hd/2) pairs [head slot][hd/2]
-  uint16_t* hraw;                // shared-memory copy of the un-normalised residual stream
-  uint32_t epoch, epoch_in;      // tag written by this phase / tag of the words it reads
 };
 
-template <int MODE, int CHX, bool FLOW>
+template <int MODE, int CHX>
 __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g, const PhaseIO& io,
                                               uint8_t* ring, uint8_t* xs_raw, MegaShared* sh,
                                               Ring& rg, int ctx, int pos,
@@ -162,13 +131,10 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
         v.y = pack2(sa.z, sa.w);
         v.z = pack2(sb.x, sb.y);
         v.w = pack2(sb.z, sb.w);
-      } else if (FLOW && io.xw) {
-        v = poll8(io.xw + (long)c * 8, io.epoch_in, &sh->err);
       } else {
         v = ldcg16(io.x + (long)c * 8);
       }
       xs[c] = v;
-      if (FLOW && T::NORM && MODE != PH_HEAD) reinterpret_cast<uint4*>(io.hraw)[c] = v;
       if (T::NORM) {
         float f[8];
         unpack8(v, f);
@@ -210,7 +176,7 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
   float run_m = -INFINITY, run_l = 0.f;
   // epilogue operands fetched BEFORE the tiles are waited for (off the critical path)
   float hpre = 0.f;  // ORES/DRES: lane i holds the residual value of this warp's i-th tile
-  if (!FLOW && (MODE == PH_ORES || MODE == PH_DRES) && sub == 0) {
+  if ((MODE == PH_ORES || MODE == PH_DRES) && sub == 0) {
     const int t = blockIdx.x + lane * gridDim.x;
     const int r = t * g.R + rloc;
     if (t < g.tiles && r < g.N) hpre = ldcg_bf(io.out + r);
@@ -244,8 +210,7 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
           bf16* dst = io.vc + ((long)(slot - p.d.n_heads - p.d.n_kv) * p.d.cap + ctx) * hd;
           dst[j] = f2bf(y1);
           dst[j + half] = f2bf(y2);
-          if (FLOW) st_word(io.qkvw + (long)slot * half + j, bf_bits(y1) | (bf_bits(y2) << 16), io.epoch);
-        } else if (!FLOW && p.qk_norm) {  // raw q / k: the q/k-norm phase normalises and rotates them
+        } else if (p.qk_norm) {  // raw q / k: the q/k-norm phase normalises and rotates them
           bf16* dst = (slot < p.d.n_heads) ? io.out + (long)slot * hd
                                            : io.kc + ((long)(slot - p.d.n_heads) * p.d.cap + ctx) * hd;
           dst[j] = f2bf(y1);
@@ -255,14 +220,11 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
           const float c = rbf(cosf(ang)), sn = rbf(sinf(ang));
           const float o1 = rbf(rbf(y1 * c) + rbf((-y2) * sn));
           const float o2 = rbf(rbf(y2 * c) + rbf(y1 * sn));
-          if (FLOW) st_word(io.qkvw + (long)slot * half + j, bf_bits(o1) | (bf_bits(o2) << 16), io.epoch);
-          if (!FLOW || slot >= p.d.n_heads) {  // dataflow mode: q travels in the words only
-            bf16* dst = (slot < p.d.n_heads)
-                            ? io.out + (long)slot * hd
-                            : io.kc + ((long)(slot - p.d.n_heads) * p.d.cap + ctx) * hd;
-            dst[j] = f2bf(o1);
-            dst[j + half] = f2bf(o2);
-          }
+          bf16* dst = (slot < p.d.n_heads)
+                          ? io.out + (long)slot * hd
+                          : io.kc + ((long)(slot - p.d.n_heads) * p.d.cap + ctx) * hd;
+          dst[j] = f2bf(o1);
+          dst[j + half] = f2bf(o2);
         }
       }
     } else if (MODE == PH_GATEUP) {
@@ -270,13 +232,8 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
     } else if (MODE == PH_ORES || MODE == PH_DRES) {
       if (mine) {
         const int r = t * g.R + rloc;
-        if (FLOW) {  // residual from the CTA's own copy of the stream; result as a tagged word
-          const float hv = __uint_as_float((uint32_t)io.hraw[r] << 16);
-          st_word(io.outw + r, bf_bits(rbf(hv + rbf(keep0))), io.epoch);
-        } else {
-          const float hv = (it0 == 0) ? hpre : ldcg_bf(io.out + r);  // lane i prefetched tile i
-          io.out[r] = f2bf(rbf(hv + rbf(keep0)));
-        }
+        const float hv = (it0 == 0) ? hpre : ldcg_bf(io.out + r);  // lane i prefetched tile i
+        io.out[r] = f2bf(rbf(hv + rbf(keep0)));
       }
     } else {  // HEAD: logits + running logsumexp (warp-parallel over the 32 tiles)
       const float a = mine ? rbf(keep0) : -INFINITY;
@@ -385,20 +342,13 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
 
 }  // namespace
 
-// FLOW: dataflow mode — the grid barriers after qkv, o_proj and down are replaced by polling
-// self-validating words (q/k/v pairs, the residual stream); the barriers after attention (its
-// fp32 partial outputs) and after gate/up (the 18 KB activation vector) remain.  Safe without
-// them because every later phase needs data from ALL CTAs of the phase before it (transitively
-// nobody can overwrite a word that a slower CTA still has to read), and the tag of a word is
-// unique per (step, layer).
-template <int CHH, int CHI, bool FLOW>
+template <int CHH, int CHI>
 __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega(const MegaP p) {
   extern __shared__ __align__(128) uint8_t sm[];
   __shared__ MegaShared sh;
   uint8_t* ring = sm;
   uint8_t* xs = sm + (long)p.n_stages * MEGA_STAGE;  // activation vector (GEMV phases) /
   float* scratch = reinterpret_cast<float*>(xs);     // attention scratch (attention phase)
-  uint16_t* hraw = reinterpret_cast<uint16_t*>(xs + p.scratch_bytes);  // FLOW: raw residual stream
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (p.st->error) return;  // a previous step gave up: do not spin again
   if (threadIdx.x == 0) {
@@ -423,28 +373,15 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega(const MegaP p) {
     // ===== producer: the whole step's weight stream, never blocked by a phase =====
     if (lane == 0) {
       const uint64_t pol = policy_evict_first();
-      Ring lag = rg;
-      int issued = 0;
-      const int mif = p.max_inflight;
       for (int l = 0; l < p.n_layers; ++l) {
         const LayerW& lw = p.layers[l];
-        // the qkv/attention/o_proj chain is latency-bound (~20 us with ~11 MB of weights):
-        // use it to pull this CTA's share of the layer's MLP weights (82 MB chip-wide,
-        // fits the 126 MB L2) into L2, so the ring later refills at L2 speed.
-        // (measured, round 1: no gain — gate/up is consumer-bound at 8 warps — and a
-        // straggler CTA in the down phase; kept behind a switch for round 2)
-        if (p.l2_prefetch == 1) {
-          l2_prefetch_phase<PH_GATEUP>(p.ph[PH_GATEUP], lw.wgu, lw.wgu + (long)d.inter * d.hidden);
-          l2_prefetch_phase<PH_DRES>(p.ph[PH_DRES], lw.wd, nullptr);
-        }
-        produce_phase<PH_QKV>(p.ph[PH_QKV], lw.wqkv, nullptr, d.hd, ring, &sh, rg, pol, lag, issued, mif);
-        produce_phase<PH_ORES>(p.ph[PH_ORES], lw.wo, nullptr, d.hd, ring, &sh, rg, pol, lag, issued, mif);
-        produce_phase<PH_GATEUP>(p.ph[PH_GATEUP], lw.wgu, lw.wgu + (long)d.inter * d.hidden, d.hd,
-                                 ring, &sh, rg, pol, lag, issued, mif,
-                                 (p.dbg && l == 5 && blockIdx.x == 0) ? p.dbg + 4096 + 96 : nullptr);
-        produce_phase<PH_DRES>(p.ph[PH_DRES], lw.wd, nullptr, d.hd, ring, &sh, rg, pol, lag, issued, mif);
+        produce_phase<PH_QKV>(p.ph[PH_QKV], lw.wqkv, nullptr, d.hd, ring, &sh, rg, pol);
+        produce_phase<PH_ORES>(p.ph[PH_ORES], lw.wo, nullptr, d.hd, ring, &sh, rg, pol);
+        produce_phase<PH_GATEUP>(p.ph[PH_GATEUP], lw.wgu, lw.wgu + (long)d.inter * d.hidden, d.hd, ring, &sh, rg,
+                                 pol, (p.dbg && l == 5 && blockIdx.x == 0) ? p.dbg + 4096 + 96 : nullptr);
+        produce_phase<PH_DRES>(p.ph[PH_DRES], lw.wd, nullptr, d.hd, ring, &sh, rg, pol);
       }
-      produce_phase<PH_HEAD>(p.ph[PH_HEAD], p.head, nullptr, d.hd, ring, &sh, rg, pol, lag, issued, mif);
+      produce_phase<PH_HEAD>(p.ph[PH_HEAD], p.head, nullptr, d.hd, ring, &sh, rg, pol);
     }
     return;
   }
@@ -452,68 +389,49 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega(const MegaP p) {
   // ===== consumers =====
   unsigned bidx = 0;
   const int ctx = p.st->ctx, pos = p.st->pos;
-  const long plane = (long)d.n_kv * d.cap * d.hd;  // one K (or V) plane of a layer, batch 1
   for (int l = 0; l < p.n_layers; ++l) {
     const LayerW& lw = p.layers[l];
     bf16* kc = p.kv + (long)l * p.kv_layer_stride;
     bf16* vc = kc + p.kv_v_offset;
-    (void)plane;
-    const uint32_t ep = (uint32_t)(sh.att_base + (unsigned long long)l + 1ull);  // tag of this layer
-    // B200_L2_PREFETCH >= 2: the CONSUMER side, entering the latency-bound qkv -> attention -> o_proj chain of this
-    // layer (~16 us during which HBM is idle once the ring is full), asks the L2 for this CTA's share of the layer's
-    // MLP weights; the first `l2_skip` gate/up tiles are already on their way into the ring.  (The producer-issued
-    // variant of round 1 fired while the PREVIOUS layer's MLP was still streaming: no gain.)
-    if (p.l2_prefetch >= 2 && threadIdx.x == 0) {
-      l2_prefetch_phase<PH_GATEUP>(p.ph[PH_GATEUP], lw.wgu, lw.wgu + (long)d.inter * d.hidden, p.l2_skip);
-      if (p.l2_prefetch >= 3) l2_prefetch_phase<PH_DRES>(p.ph[PH_DRES], lw.wd, nullptr);
-    }
     {
-      PhaseIO io = {p.h, lw.ln1, lw.bqkv, p.qbuf, kc, vc, nullptr, nullptr,
-                    (FLOW && l > 0) ? p.hout_w : nullptr, nullptr, p.qkv_w, hraw, ep, ep - 1u};
-      consume_phase<PH_QKV, CHH, FLOW>(p, p.ph[PH_QKV], io, ring, xs, &sh, rg, ctx, pos);
+      PhaseIO io = {p.h, lw.ln1, lw.bqkv, p.qbuf, kc, vc, nullptr, nullptr};
+      consume_phase<PH_QKV, CHH>(p, p.ph[PH_QKV], io, ring, xs, &sh, rg, ctx, pos);
     }
-    if (!FLOW) grid_barrier(p, &sh, bidx);
-    if (!FLOW && p.qk_norm) {
+    grid_barrier(p, &sh, bidx);
+    if (p.qk_norm) {
       if (d.hd == 128) qk_norm_phase<4>(p, l, p.qbuf, kc, ctx, pos);
       else qk_norm_phase<2>(p, l, p.qbuf, kc, ctx, pos);
       grid_barrier(p, &sh, bidx);
     }
     if ((int)blockIdx.x < p.attn_ctas) {
-      const AttnParts ap = {nullptr, nullptr, 0, p.qkv_w, ep};
-      constexpr int AM = FLOW ? ATT_FLOW : ATT_PLAIN;
-      if (d.hd == 128) attn_phase<128, AM>(p, kc, vc, scratch, &sh, ctx + 1, l, ap,
-                                           (p.dbg && l == 5 && blockIdx.x < 2) ? p.dbg + 4096 + 128 + 32 * blockIdx.x : nullptr);
-      else attn_phase<64, AM>(p, kc, vc, scratch, &sh, ctx + 1, l, ap);
+      if (d.hd == 128) attn_phase<128>(p, kc, vc, scratch, &sh, ctx + 1, l,
+                                       (p.dbg && l == 5 && blockIdx.x < 2) ? p.dbg + 4096 + 128 + 32 * blockIdx.x : nullptr);
+      else attn_phase<64>(p, kc, vc, scratch, &sh, ctx + 1, l);
     }
     grid_barrier(p, &sh, bidx);
     {
-      PhaseIO io = {p.attn, nullptr, nullptr, p.h, nullptr, nullptr, nullptr, p.att_part,
-                    nullptr, p.hmid_w, nullptr, hraw, ep, 0u};
-      if (p.ph[PH_ORES].S == 1) consume_phase<PH_ORES, CHH, FLOW>(p, p.ph[PH_ORES], io, ring, xs, &sh, rg, 0, 0);
-      else consume_phase<PH_DRES, CHH, FLOW>(p, p.ph[PH_ORES], io, ring, xs, &sh, rg, 0, 0);
+      PhaseIO io = {p.attn, nullptr, nullptr, p.h, nullptr, nullptr, nullptr, p.att_part};
+      if (p.ph[PH_ORES].S == 1) consume_phase<PH_ORES, CHH>(p, p.ph[PH_ORES], io, ring, xs, &sh, rg, 0, 0);
+      else consume_phase<PH_DRES, CHH>(p, p.ph[PH_ORES], io, ring, xs, &sh, rg, 0, 0);
     }
-    if (!FLOW) grid_barrier(p, &sh, bidx);
+    grid_barrier(p, &sh, bidx);
     {
-      PhaseIO io = {p.h, lw.ln2, nullptr, p.act, nullptr, nullptr, nullptr, nullptr,
-                    FLOW ? p.hmid_w : nullptr, nullptr, nullptr, hraw, ep, ep};
+      PhaseIO io = {p.h, lw.ln2, nullptr, p.act, nullptr, nullptr, nullptr, nullptr};
       long long* td = (p.dbg && l == 5 && (blockIdx.x == 0 || blockIdx.x == 77))
                           ? p.dbg + 4096 + (blockIdx.x ? 32 : 0) : nullptr;
-      consume_phase<PH_GATEUP, CHH, FLOW>(p, p.ph[PH_GATEUP], io, ring, xs, &sh, rg, 0, 0, td);
+      consume_phase<PH_GATEUP, CHH>(p, p.ph[PH_GATEUP], io, ring, xs, &sh, rg, 0, 0, td);
     }
     grid_barrier(p, &sh, bidx);
     {
-      PhaseIO io = {p.act, nullptr, nullptr, p.h, nullptr, nullptr, nullptr, nullptr,
-                    nullptr, p.hout_w, nullptr, hraw, ep, 0u};
+      PhaseIO io = {p.act, nullptr, nullptr, p.h, nullptr, nullptr, nullptr, nullptr};
       long long* td = (p.dbg && l == 5 && blockIdx.x == 0) ? p.dbg + 4096 + 64 : nullptr;
-      consume_phase<PH_DRES, CHI, FLOW>(p, p.ph[PH_DRES], io, ring, xs, &sh, rg, 0, 0, td);
+      consume_phase<PH_DRES, CHI>(p, p.ph[PH_DRES], io, ring, xs, &sh, rg, 0, 0, td);
     }
-    if (!FLOW) grid_barrier(p, &sh, bidx);
+    grid_barrier(p, &sh, bidx);
   }
   {
-    const uint32_t ep_last = (uint32_t)(sh.att_base + (unsigned long long)p.n_layers);
-    PhaseIO io = {p.h, p.final_norm, nullptr, p.logits, nullptr, nullptr, p.partials, nullptr,
-                  (FLOW && p.n_layers > 0) ? p.hout_w : nullptr, nullptr, nullptr, hraw, 0u, ep_last};
-    consume_phase<PH_HEAD, CHH, FLOW>(p, p.ph[PH_HEAD], io, ring, xs, &sh, rg, 0, 0);
+    PhaseIO io = {p.h, p.final_norm, nullptr, p.logits, nullptr, nullptr, p.partials, nullptr};
+    consume_phase<PH_HEAD, CHH>(p, p.ph[PH_HEAD], io, ring, xs, &sh, rg, 0, 0);
   }
   grid_barrier(p, &sh, bidx);
   mega_sample_finalize(p, sh, bidx);
@@ -537,19 +455,21 @@ static int mega_geometry(MegaPhase& g, int K, int N, bool pair, int units) {
   return B200_OK;
 }
 
-// region after the ring: attention scratch, or the activation vector of a GEMV phase
+// region after the ring: attention scratch, or the activation vector of a GEMV phase.
+// The scratch holds (MEGA_ATT_G + 2) * head_dim floats that attn_phase does not use, and
+// mega_spare_bytes() follows it unused: together they keep the ring depth and the cache capacity
+// at which decode gives way to the per-phase kernels where they were measured.
 static size_t mega_attn_scratch(const DecodeDims& d) {
   const size_t att = ((size_t)MEGA_ATT_G * cdiv(d.cap, ATT_UN) + (size_t)8 * MEGA_ATT_G * d.hd +
-                      (size_t)(MEGA_ATT_G + 2) * d.hd /* dataflow mode: q, new k, new v */) * 4;
+                      (size_t)(MEGA_ATT_G + 2) * d.hd) * 4;
   const size_t xs = (size_t)max(max(d.inter, d.hidden), d.n_heads * d.hd) * 2;
   return ((att > xs ? att : xs) + 127) & ~(size_t)127;
 }
+static size_t mega_spare_bytes(const DecodeDims& d) { return ((size_t)d.hidden * 2 + 127) & ~(size_t)127; }
 
 int mega_fill(MegaP& p, int sm_count) {
   const DecodeDims& d = p.d;
   int rc;
-  B200_REQUIRE(!p.qk_norm || (!p.flow && (d.hd == 64 || d.hd == 128)),
-               "mega: q/k norm needs the barrier mode (not dataflow) and head_dim 64 | 128");
   const int half = d.hd / 2;
   if ((rc = mega_geometry(p.ph[PH_QKV], d.hidden, 0, true, half))) return rc;
   B200_REQUIRE(half % p.ph[PH_QKV].R == 0, "mega: head_dim/2 %% tile rows != 0");
@@ -571,8 +491,7 @@ int mega_fill(MegaP& p, int sm_count) {
   B200_REQUIRE(d.hd == 64 || d.hd == 128, "mega: head_dim %d (64|128)", d.hd);
   const size_t scratch = mega_attn_scratch(d);
   p.scratch_bytes = (int)scratch;
-  const size_t hraw = ((size_t)d.hidden * 2 + 127) & ~(size_t)127;  // dataflow mode: raw residual stream
-  const long budget = 227 * 1024 - 2048 - (long)scratch - (long)hraw;
+  const long budget = 227 * 1024 - 2048 - (long)scratch - (long)mega_spare_bytes(d);
   int ns = (int)(budget / MEGA_STAGE);
   B200_REQUIRE(ns >= 2, "mega: cache capacity %d leaves no room for the weight ring", d.cap);
   p.n_stages = ns > 8 ? 8 : ns;
@@ -582,17 +501,17 @@ int mega_fill(MegaP& p, int sm_count) {
 
 static int mega_chx(const MegaPhase& g) { return cdiv(cdiv(g.K >> 3, g.S), 32); }
 
-template <int CHH, int CHI, bool FLOW>
-static int mega_launch_f(const MegaP& p, int grid, size_t smem, cudaStream_t s) {
+template <int CHH, int CHI>
+static int launch_k_mega(const MegaP& p, int grid, size_t smem, cudaStream_t s) {
   // the function attributes are per device (a second engine on another GPU of the same process
   // must opt in again)
   static unsigned long long set_mask = 0ull;
   int dev = 0;
   B200_CUDA(cudaGetDevice(&dev));
   if (!(set_mask >> (dev & 63) & 1ull)) {
-    B200_CUDA(cudaFuncSetAttribute(k_mega<CHH, CHI, FLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    B200_CUDA(cudaFuncSetAttribute(k_mega<CHH, CHI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    227 * 1024 - 2048));
-    B200_CUDA(cudaFuncSetAttribute(k_mega<CHH, CHI, FLOW>, cudaFuncAttributePreferredSharedMemoryCarveout,
+    B200_CUDA(cudaFuncSetAttribute(k_mega<CHH, CHI>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                    cudaSharedmemCarveoutMaxShared));
     set_mask |= 1ull << (dev & 63);
   }
@@ -609,18 +528,12 @@ static int mega_launch_f(const MegaP& p, int grid, size_t smem, cudaStream_t s) 
   at[0].val.cooperative = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  B200_CUDA(cudaLaunchKernelEx(&cfg, k_mega<CHH, CHI, FLOW>, p));
+  B200_CUDA(cudaLaunchKernelEx(&cfg, k_mega<CHH, CHI>, p));
   return B200_OK;
-}
-template <int CHH, int CHI>
-static int mega_launch_t(const MegaP& p, int grid, size_t smem, cudaStream_t s) {
-  return p.flow ? mega_launch_f<CHH, CHI, true>(p, grid, smem, s)
-                : mega_launch_f<CHH, CHI, false>(p, grid, smem, s);
 }
 
 int mega_launch(const MegaP& p, int sm_count, cudaStream_t s) {
-  const size_t smem = (size_t)p.n_stages * MEGA_STAGE + mega_attn_scratch(p.d) +
-                      (((size_t)p.d.hidden * 2 + 127) & ~(size_t)127);
+  const size_t smem = (size_t)p.n_stages * MEGA_STAGE + mega_attn_scratch(p.d) + mega_spare_bytes(p.d);
   int chh = mega_chx(p.ph[PH_QKV]);
   chh = max(chh, mega_chx(p.ph[PH_ORES]));
   chh = max(chh, mega_chx(p.ph[PH_GATEUP]));
@@ -628,10 +541,10 @@ int mega_launch(const MegaP& p, int sm_count, cudaStream_t s) {
   const int chi = mega_chx(p.ph[PH_DRES]);
   // every CTA must be resident at once (software grid barrier): one CTA per SM
   const int grid = sm_count;
-  if (chh <= 2 && chi <= 2) return mega_launch_t<2, 2>(p, grid, smem, s);
-  if (chh <= 6 && chi <= 10) return mega_launch_t<6, 10>(p, grid, smem, s);
-  if (chh <= 8 && chi <= 10) return mega_launch_t<8, 10>(p, grid, smem, s);  // Qwen2-VL-7B widths
-  if (chh <= 10 && chi <= 10) return mega_launch_t<10, 10>(p, grid, smem, s);
+  if (chh <= 2 && chi <= 2) return launch_k_mega<2, 2>(p, grid, smem, s);
+  if (chh <= 6 && chi <= 10) return launch_k_mega<6, 10>(p, grid, smem, s);
+  if (chh <= 8 && chi <= 10) return launch_k_mega<8, 10>(p, grid, smem, s);  // Qwen2-VL-7B widths
+  if (chh <= 10 && chi <= 10) return launch_k_mega<10, 10>(p, grid, smem, s);
   set_error("mega: unsupported widths (hidden chunks %d, inter chunks %d per lane)", chh, chi);
   return B200_ERR_INVALID;
 }

@@ -107,7 +107,6 @@ struct b200_engine {
   KvRef* kvref = nullptr;       // device: where the bound pool row lives (read by the captured prefill)
   KvRef* kvref_host = nullptr;  // pinned staging
   cudaEvent_t kvref_ev = nullptr;
-  bool v2 = true;               // weight-major GEMMs + pipelined attention (B200_PREFILL_V1=1: round-1 path)
   int log_cap = 1 << 16;
   // host mirrors of the decode state
   int ctx_host = 0, pos_host = 0;
@@ -122,20 +121,9 @@ struct b200_engine {
   int attn_cluster = 8;
   int prepared_cap = -1, prepared_cluster = -1;
   // megakernel
-  int use_mega = 1;  // 0: one kernel per phase, 1: k_mega (CUDA cores), 2: k_mega_tc (wgmma)
+  int use_mega = 1;  // 0: one kernel per phase, 1: k_mega
   bool mega_fits = true;  // false: this shape / cache capacity does not fit the persistent kernel
-  int active_mega() const { return mega_fits ? use_mega : 0; }
-  MegaTcP tp;
-  uint8_t* packed = nullptr;  // tile images of the LM weights (k_mega_tc)
-  size_t packed_bytes = 0;
-  bool packed_ready = false;
-  long long* tc_acc = nullptr;  // fixed-point split-K accumulators (k_mega_tc)
-  long tc_acc_rows = 0;
-  int tc_alias = 1;
-  int tc_inflight = 2;
-  int fma_inflight = 0, l2_prefetch = 0, l2_skip = 2;
-  int flow = 0;  // k_mega dataflow mode (set_mega(4) / B200_MEGA_FLOW=1): measured slower, see DESIGN.md
-  unsigned long long* flow_words = nullptr;
+  bool active_mega() const { return mega_fits && use_mega; }
   float* att_part = nullptr;
   float* att_stats = nullptr;
   unsigned long long* bar = nullptr;
@@ -265,9 +253,7 @@ static void invalidate_graph(b200_engine* e) {
 static int mega_prepare(b200_engine* e, cudaStream_t s) {
   const auto& c = e->cfg;
   B200_REQUIRE(c.n_layers <= MEGA_MAX_LAYERS, "mega: %d layers > %d", c.n_layers, MEGA_MAX_LAYERS);
-  B200_REQUIRE(!e->q8.codes, "mega: the persistent kernels read a bf16 KV pool; an 8-bit pool runs the per-phase kernels");
-  B200_REQUIRE(!e->qk_norm || e->use_mega == 1,
-               "mega: k_mega_tc has no q/k norm (Qwen3-VL); such a model runs k_mega or the per-phase kernels");
+  B200_REQUIRE(!e->q8.codes, "mega: the persistent kernel reads a bf16 KV pool; an 8-bit pool runs the per-phase kernels");
   if (!e->bar) {
     B200_CUDA(cudaMalloc(&e->bar, sizeof(unsigned long long)));
     B200_CUDA(cudaMemset(e->bar, 0, sizeof(unsigned long long)));
@@ -297,83 +283,8 @@ static int mega_prepare(b200_engine* e, cudaStream_t s) {
     p.qn[l] = e->qn[l];
     p.kn[l] = e->kn[l];
   }
-  // tuning aids
-  p.max_inflight = e->fma_inflight;
-  p.flow = e->flow;
-  {
-    const size_t nh = (size_t)c.hidden, nq = (size_t)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim / 2;
-    if (!e->flow_words) {
-      B200_CUDA(cudaMalloc(&e->flow_words, (2 * nh + nq) * sizeof(unsigned long long)));
-      B200_CUDA(cudaMemset(e->flow_words, 0, (2 * nh + nq) * sizeof(unsigned long long)));
-    }
-    p.hmid_w = e->flow_words;
-    p.hout_w = e->flow_words + nh;
-    p.qkv_w = e->flow_words + 2 * nh;
-  }
-  p.l2_prefetch = e->l2_prefetch;
-  p.l2_skip = e->l2_skip;
   int rc;
-  if (e->use_mega == 2) {
-    // ---- tensor-core variant: tile images of the weights + split-K partial buffers ----
-    const int QKV = (c.n_heads + 2 * c.n_kv_heads) * c.head_dim, H = c.hidden, I = c.inter;
-    const int OK_ = c.n_heads * c.head_dim;
-    const size_t b_qkv = mega_tc_packed_bytes(QKV, H, false), b_o = mega_tc_packed_bytes(H, OK_, false);
-    const size_t b_gu = mega_tc_packed_bytes(I, H, true), b_d = mega_tc_packed_bytes(H, I, false);
-    const size_t b_head = mega_tc_packed_bytes(c.vocab, H, false);
-    const size_t total = (size_t)c.n_layers * (b_qkv + b_o + b_gu + b_d) + b_head;
-    if (!e->packed || e->packed_bytes < total) {
-      if (e->packed) cudaFree(e->packed);
-      e->packed = nullptr;
-      B200_CUDA(cudaMalloc(&e->packed, total));
-      e->packed_bytes = total;
-      e->packed_ready = false;
-    }
-    MegaTcP& P = e->tp;
-    memset(&P, 0, sizeof(P));
-    uint8_t* w = e->packed;
-    for (int l = 0; l < c.n_layers; ++l) {
-      const LayerW& lw = e->layers[l];
-      LayerWT& lt = P.lt[l];
-      lt.wqkv = w; w += b_qkv;
-      lt.wo = w; w += b_o;
-      lt.wgu = w; w += b_gu;
-      lt.wd = w; w += b_d;
-      if (!e->packed_ready) {
-        if ((rc = mega_tc_pack(lw.wqkv, nullptr, QKV, H, false, (void*)lt.wqkv, s))) return rc;
-        if ((rc = mega_tc_pack(lw.wo, nullptr, H, OK_, false, (void*)lt.wo, s))) return rc;
-        if ((rc = mega_tc_pack(lw.wgu, lw.wgu + (long)I * H, I, H, true, (void*)lt.wgu, s))) return rc;
-        if ((rc = mega_tc_pack(lw.wd, nullptr, H, I, false, (void*)lt.wd, s))) return rc;
-      }
-    }
-    P.head_t = w;
-    if (!e->packed_ready)
-      if ((rc = mega_tc_pack(e->head, nullptr, c.vocab, H, false, (void*)w, s))) return rc;
-    e->packed_ready = true;
-    const long acc_rows = ((long)(QKV > H ? QKV : H) + 127) & ~127L;
-    if (!e->tc_acc || e->tc_acc_rows < acc_rows) {
-      if (e->tc_acc) cudaFree(e->tc_acc);
-      e->tc_acc = nullptr;
-      B200_CUDA(cudaMalloc(&e->tc_acc, (size_t)3 * acc_rows * sizeof(long long)));
-      e->tc_acc_rows = acc_rows;
-    }
-    // the kernel keeps the accumulators zero between uses; (re)establish that here
-    B200_CUDA(cudaMemsetAsync(e->tc_acc, 0, (size_t)3 * acc_rows * sizeof(long long), s));
-    P.qkv_acc = e->tc_acc;
-    P.o_acc = e->tc_acc + acc_rows;
-    P.d_acc = e->tc_acc + 2 * acc_rows;
-    P.max_inflight = e->tc_inflight;  // clamped below to n_stages - 1 (a lagging slot must not be reused)
-    P.x_kstride = e->tc_alias ? 1024 : 2048;
-    P.x_sbo = e->tc_alias ? 0 : 1024;
-    P.base = p;
-    if ((rc = mega_tc_fill(P, e->sm_count))) return rc;
-    if (P.max_inflight > P.base.n_stages - 1) P.max_inflight = P.base.n_stages - 1;
-    if (P.max_inflight < 1) P.max_inflight = 1;
-    e->mega_ready = true;
-    return B200_OK;
-  }
-  rc = mega_fill(p, e->sm_count);
-  if (rc) return rc;
-  if (p.max_inflight >= p.n_stages) p.max_inflight = p.n_stages - 1;  // a lagging slot must not be reused
+  if ((rc = mega_fill(p, e->sm_count))) return rc;
   e->mega_ready = true;
   return B200_OK;
 }
@@ -383,7 +294,6 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
   const DecodeDims d = e->dims();
   const auto& c = e->cfg;
   int rc;
-  if (e->active_mega() == 2) return mega_tc_launch(e->tp, e->sm_count, s);
   if (e->active_mega()) return mega_launch(e->mp, e->sm_count, s);
   if (e->q8.codes) {
     bf16* sk = e->q8_stage;
@@ -427,12 +337,65 @@ static int kernels_per_step(const b200_engine* e) {
 
 
 // ---------------------------------------------------------------------------------------------
-// round-2 prefill / vision path: weight-major GEMMs (gemm_wt.cu), split-K partials finished by
+// prefill / vision path: weight-major GEMMs (gemm_wt.cu), split-K partials finished by
 // finish_rows (bias + residual + the NEXT norm fused), pipelined attention (attention_fa.cu)
 // ---------------------------------------------------------------------------------------------
 static long align256(long x) { return (x + 255) & ~255L; }
 static const long WT_PARTIAL_BYTES = 48L << 20;  // fp32 split-K partial tiles (bounded: see gemm_wt_auto)
 static long round8(long x) { return (x + 7) & ~7L; }
+
+// Workspace layout, the one place that knows it: byte offsets of the buffers of an LM prefill of T tokens
+// and of a vision tower call of N patches.  Both start at the workspace base; the fp32 split-K partials
+// (ws_partial) sit at its end.
+struct WsCarver {
+  long end = 0;
+  long take(long bytes) {
+    const long at = end;
+    end += align256(bytes);
+    return at;
+  }
+};
+struct LmWs {
+  long h, xn, qkv, att, act, pos, vt, kws, end;
+};
+static LmWs lm_ws(const b200_qwen2vl_config& c, long T) {
+  const long QKV = (long)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim, QH = (long)c.n_heads * c.head_dim;
+  WsCarver w;
+  LmWs o;
+  o.h = w.take(T * c.hidden * 2);    // residual stream (graph input: the embeddings)
+  o.xn = w.take(T * c.hidden * 2);   // normalised rows
+  o.qkv = w.take(T * QKV * 2);
+  o.att = w.take(T * QH * 2);
+  // T x 2 x inter bf16 that no kernel addresses.  Without it the batched prefill of
+  // test_qwen3_vl_gpu::test_lock_step_rows_equal_single_requests[tiny] samples a wrong first token (the same
+  // bytes placed after `kws` also pass): kept until that dependency is found.
+  w.take(T * 2L * c.inter * 2);
+  o.act = w.take(T * c.inter * 2);   // SwiGLU output
+  o.pos = w.take(3L * T * 4);        // position ids (graph input)
+  o.vt = w.take((long)c.n_kv_heads * c.head_dim * round8(T) * 2);  // V^T of the prompt chunk
+  o.kws = w.take((long)c.n_kv_heads * c.head_dim * T * 2);         // rotated K of the prompt chunk
+  o.end = w.end;
+  return o;
+}
+struct TowerWs {
+  long x, h, y, qkv, mlp, att, vt, xin, fout, end;
+};
+static TowerWs tower_ws(const b200_qwen2vl_config& c, long N) {
+  const long E = c.v_embed;
+  WsCarver w;
+  TowerWs o;
+  o.x = w.take(N * c.v_patch_dim * 2);  // bf16 patches, then the rotary cos / sin table
+  o.h = w.take(N * E * 2);
+  o.y = w.take(N * E * 2);
+  o.qkv = w.take(N * 3 * E * 2);
+  o.mlp = w.take(N * (long)c.v_mlp * 2);
+  o.att = w.take(N * E * 2);
+  o.vt = w.take(E * round8(N) * 2);                // V^T of the tower
+  o.xin = w.take(N * c.v_patch_dim * 4);           // staged fp32 pixel_values (graph input)
+  o.fout = w.take((N / ((long)c.v_merge * c.v_merge) + 1) * c.v_out * 2);  // staged features (graph output)
+  o.end = w.end;
+  return o;
+}
 // creation-time helper: a bf16 buffer of -inf (the padding of logits rows beyond an odd vocabulary)
 static int fill_bf16_neg_inf(void* dst, long n) {
   std::vector<uint16_t> host((size_t)n, (uint16_t)0xFF80);
@@ -444,17 +407,17 @@ static float* ws_partial(b200_engine* e) {
 }
 
 // y = epi(bf16(x . W^T + b))
-static int v2_linear(b200_engine* e, const bf16* x, long ldx, const bf16* W, const bf16* b, bf16* y, long ldy,
-                     int T, int N, int K, int epi, cudaStream_t s) {
+static int linear(b200_engine* e, const bf16* x, long ldx, const bf16* W, const bf16* b, bf16* y, long ldy,
+                  int T, int N, int K, int epi, cudaStream_t s) {
   e->launches += 1;
   return gemm_wt_tuned(x, ldx, W, b, nullptr, 0, y, ldy, nullptr, 0, T, N, K, epi, B200_WT_BF16, 0, false,
                        e->sm_count, nullptr, s);
 }
 
 // h = bf16(h + bf16(x . W^T + b)); xn = norm(h)   (split-K GEMM + one finishing row op)
-static int v2_linear_residual_norm(b200_engine* e, const bf16* x, long ldx, const bf16* W, const bf16* b,
-                                   bf16* h, long ldh, int norm_kind, const bf16* nw, const bf16* nb, float eps,
-                                   bf16* xn, long ldxn, int T, int N, int K, cudaStream_t s) {
+static int linear_residual_norm(b200_engine* e, const bf16* x, long ldx, const bf16* W, const bf16* b,
+                                bf16* h, long ldh, int norm_kind, const bf16* nw, const bf16* nb, float eps,
+                                bf16* xn, long ldxn, int T, int N, int K, cudaStream_t s) {
   float* P = ws_partial(e);
   int split = 1;
   int rc;
@@ -476,7 +439,7 @@ static int v2_linear_residual_norm(b200_engine* e, const bf16* x, long ldx, cons
   return finish_rows(P, split, b, h, ldh, h, ldh, norm_kind, nw, nb, eps, xn, ldxn, T, N, s);
 }
 
-static int v2_upload_pos(b200_engine* e, const std::vector<int>& pos, cudaStream_t s) {
+static int upload_pos(b200_engine* e, const std::vector<int>& pos, cudaStream_t s) {
   const long n = (long)pos.size();
   if (n > e->pos_hw_cap) {
     if (e->pos_hw) B200_CUDA(cudaFree(e->pos_hw));
@@ -579,50 +542,47 @@ static int seq_run(b200_engine* e, std::vector<b200_engine::SeqGraph>& cache, co
   return B200_OK;
 }
 
-static int vision_v2_body(b200_engine* e, const float* pixel_values, const int* grid, int n_images, long N,
-                          void* feats_out, cudaStream_t s);
+static int vision_body(b200_engine* e, const float* pixel_values, const int* grid, int n_images, long N,
+                       void* feats_out, cudaStream_t s);
 
-static int vision_v2(b200_engine* e, const float* pixel_values, const int* grid, int n_images, long N,
-                     void* feats_out, cudaStream_t s) {
+static int vision(b200_engine* e, const float* pixel_values, const int* grid, int n_images, long N,
+                  void* feats_out, cudaStream_t s) {
   const auto& c = e->cfg;
   // graph input / output live at fixed workspace addresses: stage them around the captured body
-  uint8_t* p = e->ws;
-  p += align256(N * (long)c.v_patch_dim * 2) + 2 * align256(N * (long)c.v_embed * 2) +
-       align256(N * 3L * c.v_embed * 2) + align256(N * (long)c.v_mlp * 2) + align256(N * (long)c.v_embed * 2) +
-       align256((long)c.v_embed * round8(N) * 2);
-  float* xin = (float*)p; p += align256(N * (long)c.v_patch_dim * 4);
-  bf16* fout = (bf16*)p;
+  const TowerWs w = tower_ws(c, N);
+  float* xin = (float*)(e->ws + w.xin);
+  bf16* fout = (bf16*)(e->ws + w.fout);
   const long Nm = N / ((long)c.v_merge * c.v_merge);
   int rc;
   std::vector<int> pos;
   build_pos_hw(grid, n_images, c.v_merge, &pos);
-  if ((rc = v2_upload_pos(e, pos, s))) return rc;
+  if ((rc = upload_pos(e, pos, s))) return rc;
   B200_CUDA(cudaMemcpyAsync(xin, pixel_values, (size_t)N * c.v_patch_dim * 4, cudaMemcpyDeviceToDevice, s));
   std::vector<long> key = {(long)(uintptr_t)e->ws, (long)e->ws_bytes, N, (long)n_images, (long)(uintptr_t)e->pos_hw};
   for (int i = 0; i < n_images * 3; ++i) key.push_back(grid[i]);
-  rc = seq_run(e, e->vis_graphs, key, s, [&]() { return vision_v2_body(e, xin, grid, n_images, N, fout, s); });
+  rc = seq_run(e, e->vis_graphs, key, s, [&]() { return vision_body(e, xin, grid, n_images, N, fout, s); });
   if (rc) return rc;
   B200_CUDA(cudaMemcpyAsync(feats_out, fout, (size_t)Nm * c.v_out * 2, cudaMemcpyDeviceToDevice, s));
   return B200_OK;
 }
 
-static int vision_v2_body(b200_engine* e, const float* pixel_values, const int* grid, int n_images, long N,
-                          void* feats_out, cudaStream_t s) {
+static int vision_body(b200_engine* e, const float* pixel_values, const int* grid, int n_images, long N,
+                       void* feats_out, cudaStream_t s) {
   const auto& c = e->cfg;
   const long E = c.v_embed, Em = c.v_mlp;
   const int nh = c.v_heads, hd = c.v_embed / c.v_heads;
   const int t_ld = (int)round8(N);
-  uint8_t* p = e->ws;
-  bf16* x = (bf16*)p; p += align256(N * (long)c.v_patch_dim * 2);
-  bf16* h = (bf16*)p; p += align256(N * E * 2);
-  bf16* y = (bf16*)p; p += align256(N * E * 2);
-  bf16* qkv = (bf16*)p; p += align256(N * 3 * E * 2);
-  bf16* mlp = (bf16*)p; p += align256(N * Em * 2);
-  bf16* att = (bf16*)p; p += align256(N * E * 2);
-  bf16* vt = (bf16*)p; p += align256(E * (long)t_ld * 2);
+  const TowerWs w = tower_ws(c, N);
+  bf16* x = (bf16*)(e->ws + w.x);
+  bf16* h = (bf16*)(e->ws + w.h);
+  bf16* y = (bf16*)(e->ws + w.y);
+  bf16* qkv = (bf16*)(e->ws + w.qkv);
+  bf16* mlp = (bf16*)(e->ws + w.mlp);
+  bf16* att = (bf16*)(e->ws + w.att);
+  bf16* vt = (bf16*)(e->ws + w.vt);
   int rc;
   if ((rc = cast_f32_bf16(pixel_values, x, N * c.v_patch_dim, s))) return rc;
-  if ((rc = v2_linear(e, x, c.v_patch_dim, e->v_patch, nullptr, h, E, (int)N, (int)E, c.v_patch_dim, B200_EPI_NONE, s)))
+  if ((rc = linear(e, x, c.v_patch_dim, e->v_patch, nullptr, h, E, (int)N, (int)E, c.v_patch_dim, B200_EPI_NONE, s)))
     return rc;
   if ((rc = layer_norm(h, e->vblk[0].ln1w, e->vblk[0].ln1b, y, (int)N, (int)E, c.v_ln_eps, s))) return rc;
   e->launches += 2;
@@ -636,7 +596,7 @@ static int vision_v2_body(b200_engine* e, const float* pixel_values, const int* 
   }
   bool fa = attention_fa_supported(qkv, 3 * E, hd, qkv + E, 3 * E, hd, vt, (long)hd * t_ld, t_ld, att, E, hd);
   {  // the pipelined kernel loads V^T tiles with tokens innermost: a segment must start on a 16-byte boundary
-     // (8 tokens); frames with other offsets (e.g. a 6 x 6-patch image followed by another) take the round-1 kernel
+     // (8 tokens); frames with other offsets (e.g. a 6 x 6-patch image followed by another) take `attention()`
     long o = 0;
     for (int im = 0; im < n_images && fa; ++im)
       for (int tt = 0; tt < grid[im * 3]; ++tt) {
@@ -646,7 +606,7 @@ static int vision_v2_body(b200_engine* e, const float* pixel_values, const int* 
   }
   for (int i = 0; i < c.v_depth; ++i) {
     const VBlk& b = e->vblk[i];
-    if ((rc = v2_linear(e, y, E, b.qkvw, b.qkvb, qkv, 3 * E, (int)N, (int)(3 * E), (int)E, B200_EPI_NONE, s))) return rc;
+    if ((rc = linear(e, y, E, b.qkvw, b.qkvb, qkv, 3 * E, (int)N, (int)(3 * E), (int)E, B200_EPI_NONE, s))) return rc;
     if (fa) {
       if ((rc = vision_qkv_post(qkv, e->pos_hw, e->v_inv_freq, (int)N, nh, hd, scale, vt, t_ld, s, rope_cs))) return rc;
     } else {
@@ -671,24 +631,24 @@ static int vision_v2_body(b200_engine* e, const float* pixel_values, const int* 
         e->launches += 1;
       }
     }
-    if ((rc = v2_linear_residual_norm(e, att, E, b.projw, b.projb, h, E, B200_NORM_LN, b.ln2w, b.ln2b, c.v_ln_eps,
-                                      y, E, (int)N, (int)E, (int)E, s)))
+    if ((rc = linear_residual_norm(e, att, E, b.projw, b.projb, h, E, B200_NORM_LN, b.ln2w, b.ln2b, c.v_ln_eps,
+                                   y, E, (int)N, (int)E, (int)E, s)))
       return rc;
-    if ((rc = v2_linear(e, y, E, b.fc1w, b.fc1b, mlp, Em, (int)N, (int)Em, (int)E, B200_EPI_GELU_FAST, s))) return rc;
+    if ((rc = linear(e, y, E, b.fc1w, b.fc1b, mlp, Em, (int)N, (int)Em, (int)E, B200_EPI_GELU_FAST, s))) return rc;
     const bool last = (i + 1 == c.v_depth);
     const bf16* nw = last ? e->m_lnw : e->vblk[i + 1].ln1w;
     const bf16* nb = last ? e->m_lnb : e->vblk[i + 1].ln1b;
-    if ((rc = v2_linear_residual_norm(e, mlp, Em, b.fc2w, b.fc2b, h, E, B200_NORM_LN, nw, nb,
-                                      last ? 1e-6f : c.v_ln_eps, y, E, (int)N, (int)E, (int)Em, s)))
+    if ((rc = linear_residual_norm(e, mlp, Em, b.fc2w, b.fc2b, h, E, B200_NORM_LN, nw, nb,
+                                   last ? 1e-6f : c.v_ln_eps, y, E, (int)N, (int)E, (int)Em, s)))
       return rc;
   }
   // PatchMerger (vision.py:105-120): y already holds LayerNorm(h) of the last block
   const long mg = (long)c.v_merge * c.v_merge * E;
   const long Nm = N / ((long)c.v_merge * c.v_merge);
-  if ((rc = v2_linear(e, y, mg, e->m_fc1w, e->m_fc1b, mlp, mg, (int)Nm, (int)mg, (int)mg, B200_EPI_GELU_EXACT, s)))
+  if ((rc = linear(e, y, mg, e->m_fc1w, e->m_fc1b, mlp, mg, (int)Nm, (int)mg, (int)mg, B200_EPI_GELU_EXACT, s)))
     return rc;
-  if ((rc = v2_linear(e, mlp, mg, e->m_fc2w, e->m_fc2b, (bf16*)feats_out, c.v_out, (int)Nm, c.v_out, (int)mg,
-                      B200_EPI_NONE, s)))
+  if ((rc = linear(e, mlp, mg, e->m_fc2w, e->m_fc2b, (bf16*)feats_out, c.v_out, (int)Nm, c.v_out, (int)mg,
+                   B200_EPI_NONE, s)))
     return rc;
   return B200_OK;
 }
@@ -696,24 +656,18 @@ static int vision_v2_body(b200_engine* e, const float* pixel_values, const int* 
 // one sequence of a batched prefill: tokens [off, off + T) of the concatenated batch go to KV pool row `row`
 struct PreSeg { int off, T, row; };
 
-static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ctx0, void* all_logits_out,
-                                  cudaStream_t s, const PreSeg* segs = nullptr, int n_seg = 0,
-                                  const void* tok_loc = nullptr);
+static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0, void* all_logits_out,
+                               cudaStream_t s, const PreSeg* segs = nullptr, int n_seg = 0,
+                               const void* tok_loc = nullptr);
 
-static int prefill_layers_v2(b200_engine* e, const void* embeds, const int* pos3, int T, int ctx0,
-                             void* all_logits_out, bf16** h_out, cudaStream_t s) {
+static int prefill_layers(b200_engine* e, const void* embeds, const int* pos3, int T, int ctx0,
+                          void* all_logits_out, cudaStream_t s) {
   const auto& c = e->cfg;
-  const long H = c.hidden, I = c.inter, QH = (long)c.n_heads * c.head_dim;
-  const long QKV = (long)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim;
-  uint8_t* p = e->ws;
-  bf16* h = (bf16*)p;
-  p += 2 * align256((long)T * H * 2) + align256((long)T * QKV * 2) + align256((long)T * QH * 2) +
-       align256((long)T * 2 * I * 2) + align256((long)T * I * 2);
-  int* pos_stage = (int*)p;
+  const LmWs w = lm_ws(c, T);
+  int* pos_stage = (int*)(e->ws + w.pos);
   // graph inputs at fixed workspace addresses: the embeddings (residual stream) and the position ids
-  B200_CUDA(cudaMemcpyAsync(h, embeds, (size_t)T * H * 2, cudaMemcpyDeviceToDevice, s));
+  B200_CUDA(cudaMemcpyAsync(e->ws + w.h, embeds, (size_t)T * c.hidden * 2, cudaMemcpyDeviceToDevice, s));
   B200_CUDA(cudaMemcpyAsync(pos_stage, pos3, (size_t)3 * T * 4, cudaMemcpyDeviceToDevice, s));
-  *h_out = h;
   // where the cache lives travels through device memory (the captured graph survives a new pool)
   if (!e->kvref) {
     B200_CUDA(cudaMalloc(&e->kvref, sizeof(KvRef)));
@@ -729,9 +683,9 @@ static int prefill_layers_v2(b200_engine* e, const void* embeds, const int* pos3
   B200_CUDA(cudaMemcpyAsync(e->kvref, e->kvref_host, sizeof(KvRef), cudaMemcpyHostToDevice, s));
   B200_CUDA(cudaEventRecord(e->kvref_ev, s));
   if (all_logits_out || ctx0 != 0 || e->pre_q8.codes)  // all-row logits / a later chunk / 8-bit write-through: plain launches
-    return prefill_layers_v2_body(e, pos_stage, T, ctx0, all_logits_out, s);
+    return prefill_layers_body(e, pos_stage, T, ctx0, all_logits_out, s);
   const std::vector<long> key = {(long)(uintptr_t)e->ws, (long)e->ws_bytes, (long)T};
-  return seq_run(e, e->pre_graphs, key, s, [&]() { return prefill_layers_v2_body(e, pos_stage, T, 0, nullptr, s); });
+  return seq_run(e, e->pre_graphs, key, s, [&]() { return prefill_layers_body(e, pos_stage, T, 0, nullptr, s); });
 }
 
 // segs == nullptr: ONE sequence bound to e->kv_row (graph-capturable: the cache is addressed through e->kvref).
@@ -739,22 +693,20 @@ static int prefill_layers_v2(b200_engine* e, const void* embeds, const int* pos3
 // axis — every GEMM / norm / SwiGLU runs once over all T tokens (the weights are streamed once for the whole
 // batch), M-RoPE + KV append scatter each token to (its row, its position) through `tok_loc`, and attention runs
 // per sequence on its own block of the shared q / K / V^T buffers (block-diagonal causal).
-static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ctx0, void* all_logits_out,
-                                  cudaStream_t s, const PreSeg* segs, int n_seg, const void* tok_loc) {
+static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0, void* all_logits_out,
+                               cudaStream_t s, const PreSeg* segs, int n_seg, const void* tok_loc) {
   const auto& c = e->cfg;
   const long H = c.hidden, I = c.inter, QH = (long)c.n_heads * c.head_dim;
   const long QKV = (long)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim;
   const int hd = c.head_dim, t_ld = (int)round8(T);
-  uint8_t* p = e->ws;
-  bf16* h = (bf16*)p; p += align256((long)T * H * 2);
-  bf16* xn = (bf16*)p; p += align256((long)T * H * 2);
-  bf16* qkv = (bf16*)p; p += align256((long)T * QKV * 2);
-  bf16* att = (bf16*)p; p += align256((long)T * QH * 2);
-  p += align256((long)T * 2 * I * 2);  // (gate/up buffer of the round-1 path)
-  bf16* act = (bf16*)p; p += align256((long)T * I * 2);
-  p += align256(3L * T * 4);
-  bf16* vt = (bf16*)p; p += align256((long)c.n_kv_heads * hd * t_ld * 2);
-  bf16* kws = (bf16*)p; p += align256((long)c.n_kv_heads * hd * T * 2);
+  const LmWs w = lm_ws(c, T);
+  bf16* h = (bf16*)(e->ws + w.h);
+  bf16* xn = (bf16*)(e->ws + w.xn);
+  bf16* qkv = (bf16*)(e->ws + w.qkv);
+  bf16* att = (bf16*)(e->ws + w.att);
+  bf16* act = (bf16*)(e->ws + w.act);
+  bf16* vt = (bf16*)(e->ws + w.vt);
+  bf16* kws = (bf16*)(e->ws + w.kws);
   int rc;
   if ((rc = rms_norm(h, e->layers[0].ln1, xn, T, (int)H, c.rms_eps, s))) return rc;
   e->launches += 1;
@@ -765,7 +717,7 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
     const LayerW& lw = e->layers[l];
     bf16* kc = e->kptr(l, e->kv_row);
     bf16* vc = e->vptr(l, e->kv_row);
-    if ((rc = v2_linear(e, xn, H, lw.wqkv, lw.bqkv, qkv, QKV, T, (int)QKV, (int)H, B200_EPI_NONE, s))) return rc;
+    if ((rc = linear(e, xn, H, lw.wqkv, lw.bqkv, qkv, QKV, T, (int)QKV, (int)H, B200_EPI_NONE, s))) return rc;
     if (e->qk_norm) {
       if ((rc = qk_norm(qkv, T, c.n_heads, c.n_kv_heads, hd, e->qn[l], e->kn[l], c.rms_eps, s))) return rc;
       e->launches += 1;
@@ -811,8 +763,8 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
     if (rc) return rc;
     e->launches += 2;
     }
-    if ((rc = v2_linear_residual_norm(e, att, QH, lw.wo, nullptr, h, H, B200_NORM_RMS, lw.ln2, nullptr, c.rms_eps, xn,
-                                      H, T, (int)H, (int)QH, s)))
+    if ((rc = linear_residual_norm(e, att, QH, lw.wo, nullptr, h, H, B200_NORM_RMS, lw.ln2, nullptr, c.rms_eps, xn,
+                                   H, T, (int)H, (int)QH, s)))
       return rc;
     {  // gate/up with SwiGLU fused in the epilogue
       if ((rc = gemm_wt_tuned(xn, H, lw.wgu, nullptr, nullptr, 0, act, I, nullptr, 0, T, (int)(2 * I), (int)H,
@@ -823,14 +775,14 @@ static int prefill_layers_v2_body(b200_engine* e, const int* pos3, int T, int ct
     const bool last = (l + 1 == c.n_layers);
     const bool want_norm = !last || all_logits_out;
     const bf16* nw = last ? e->norm : e->layers[l + 1].ln1;
-    if ((rc = v2_linear_residual_norm(e, act, I, lw.wd, nullptr, h, H, want_norm ? B200_NORM_RMS : B200_NORM_NONE, nw,
-                                      nullptr, c.rms_eps, xn, H, T, (int)H, (int)I, s)))
+    if ((rc = linear_residual_norm(e, act, I, lw.wd, nullptr, h, H, want_norm ? B200_NORM_RMS : B200_NORM_NONE, nw,
+                                   nullptr, c.rms_eps, xn, H, T, (int)H, (int)I, s)))
       return rc;
   }
   if (all_logits_out) {  // the reference computes the head on every row (ar.py:358); xn = final norm
     // rows of the caller's buffer are round8(vocab) apart (16-byte aligned rows for any vocabulary)
-    if ((rc = v2_linear(e, xn, H, e->head, nullptr, (bf16*)all_logits_out, round8(c.vocab), T, c.vocab, (int)H,
-                        B200_EPI_NONE, s)))
+    if ((rc = linear(e, xn, H, e->head, nullptr, (bf16*)all_logits_out, round8(c.vocab), T, c.vocab, (int)H,
+                     B200_EPI_NONE, s)))
       return rc;
   }
   return B200_OK;
@@ -870,8 +822,6 @@ int b200_engine_create(const b200_qwen2vl_config* cfg, int device, b200_engine**
   e->device = device;
   e->sm_count = sm;
   decode_set_sm_count(sm);
-  if (const char* v = getenv("B200_MEGA_FLOW")) e->flow = atoi(v) != 0;  // tuning aid (A/B)
-  if (const char* v = getenv("B200_PREFILL_V1")) e->v2 = atoi(v) == 0;    // A/B: round-1 prefill kernels
   if (const char* v = getenv("B200_SEQ_GRAPH")) e->seq_graphs = atoi(v) != 0;
   const auto& c = e->cfg;
   B200_CUDA(cudaMalloc(&e->st, sizeof(DecState)));
@@ -940,9 +890,6 @@ int b200_engine_destroy(b200_engine* e) {
   if (e->att_stats) cudaFree(e->att_stats);
   if (e->bar) cudaFree(e->bar);
   if (e->dbg) cudaFree(e->dbg);
-  if (e->packed) cudaFree(e->packed);
-  if (e->tc_acc) cudaFree(e->tc_acc);
-  if (e->flow_words) cudaFree(e->flow_words);
   if (e->q8_stage) cudaFree(e->q8_stage);
   if (e->batch) batch_decoder_destroy(e->batch);
   if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
@@ -959,7 +906,6 @@ int b200_engine_set_weight(b200_engine* e, const char* name, const void* ptr, lo
   e->wn[name] = n_elems;
   drop_seq_graphs(e);
   e->resolved = false;
-  e->packed_ready = false;
   invalidate_graph(e);
   return B200_OK;
 }
@@ -990,20 +936,7 @@ int b200_engine_set_axis_sel(b200_engine* e, const int* axis_sel_host) {
 }
 
 long b200_engine_workspace_bytes(const b200_engine* e, int max_tokens, int max_patches) {
-  const auto& c = e->cfg;
-  const long T = max_tokens, N = max_patches;
-  const long QKV = (long)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim;
-  long lm = align256(T * c.hidden * 2) * 2 + align256(T * QKV * 2) +
-            align256(T * (long)c.n_heads * c.head_dim * 2) + align256(T * 2L * c.inter * 2) +
-            align256(T * (long)c.inter * 2) + align256(3L * T * 4);
-  long v = align256(N * (long)c.v_patch_dim * 2) + align256(N * (long)c.v_embed * 2) * 2 +
-           align256(N * 3L * c.v_embed * 2) + align256(N * (long)c.v_mlp * 2) +
-           align256(N * (long)c.v_embed * 2);
-  lm += align256((long)c.n_kv_heads * c.head_dim * round8(T) * 2);  // V^T of the prompt chunk
-  lm += align256((long)c.n_kv_heads * c.head_dim * T * 2);          // rotated K of the prompt chunk
-  v += align256((long)c.v_embed * round8(N) * 2);                   // V^T of the vision tower
-  v += align256(N * (long)c.v_patch_dim * 4);                       // staged fp32 pixel_values (graph input)
-  v += align256((N / ((long)c.v_merge * c.v_merge) + 1) * c.v_out * 2);  // staged features (graph output)
+  const long lm = lm_ws(e->cfg, max_tokens).end, v = tower_ws(e->cfg, max_patches).end;
   return (lm > v ? lm : v) + WT_PARTIAL_BYTES + 4096;
 }
 
@@ -1066,7 +999,7 @@ int b200_engine_set_prefill_kvq_row(b200_engine* e, void* codes, void* scales, v
                "set_prefill_kvq_row: bad arguments");
   B200_REQUIRE(n_q8_layers >= 1 && n_q8_layers <= e->cfg.n_layers, "set_prefill_kvq_row: %d 8-bit layers of %d",
                n_q8_layers, e->cfg.n_layers);
-  B200_REQUIRE(e->kv && e->v2, "set_prefill_kvq_row: bind the bf16 pool first / round-1 prefill selected");
+  B200_REQUIRE(e->kv, "set_prefill_kvq_row: bind the bf16 pool first");
   B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && e->cfg.head_dim % group_size == 0,
                "set_prefill_kvq_row: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size,
                e->cfg.head_dim);
@@ -1086,7 +1019,7 @@ int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void*
     e->pre_q8 = KvqPlanes{};
     return B200_OK;
   }
-  B200_REQUIRE(e->kv && scales && biases && e->v2, "set_prefill_kvq: bind the bf16 pool first / round-1 prefill selected");
+  B200_REQUIRE(e->kv && scales && biases, "set_prefill_kvq: bind the bf16 pool first");
   B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && e->cfg.head_dim % group_size == 0,
                "set_prefill_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size,
                e->cfg.head_dim);
@@ -1140,77 +1073,7 @@ int b200_engine_vision(b200_engine* e, const float* pixel_values, const int* gri
   }
   B200_REQUIRE(e->ws && b200_engine_workspace_bytes(e, 1, (int)N) <= e->ws_bytes,
                "engine_vision: workspace too small for %ld patches", N);
-  if (e->v2) return vision_v2(e, pixel_values, grid_thw_host, n_images, N, feats_out, s);
-  const long E = c.v_embed, Em = c.v_mlp;
-  const int nh = c.v_heads, hd = c.v_embed / c.v_heads;
-  uint8_t* p = e->ws;
-  bf16* x = (bf16*)p; p += align256(N * (long)c.v_patch_dim * 2);
-  bf16* h = (bf16*)p; p += align256(N * E * 2);
-  bf16* y = (bf16*)p; p += align256(N * E * 2);
-  bf16* qkv = (bf16*)p; p += align256(N * 3 * E * 2);
-  bf16* mlp = (bf16*)p; p += align256(N * Em * 2);
-  bf16* att = (bf16*)p; p += align256(N * E * 2);
-  // position ids -> device
-  std::vector<int> pos;
-  build_pos_hw(grid_thw_host, n_images, c.v_merge, &pos);
-  if ((long)pos.size() > e->pos_hw_cap) {
-    if (e->pos_hw) B200_CUDA(cudaFree(e->pos_hw));
-    B200_CUDA(cudaMalloc(&e->pos_hw, pos.size() * 4));
-    e->pos_hw_cap = (long)pos.size();
-  }
-  B200_CUDA(cudaMemcpyAsync(e->pos_hw, pos.data(), pos.size() * 4, cudaMemcpyHostToDevice, s));
-  B200_CUDA(cudaStreamSynchronize(s));  // `pos` is a stack-lifetime pageable buffer
-
-  if ((rc = cast_f32_bf16(pixel_values, x, N * c.v_patch_dim, s))) return rc;
-  if ((rc = gemm_bf16_tn(x, c.v_patch_dim, e->v_patch, nullptr, nullptr, 0, h, E, (int)N, (int)E,
-                         c.v_patch_dim, B200_EPI_NONE, s)))
-    return rc;
-  e->launches += 2;
-  const float scale = 1.0f / sqrtf((float)hd);
-  for (int i = 0; i < c.v_depth; ++i) {
-    const VBlk& b = e->vblk[i];
-    if ((rc = layer_norm(h, b.ln1w, b.ln1b, y, (int)N, (int)E, c.v_ln_eps, s))) return rc;
-    if ((rc = gemm_bf16_tn(y, E, b.qkvw, b.qkvb, nullptr, 0, qkv, 3 * E, (int)N, (int)(3 * E),
-                           (int)E, B200_EPI_NONE, s)))
-      return rc;
-    if ((rc = vision_rope(qkv, e->pos_hw, e->v_inv_freq, (int)N, nh, hd, s))) return rc;
-    long off = 0;
-    for (int im = 0; im < n_images; ++im) {
-      const int t = grid_thw_host[im * 3];
-      const int seg = grid_thw_host[im * 3 + 1] * grid_thw_host[im * 3 + 2];
-      for (int tt = 0; tt < t; ++tt) {  // one attention segment per frame (vision.py:270-281)
-        const bf16* qb = qkv + off * 3 * E;
-        if ((rc = attention(qb, 3 * E, hd, qb + E, 3 * E, hd, qb + 2 * E, 3 * E, hd,
-                            att + off * E, E, nh, nh, hd, seg, seg, 0, scale, s)))
-          return rc;
-        off += seg;
-        e->launches += 1;
-      }
-    }
-    if ((rc = gemm_bf16_tn(att, E, b.projw, b.projb, h, E, h, E, (int)N, (int)E, (int)E,
-                           B200_EPI_NONE, s)))
-      return rc;
-    if ((rc = layer_norm(h, b.ln2w, b.ln2b, y, (int)N, (int)E, c.v_ln_eps, s))) return rc;
-    if ((rc = gemm_bf16_tn(y, E, b.fc1w, b.fc1b, nullptr, 0, mlp, Em, (int)N, (int)Em, (int)E,
-                           B200_EPI_GELU_FAST, s)))
-      return rc;
-    if ((rc = gemm_bf16_tn(mlp, Em, b.fc2w, b.fc2b, h, E, h, E, (int)N, (int)E, (int)Em,
-                           B200_EPI_NONE, s)))
-      return rc;
-    e->launches += 7;
-  }
-  // PatchMerger (vision.py:105-120)
-  const long mg = (long)c.v_merge * c.v_merge * E;
-  const long Nm = N / ((long)c.v_merge * c.v_merge);
-  if ((rc = layer_norm(h, e->m_lnw, e->m_lnb, y, (int)N, (int)E, 1e-6f, s))) return rc;
-  if ((rc = gemm_bf16_tn(y, mg, e->m_fc1w, e->m_fc1b, nullptr, 0, mlp, mg, (int)Nm, (int)mg,
-                         (int)mg, B200_EPI_GELU_EXACT, s)))
-    return rc;
-  if ((rc = gemm_bf16_tn(mlp, mg, e->m_fc2w, e->m_fc2b, nullptr, 0, feats_out, c.v_out, (int)Nm,
-                         c.v_out, (int)mg, B200_EPI_NONE, s)))
-    return rc;
-  e->launches += 3;
-  return B200_OK;
+  return vision(e, pixel_values, grid_thw_host, n_images, N, feats_out, s);
 }
 
 int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int T, int ctx0,
@@ -1228,60 +1091,8 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   B200_CUDA(cudaSetDevice(e->device));
   cudaStream_t s = (cudaStream_t)stream;
   const auto& c = e->cfg;
-  const long H = c.hidden, I = c.inter, QH = (long)c.n_heads * c.head_dim;
-  const long QKV = (long)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim;
-  uint8_t* p = e->ws;
-  bf16* h = (bf16*)p; p += align256((long)T * H * 2);
-  bf16* xn = (bf16*)p; p += align256((long)T * H * 2);
-  bf16* qkv = (bf16*)p; p += align256((long)T * QKV * 2);
-  bf16* att = (bf16*)p; p += align256((long)T * QH * 2);
-  bf16* gu = (bf16*)p; p += align256((long)T * 2 * I * 2);
-  bf16* act = (bf16*)p; p += align256((long)T * I * 2);
-  if (e->v2) {
-    if ((rc = prefill_layers_v2(e, embeds, pos3, T, ctx0, all_logits_out, &h, s))) return rc;
-  } else {
-  B200_CUDA(cudaMemcpyAsync(h, embeds, (size_t)T * H * 2, cudaMemcpyDeviceToDevice, s));
-  const float scale = 1.0f / sqrtf((float)c.head_dim);
-  const int S = ctx0 + T;
-  for (int l = 0; l < c.n_layers; ++l) {
-    const LayerW& lw = e->layers[l];
-    bf16* kc = e->kptr(l, e->kv_row);
-    bf16* vc = e->vptr(l, e->kv_row);
-    if ((rc = rms_norm(h, lw.ln1, xn, T, (int)H, c.rms_eps, s))) return rc;
-    if ((rc = gemm_bf16_tn(xn, H, lw.wqkv, lw.bqkv, nullptr, 0, qkv, QKV, T, (int)QKV, (int)H,
-                           B200_EPI_NONE, s)))
-      return rc;
-    if (e->qk_norm && (rc = qk_norm(qkv, T, c.n_heads, c.n_kv_heads, c.head_dim, e->qn[l], e->kn[l], c.rms_eps, s)))
-      return rc;
-    if ((rc = mrope_kv_write(qkv, pos3, e->lm_inv_freq, e->axis_sel, kc, vc, T, ctx0, e->kv_cap,
-                             c.n_heads, c.n_kv_heads, c.head_dim, s)))
-      return rc;
-    if ((rc = attention(qkv, QKV, c.head_dim, kc, c.head_dim, (long)e->kv_cap * c.head_dim, vc,
-                        c.head_dim, (long)e->kv_cap * c.head_dim, att, QH, c.n_heads,
-                        c.n_kv_heads, c.head_dim, T, S, 1, scale, s)))
-      return rc;
-    if ((rc = gemm_bf16_tn(att, QH, lw.wo, nullptr, h, H, h, H, T, (int)H, (int)QH, B200_EPI_NONE,
-                           s)))
-      return rc;
-    if ((rc = rms_norm(h, lw.ln2, xn, T, (int)H, c.rms_eps, s))) return rc;
-    if ((rc = gemm_bf16_tn(xn, H, lw.wgu, nullptr, nullptr, 0, gu, 2 * I, T, (int)(2 * I), (int)H,
-                           B200_EPI_NONE, s)))
-      return rc;
-    if ((rc = swiglu(gu, act, T, (int)I, s))) return rc;
-    if ((rc = gemm_bf16_tn(act, I, lw.wd, nullptr, h, H, h, H, T, (int)H, (int)I, B200_EPI_NONE,
-                           s)))
-      return rc;
-    e->launches += 9;
-  }
-  if (all_logits_out) {  // the reference computes the head on every row (ar.py:358)
-    if ((rc = rms_norm(h, e->norm, xn, T, (int)H, c.rms_eps, s))) return rc;
-    B200_REQUIRE(c.vocab % 8 == 0, "prefill (round-1 kernels): all-row logits need vocab %% 8 == 0");
-    if ((rc = gemm_bf16_tn(xn, H, e->head, nullptr, nullptr, 0, all_logits_out, c.vocab, T,
-                           c.vocab, (int)H, B200_EPI_NONE, s)))
-      return rc;
-    e->launches += 2;
-  }
-  }
+  if ((rc = prefill_layers(e, embeds, pos3, T, ctx0, all_logits_out, s))) return rc;
+  const bf16* h = (const bf16*)(e->ws + lm_ws(c, T).h);
   // last row through the fused head + sampler; arms the decode state
   const DecodeDims d = e->dims();
   if (e->prepared_cap != e->kv_cap || e->prepared_cluster != e->attn_cluster) {
@@ -1293,7 +1104,7 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   e->pos_host = ctx0 + T + rope_delta;
   if ((rc = launch_set_state(e->st, 0, e->ctx_host, e->pos_host, 0, 0, e->embed, e->h, c.hidden, s)))
     return rc;
-  if ((rc = launch_head(d, e->norm, e->head, h + (long)(T - 1) * H, e->logits, e->partials, s)))
+  if ((rc = launch_head(d, e->norm, e->head, h + (long)(T - 1) * c.hidden, e->logits, e->partials, s)))
     return rc;
   if ((rc = launch_sample(d, e->logits, e->partials, e->logprobs, e->embed, e->h, e->st,
                           e->token_log, e->log_cap, e->force, 0, s)))
@@ -1313,8 +1124,7 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_REQUIRE(e && embeds && pos3 && n_seq > 0 && seq_len && rows, "engine_prefill_batch: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv && !e->bq8.codes && e->v2,
-               "engine_prefill_batch: KV pool not bound / 8-bit batch pool bound / round-1 prefill kernels selected");
+  B200_REQUIRE(e->kv && !e->bq8.codes, "engine_prefill_batch: KV pool not bound / 8-bit batch pool bound");
   B200_REQUIRE(!e->pre_q8.codes, "engine_prefill_batch: no 8-bit write-through in the batched prefill");
   long T = 0;
   std::vector<PreSeg> segs(n_seq);
@@ -1331,13 +1141,10 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_CUDA(cudaSetDevice(e->device));
   cudaStream_t s = (cudaStream_t)stream;
   const auto& c = e->cfg;
-  const long H = c.hidden, I = c.inter, QH = (long)c.n_heads * c.head_dim;
-  const long QKV = (long)(c.n_heads + 2 * c.n_kv_heads) * c.head_dim;
-  uint8_t* p = e->ws;
-  bf16* h = (bf16*)p;
-  p += 2 * align256(T * H * 2) + align256(T * QKV * 2) + align256(T * QH * 2) + align256(T * 2 * I * 2) +
-       align256(T * I * 2);
-  int* pos_stage = (int*)p;   // 3 * T ints; the tokens' (row, position) table lives in e->loc_dev
+  const long H = c.hidden;
+  const LmWs w = lm_ws(c, T);
+  bf16* h = (bf16*)(e->ws + w.h);
+  int* pos_stage = (int*)(e->ws + w.pos);   // 3 * T ints; the tokens' (row, position) table lives in e->loc_dev
   B200_CUDA(cudaMemcpyAsync(h, embeds, (size_t)T * H * 2, cudaMemcpyDeviceToDevice, s));
   B200_CUDA(cudaMemcpyAsync(pos_stage, pos3, (size_t)3 * T * 4, cudaMemcpyDeviceToDevice, s));
   std::vector<int> loc(2 * (size_t)T, -1);   // padding tokens: row -1 = no cache write
@@ -1349,7 +1156,7 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   for (int g = 0; g < n_seq; ++g)   // attention segments (q0, Lq, k0, S), 16-byte aligned behind the table (T % 8 == 0)
     for (int v : {segs[g].off, segs[g].T, segs[g].off, segs[g].T}) loc.push_back(v);
   if ((rc = upload_loc(e, loc, s))) return rc;
-  rc = prefill_layers_v2_body(e, pos_stage, (int)T, 0, nullptr, s, segs.data(), n_seq, e->loc_dev);
+  rc = prefill_layers_body(e, pos_stage, (int)T, 0, nullptr, s, segs.data(), n_seq, e->loc_dev);
   B200_CUDA(cudaEventRecord(e->loc_ev, s));   // the table (and its staging copy) may be rewritten after this point
   if (rc) return rc;
   const DecodeDims d = e->dims();
@@ -1468,17 +1275,8 @@ int b200_engine_set_graph(b200_engine* e, int enabled) {
 }
 int b200_engine_set_mega(b200_engine* e, int enabled) {
   B200_REQUIRE(e, "set_mega: null engine");
-  B200_REQUIRE(enabled >= 0 && enabled <= 4,
-               "set_mega: mode %d (0 off, 1 k_mega, 2 k_mega_tc, 3 k_mega_tc with a 16-row operand, 4 k_mega dataflow)",
-               enabled);
-  e->use_mega = enabled == 3 ? 2 : (enabled == 4 ? 1 : enabled);
-  e->tc_alias = enabled == 3 ? 0 : 1;
-  e->flow = enabled == 4 ? 1 : 0;
-  if (const char* v = getenv("B200_TC_INFLIGHT")) e->tc_inflight = atoi(v) > 0 ? atoi(v) : 2;  // tuning aids
-  if (const char* v = getenv("B200_FMA_INFLIGHT")) e->fma_inflight = atoi(v);
-
-  if (const char* v = getenv("B200_L2_PREFETCH")) e->l2_prefetch = atoi(v);
-  if (const char* v = getenv("B200_L2_SKIP")) e->l2_skip = atoi(v);
+  B200_REQUIRE(enabled == 0 || enabled == 1, "set_mega: mode %d (0: one kernel per phase, 1: k_mega)", enabled);
+  e->use_mega = enabled;
   invalidate_graph(e);
   return B200_OK;
 }
@@ -1487,7 +1285,6 @@ int b200_engine_debug_buffer(b200_engine* e, const char* name, void** ptr, long*
   const std::string n(name);
   if (n == "h") { *ptr = e->h; *bytes = (long)e->cfg.hidden * 2; }
   else if (n == "act") { *ptr = e->act; *bytes = (long)e->cfg.inter * 2; }
-  else if (n == "tc_acc" && e->tc_acc) { *ptr = e->tc_acc; *bytes = 3 * e->tc_acc_rows * 8; }
   else {
     set_error("debug_buffer: unknown or unallocated buffer '%s'", name);
     return B200_ERR_INVALID;

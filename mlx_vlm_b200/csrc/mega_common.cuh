@@ -1,5 +1,4 @@
-// Device pieces shared by the two persistent decode kernels (k_mega: CUDA-core consumers,
-// decode_mega.cu; k_mega_tc: wgmma consumers, decode_mega_tc.cu): mbarrier / bulk-copy
+// Device pieces of the persistent decode kernel k_mega (decode_mega.cu): mbarrier / bulk-copy
 // wrappers, the software grid barrier, the distributed attention phase and the sampler.
 #pragma once
 #include "common.cuh"
@@ -59,48 +58,6 @@ __device__ __forceinline__ uint64_t policy_evict_first() {
 __device__ __forceinline__ uint4 ldcg16(const void* p) {
   return __ldcg(reinterpret_cast<const uint4*>(p));
 }
-// ---- self-validating activation words (dataflow mode of k_mega) -------------------------
-// A value that crosses CTAs inside a layer is published as an 8-byte word {payload << 32 |
-// epoch}; 8-byte accesses are single-copy atomic, the epoch is unique per (step, layer), so a
-// reader simply re-loads until the tag matches: barrier + load (3 dependent L2 round trips)
-// become one polled load.
-__device__ __forceinline__ void st_word(unsigned long long* p, uint32_t payload, uint32_t epoch) {
-  const unsigned long long w = ((unsigned long long)payload << 32) | epoch;
-  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
-}
-__device__ __forceinline__ void ld_word2(const unsigned long long* p, unsigned long long& a,
-                                         unsigned long long& b) {
-  asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(p) : "memory");
-}
-// 8 consecutive per-element words (payload = bf16 bits) -> one 16-byte vector of 8 bf16
-__device__ __forceinline__ uint4 poll8(const unsigned long long* w, uint32_t epoch, int* err) {
-  unsigned long long a[8];
-  unsigned spins = 0;
-  bool ok;
-  do {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) ld_word2(w + 2 * i, a[2 * i], a[2 * i + 1]);
-    ok = true;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) ok = ok && ((uint32_t)a[i] == epoch);
-    if (!ok) {
-      __nanosleep(200);  // back off: ~28k threads poll the same few KB of L2
-      if (++spins > (1u << 20)) {
-        *err = 4;
-        break;
-      }
-    }
-  } while (!ok);
-  uint4 v;
-  v.x = ((uint32_t)(a[0] >> 32) & 0xffffu) | ((uint32_t)(a[1] >> 32) << 16);
-  v.y = ((uint32_t)(a[2] >> 32) & 0xffffu) | ((uint32_t)(a[3] >> 32) << 16);
-  v.z = ((uint32_t)(a[4] >> 32) & 0xffffu) | ((uint32_t)(a[5] >> 32) << 16);
-  v.w = ((uint32_t)(a[6] >> 32) & 0xffffu) | ((uint32_t)(a[7] >> 32) << 16);
-  return v;
-}
-__device__ __forceinline__ uint32_t bf_bits(float x) {
-  return (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(x));
-}
 __device__ __forceinline__ float ldcg_bf(const bf16* p) {
   return __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const unsigned short*>(p)) << 16);
 }
@@ -138,19 +95,6 @@ constexpr int MEGA_THREADS = 288;
 constexpr int MEGA_STAGE = 48 * 1024;
 constexpr int MEGA_ATT_G = 4;
 constexpr int ATT_UN = 8;  // key ranges per (kv head, q-head group) in the attention phase
-// k_mega_tc: split-K partial sums are accumulated EXACTLY in 64-bit fixed point (2^-32 units)
-// with red.global.add.u64: the sum is independent of the arrival order (deterministic) and the
-// reader needs ONE load per row instead of one per split.  fp32 -> fixed is exact for
-// |v| >= 2^-9 and within 2^-33 absolute below; |v| < 2^31.
-constexpr float TC_FIX_SCALE = 4294967296.0f;
-constexpr float TC_FIX_INV = 1.0f / 4294967296.0f;
-__device__ __forceinline__ void fix_add(long long* acc, float v) {
-  const long long q = __float2ll_rn(v * TC_FIX_SCALE);
-  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(acc), "l"(q) : "memory");
-}
-__device__ __forceinline__ float fix_get(const long long* acc) {
-  return __ll2float_rn(__ldcg(acc)) * TC_FIX_INV;
-}
 
 struct MegaShared {
   uint64_t full_bar[8], empty_bar[8];
@@ -163,7 +107,6 @@ struct MegaShared {
   unsigned long long best;
   int feed;
   int err;
-  float invf[64];  // rotary inverse frequencies (k_mega_tc: no global round trip in the prologue)
 };
 
 // ring position shared by producer and consumers (each keeps its own copy)
@@ -199,25 +142,10 @@ namespace {
 // group) 15.9 us; one CTA per q head 17.1 us; every unit recomputing all scores 11.1 us;
 // counter barrier + last-arriver combine 10.6 us; one-warp statistics read, no combine 5.4 us;
 // polled statistics words 4.7 us.
-// PARTS (k_mega_tc): q / k / v of this step arrive as fixed-point split-K sums of the qkv
-// GEMV; the phase prologue finishes them (+ bias, round, rotary, q * scale) in shared
-// memory, the unit that owns the new key scores it from there and one CTA per kv head
-// appends it to the cache.
-struct AttnParts {
-  const long long* acc;  // PARTS: [qkv rows] fixed-point sums
-  const bf16* bias;
-  int pos;
-  // FLOW (k_mega dataflow mode): q / k / v of this step as finished, rotated bf16 PAIRS (dims j and
-  // j + hd/2 of a head) in self-validating words [head slot][hd/2]
-  const unsigned long long* qkvw;
-  uint32_t epoch;
-};
-
-enum { ATT_PLAIN = 0, ATT_PARTS = 1, ATT_FLOW = 2 };
-template <int HD, int AMODE>
+template <int HD>
 __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const bf16* vc,
                                            float* scratch, MegaShared* sh, int nkeys, int layer,
-                                           const AttnParts& ap, long long* tdbg = nullptr) {
+                                           long long* tdbg = nullptr) {
   int tn = 0;
 #define ATT_STAMP() do { if (tdbg && threadIdx.x == 0 && tn < 30) tdbg[tn++] = gtimer(); } while (0)
   ATT_STAMP();
@@ -239,25 +167,17 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
   const bf16* vb = vc + (long)kvh * d.cap * HD;
   const int per = (nkeys + ATT_UN - 1) / ATT_UN;
   const int u0 = min(nkeys, unit * per), u1 = min(nkeys, u0 + per);
-  constexpr bool PARTS = (AMODE != ATT_PLAIN);  // q / new k / new v come through shared memory
-  const bool owner = PARTS && (u1 == nkeys) && (u1 > u0);  // holds the new key (index nkeys-1)
-  const int u1g = u1 - (owner ? 1 : 0);                    // keys that are read from the cache
-  float* qs = red + (long)8 * AG * HD;                     // PARTS: [AG][HD] q * scale
-  float* kn = qs + (long)AG * HD;                          //        [HD] new key
-  float* vn = kn + HD;                                     //        [HD] new value
   const int seg = lane & 7, ksub = lane >> 3;
   // ---- all global requests of the phase are issued before the first use: q, the first
   // 2 x 4 keys of this warp, and the V rows of its first VPRE keys (one round trip) ----
   constexpr int VPRE = 8;
   uint4 qraw[AG][NV];
-  if (!PARTS) {
 #pragma unroll
-    for (int g = 0; g < AG; ++g)
+  for (int g = 0; g < AG; ++g)
 #pragma unroll
-      for (int v = 0; v < NV; ++v)
-        qraw[g][v] = (g < G) ? ldcg16(p.qbuf + (long)(h0 + g) * HD + seg * SEG + v * 8)
-                             : make_uint4(0, 0, 0, 0);
-  }
+    for (int v = 0; v < NV; ++v)
+      qraw[g][v] = (g < G) ? ldcg16(p.qbuf + (long)(h0 + g) * HD + seg * SEG + v * 8)
+                           : make_uint4(0, 0, 0, 0);
   uint4 kvn[UNR][NV];
   {
     const int j0 = u0 + warp * 4;
@@ -266,7 +186,7 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
       const int j = j0 + 32 * q + ksub;
 #pragma unroll
       for (int v = 0; v < NV; ++v)
-        kvn[q][v] = (j < u1g) ? ldcg16(kb + (long)j * HD + seg * SEG + v * 8) : make_uint4(0, 0, 0, 0);
+        kvn[q][v] = (j < u1) ? ldcg16(kb + (long)j * HD + seg * SEG + v * 8) : make_uint4(0, 0, 0, 0);
     }
   }
   uint2 vraw[VPRE];
@@ -274,117 +194,40 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
   for (int q = 0; q < VPRE; ++q) {
     const int j = u0 + warp + 8 * q;
     vraw[q] = make_uint2(0, 0);
-    if (j < u1g) {
+    if (j < u1) {
       const bf16* vr = vb + (long)j * HD + lane * EPL;
       if (EPL == 4) vraw[q] = __ldcg(reinterpret_cast<const uint2*>(vr));
       else vraw[q].x = __ldcg(reinterpret_cast<const uint32_t*>(vr));
     }
   }
   float qr[AG][SEG];
-  if (AMODE == ATT_FLOW) {
-    // poll the finished q (x scale) / new k / new v pairs published by the qkv phase
-    const int half = HD / 2;
-    const int nslot = G + (owner ? 2 : 0);
-    for (int i = threadIdx.x; i < nslot * half; i += 256) {
-      const int slot = i / half, j = i % half;
-      const int hs = (slot < G) ? (h0 + slot) : (slot == G ? d.n_heads + kvh : d.n_heads + d.n_kv + kvh);
-      const unsigned long long* wp = ap.qkvw + (long)hs * half + j;
-      unsigned long long w;
-      unsigned spins = 0;
-      do {
-        asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(w) : "l"(wp) : "memory");
-        if ((uint32_t)w != ap.epoch) {
-          __nanosleep(200);
-          if (++spins > (1u << 20)) {
-            sh->err = 4;
-            break;
-          }
-        }
-      } while ((uint32_t)w != ap.epoch);
-      const uint32_t pr = (uint32_t)(w >> 32);
-      float lo = __uint_as_float(pr << 16), hi = __uint_as_float(pr & 0xffff0000u);
-      float* dst = (slot < G) ? qs + (long)slot * HD : (slot == G ? kn : vn);
-      if (slot < G) {
-        lo = rbf(lo * d.scale_bf);
-        hi = rbf(hi * d.scale_bf);
-      }
-      dst[j] = lo;
-      dst[j + half] = hi;
+#pragma unroll
+  for (int g = 0; g < AG; ++g)
+#pragma unroll
+    for (int v = 0; v < NV; ++v) {
+      float f[8];
+      unpack8(qraw[g][v], f);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) qr[g][v * 8 + i] = rbf(f[i] * d.scale_bf);
     }
-    cbar();
-#pragma unroll
-    for (int g = 0; g < AG; ++g)
-#pragma unroll
-      for (int i = 0; i < SEG; ++i) qr[g][i] = (g < G) ? qs[(long)g * HD + seg * SEG + i] : 0.f;
-  } else if (PARTS) {
-    const int half = HD / 2;
-    const int nslot = G + (owner ? 2 : 0);
-    for (int i = threadIdx.x; i < nslot * HD; i += 256) {
-      const int slot = i / HD, j = i % HD;
-      const int row = (slot < G) ? (h0 + slot) * HD + j
-                                 : ((slot == G ? d.n_heads + kvh : d.n_heads + d.n_kv + kvh) * HD + j);
-      const float s = fix_get(ap.acc + row);
-      (slot < G ? qs + (long)slot * HD : (slot == G ? kn : vn))[j] = rbf(s + bf2f(ap.bias[row]));
-    }
-    cbar();
-    const int nrot = G + (owner ? 1 : 0);
-    for (int i = threadIdx.x; i < nrot * half; i += 256) {
-      const int slot = i / half, j = i % half;
-      float* v = (slot < G) ? qs + (long)slot * HD : kn;
-      const float y1 = v[j], y2 = v[j + half];
-      const float ang = (float)ap.pos * sh->invf[j];
-      const float c = rbf(cosf(ang)), sn = rbf(sinf(ang));
-      float o1 = rbf(rbf(y1 * c) + rbf((-y2) * sn));
-      float o2 = rbf(rbf(y2 * c) + rbf(y1 * sn));
-      if (slot < G) {
-        o1 = rbf(o1 * d.scale_bf);
-        o2 = rbf(o2 * d.scale_bf);
-      }
-      v[j] = o1;
-      v[j + half] = o2;
-    }
-    cbar();
-    if (owner && part == 0) {  // append the new position to the cache (one CTA per kv head)
-      bf16* kw = const_cast<bf16*>(kb) + (long)(nkeys - 1) * HD;
-      bf16* vw = const_cast<bf16*>(vb) + (long)(nkeys - 1) * HD;
-      for (int i = threadIdx.x; i < HD; i += 256) {
-        kw[i] = f2bf(kn[i]);
-        vw[i] = f2bf(vn[i]);
-      }
-    }
-#pragma unroll
-    for (int g = 0; g < AG; ++g)
-#pragma unroll
-      for (int i = 0; i < SEG; ++i) qr[g][i] = (g < G) ? qs[(long)g * HD + seg * SEG + i] : 0.f;
-  } else {
-#pragma unroll
-    for (int g = 0; g < AG; ++g)
-#pragma unroll
-      for (int v = 0; v < NV; ++v) {
-        float f[8];
-        unpack8(qraw[g][v], f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) qr[g][v * 8 + i] = rbf(f[i] * d.scale_bf);
-      }
-  }
   ATT_STAMP();  // q loaded
   // ---- 1. scores of the own range (software-pipelined over trips of 2 x 4 keys) ----
   float lm[AG];
 #pragma unroll
   for (int g = 0; g < AG; ++g) lm[g] = -INFINITY;
-  for (int j0 = u0 + warp * 4; j0 < u1g; j0 += 32 * UNR) {
+  for (int j0 = u0 + warp * 4; j0 < u1; j0 += 32 * UNR) {
     uint4 kv[UNR][NV];
 #pragma unroll
     for (int q = 0; q < UNR; ++q)
 #pragma unroll
       for (int v = 0; v < NV; ++v) kv[q][v] = kvn[q][v];
-    if (j0 + 32 * UNR < u1g) {
+    if (j0 + 32 * UNR < u1) {
 #pragma unroll
       for (int q = 0; q < UNR; ++q) {
         const int j = j0 + 32 * UNR + 32 * q + ksub;
 #pragma unroll
         for (int v = 0; v < NV; ++v)
-          kvn[q][v] = (j < u1g) ? ldcg16(kb + (long)j * HD + seg * SEG + v * 8)
+          kvn[q][v] = (j < u1) ? ldcg16(kb + (long)j * HD + seg * SEG + v * 8)
                                 : make_uint4(0, 0, 0, 0);
       }
     }
@@ -407,7 +250,7 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
       for (int o = 1; o < 8; o <<= 1)
 #pragma unroll
         for (int g = 0; g < AG; ++g) s[g] += __shfl_xor_sync(0xffffffffu, s[g], o);
-      if (j < u1g && seg == 0) {
+      if (j < u1 && seg == 0) {
 #pragma unroll
         for (int g = 0; g < AG; ++g) {
           const float r = rbf(s[g]);
@@ -415,19 +258,6 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
           lm[g] = fmaxf(lm[g], r);
         }
       }
-    }
-  }
-  if (PARTS && owner && warp == 0) {  // the new key: q . k from shared memory
-#pragma unroll
-    for (int g = 0; g < AG; ++g) {
-      float s = 0.f;
-#pragma unroll
-      for (int e = 0; e < EPL; ++e)
-        s = fmaf((g < G) ? qs[(long)g * HD + lane * EPL + e] : 0.f, kn[lane * EPL + e], s);
-      s = warp_sum(s);
-      const float r = rbf(s);
-      if (lane == 0) sc[(long)g * ucap + (nkeys - 1 - u0)] = r;
-      lm[g] = fmaxf(lm[g], r);
     }
   }
   ATT_STAMP();  // scores done
@@ -539,7 +369,7 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
 #pragma unroll
   for (int q = 0; q < VPRE; ++q) {
     const int j = u0 + warp + 8 * q;
-    if (j < u1g) {
+    if (j < u1) {
 #pragma unroll
       for (int g = 0; g < AG; ++g) {
         const float pj = sc[(long)g * ucap + (j - u0)];
@@ -548,22 +378,14 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
       }
     }
   }
-  if (PARTS && owner && warp == 0) {  // the new value row comes from shared memory
-#pragma unroll
-    for (int g = 0; g < AG; ++g) {
-      const float pj = sc[(long)g * ucap + (nkeys - 1 - u0)];
-#pragma unroll
-      for (int e = 0; e < EPL; ++e) acc[g][e] = fmaf(pj, vn[lane * EPL + e], acc[g][e]);
-    }
-  }
-  for (int j0 = u0 + warp + 8 * VPRE; j0 < u1g; j0 += 32) {  // 4 keys per trip, loads first
+  for (int j0 = u0 + warp + 8 * VPRE; j0 < u1; j0 += 32) {  // 4 keys per trip, loads first
     float vf[4][EPL];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int j = j0 + 8 * q;
 #pragma unroll
       for (int e = 0; e < EPL; ++e) vf[q][e] = 0.f;
-      if (j < u1g) {
+      if (j < u1) {
         const bf16* vr = vb + (long)j * HD + lane * EPL;
         if (EPL == 4) {
           float t4[4];
@@ -580,7 +402,7 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int j = j0 + 8 * q;
-      if (j < u1g) {
+      if (j < u1) {
 #pragma unroll
         for (int g = 0; g < AG; ++g) {
           const float pj = sc[(long)g * ucap + (j - u0)];

@@ -499,8 +499,7 @@ int mrope_kv_write(void* qkv, const int* pos3, const float* inv_freq, const int*
   B200_REQUIRE(T > 0 && ctx0 >= 0 && (ref || tok_loc || ctx0 + T <= cap), "mrope_kv_write: T=%d ctx0=%d cap=%d", T,
                ctx0, cap);
   B200_REQUIRE(!vt || t_ld >= T, "mrope_kv_write: V^T pitch %d < T %d", t_ld, T);
-  static const bool scalar_only = getenv("B200_MROPE_SCALAR") != nullptr;   // A/B and fallback
-  if (!scalar_only && (hd % 16) == 0 && hd <= 128 && (!vt || (t_ld % 8) == 0)) {
+  if ((hd % 16) == 0 && hd <= 128 && (!vt || (t_ld % 8) == 0)) {
     const int slots = n_heads + 2 * n_kv, tiles = (T + 31) / 32;
     int groups = (4 * 132 + tiles - 1) / tiles;          // about four waves of CTAs
     if (groups > slots) groups = slots;

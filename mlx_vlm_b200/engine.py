@@ -303,9 +303,8 @@ class Engine:
         N.check(self.lib.b200_engine_set_graph(self.h, int(enabled)), "set_graph")
 
     def set_mega(self, enabled):
-        """0/False: one kernel per phase; 1/True: k_mega (CUDA-core consumers); 2: k_mega_tc
-        (wgmma consumers); 3: k_mega_tc with a full 16-row activation operand; 4: k_mega in
-        dataflow mode (polled self-validating activation words instead of 3 of the 5 barriers)."""
+        """0/False: one kernel per phase; 1/True: k_mega, the persistent decode-step kernel
+        (default).  Any other value raises B200Error and leaves the mode unchanged."""
         N.check(self.lib.b200_engine_set_mega(self.h, int(enabled)), "set_mega")
 
     def debug_buffer(self, name: str, dtype=torch.float32) -> torch.Tensor:

@@ -9,8 +9,6 @@ from mlx_vlm_b200.utils import load_synthetic, prepare_inputs
 model, proc = load_synthetic("qwen2-vl-2b", seed=0, device="cuda:0", n_text_tokens=128)
 eng = model.engine
 eng.set_graph(False)
-if len(sys.argv) > 1:
-    eng.set_mega(int(sys.argv[1]))  # 1: k_mega, 2: k_mega_tc, 4: k_mega dataflow mode
 N.check(eng.lib.b200_engine_mega_timeline(eng.h, 0))
 img = np.random.default_rng(0).integers(0, 256, size=(336, 336, 3), dtype=np.uint8)
 inp = prepare_inputs(proc, images=[img], prompts="x", device=eng.device, stream=eng.stream)
@@ -26,13 +24,7 @@ raw = np.zeros(2 * 1024 * 2 + 256, dtype=np.int64)
 buf = raw[:4096].reshape(2, 1024, 2)
 N.check(eng.lib.b200_engine_mega_timeline(eng.h, raw.ctypes.data))
 L = 28
-mode = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-flow = mode == 4 or (mode == 1 and os.environ.get("B200_MEGA_FLOW", "0") == "1")
-if flow:
-    # dataflow mode: two grid barriers per layer (after attention, after gate/up)
-    names, per = ["down(l-1) + qkv + attention", "o_proj + gate/up"], 2
-else:
-    names, per = ["qkv", "attn", "ores", "gateup", "dres"], 5
+names, per = ["qkv", "attn", "ores", "gateup", "dres"], 5
 for cta in (0, 1):
     a = buf[cta]
     nb = per * L + 2
@@ -40,8 +32,7 @@ for cta in (0, 1):
     comp = np.empty(nb); comp[0] = np.nan
     comp[1:] = arrive[1:] - release[:-1]
     wait = release - arrive
-    print(f"--- CTA {'0' if cta == 0 else 'last'}: step span {(release[nb-1]-arrive[0])/1e3:.1f} us (first arrive -> last release)"
-          + (" [dataflow mode]" if flow else ""))
+    print(f"--- CTA {'0' if cta == 0 else 'last'}: step span {(release[nb-1]-arrive[0])/1e3:.1f} us (first arrive -> last release)")
     for k, nm in enumerate(names):
         idx = np.arange(L) * per + k
         c = comp[idx[1:] if k == 0 else idx]
@@ -70,9 +61,3 @@ for cta in (0, 1):
     t = raw[4096 + 128 + 32 * cta:4096 + 128 + 32 * cta + 12]; t = t[t > 0]
     if len(t) > 2:
         print(f"attention CTA{cta} (layer 5) step durations us:", list(zip(names[1:], [round(x / 1e3, 2) for x in np.diff(t)])))
-
-for name, off, labels in (("gateup prologue (k_mega_tc, CTA0 layer 5)", 4096 + 160, ["partials+residual", "cbar", "normalise+write", "fence.proxy.async", "cbar"]),
-                          ("down prologue (k_mega_tc, CTA0 layer 5)", 4096 + 176, ["load+write slice", "fence.proxy.async", "cbar"])):
-    t = raw[off:off + 8]; t = t[t > 0]
-    if len(t) > 2:
-        print(name, list(zip(labels, [round(x / 1e3, 2) for x in np.diff(t)])))

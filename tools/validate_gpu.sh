@@ -9,8 +9,6 @@ timeout -s KILL 900 python bench.py > gpurun_out/bench_r1.json 2> gpurun_out/ben
 echo "bench exit $?" >> gpurun_out/summary.txt
 timeout -s KILL 900 python bench.py --impl reference --steps 2 --warmup 1 > gpurun_out/bench_r1_reference.json 2>> gpurun_out/bench_r1.err
 echo "bench ref exit $?" >> gpurun_out/summary.txt
-timeout -s KILL 300 python bench.py --steps 3 --warmup 3 --no-cpu-baseline --mega-mode 2 > gpurun_out/bench_r1_tc.json 2>> gpurun_out/bench_r1.err
-echo "bench tc exit $?" >> gpurun_out/summary.txt
 timeout -s KILL 300 python tools/mega_timeline.py 1 > gpurun_out/mega_timeline_r1.txt 2>&1
 timeout -s KILL 900 ncu --metrics gpu__time_duration.sum --clock-control none -k "regex:attention|cast_f32|embed_merge|k_attn|k_mega|k_sample|k_set_state|k_stream|layer_norm|mrope_kv|rms_norm|swiglu_kernel|vision_rope|gemm|k_pack" -c 3000 --csv --log-file gpurun_out/launches_request_r1.csv python tools/profile_decode.py 3 > gpurun_out/prof.log 2>&1
 echo "ncu list exit $?" >> gpurun_out/summary.txt
@@ -21,11 +19,4 @@ grep -E "passed|failed" gpurun_out/t_gpu_all.log | tail -3
 tail -2 gpurun_out/smoke.log
 cut -c1-900 gpurun_out/bench_r1.json
 cut -c1-300 gpurun_out/bench_r1_reference.json
-python - <<'PY'
-import json
-for f in ('gpurun_out/bench_r1.json','gpurun_out/bench_r1_tc.json'):
-    try:
-        d=json.load(open(f)); print(f, 'decode tok/s', round(d['value'],1), 'ms/tok', round(d['decode_ms_per_token'],4), 'prefill ms', round(d['prefill_ms'],2), 'frac', round(d['roofline']['frac'],3), 'e2e', round(d['e2e']['value'],1))
-    except Exception as e: print(f, 'ERR', e)
-PY
 tail -5 gpurun_out/bench_r1.err
