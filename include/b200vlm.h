@@ -187,7 +187,9 @@ int b200_engine_set_weight(b200_engine* e, const char* name, const void* ptr, lo
 long b200_engine_workspace_bytes(const b200_engine* e, int max_tokens, int max_patches);
 int b200_engine_set_workspace(b200_engine* e, void* ptr, long bytes);
 /* KV pool laid out (n_layers, 2, batch, n_kv, cap, head_dim) bf16 — per layer the
- * reference KVCache layout (B, n_kv_heads, S, head_dim), cache.py:345-367. */
+ * reference KVCache layout (B, n_kv_heads, S, head_dim), cache.py:345-367.
+ * Every bind (this one, b200_engine_bind_kvq, b200_engine_bind_batch_kvq) replaces the previous binding, switches
+ * a prefill write-through off and, when the new pool has no row b200_engine_set_kv_row selected, selects row 0. */
 int b200_engine_bind_kv(b200_engine* e, void* pool, int batch, int cap);
 /* 8-bit KV pool (kv_bits=8; format in csrc/kvq.cuh): codes (n_layers, 2, batch, n_kv, cap, head_dim) uint8,
  * scales and biases (n_layers, 2, batch, n_kv, cap, head_dim / group_size) bf16, group_size 32 | 64 | 128.
@@ -199,8 +201,8 @@ int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases
 /* Prefill over an 8-bit cache: with the bf16 pool bound (its rows [0, ctx0) holding the dequantized prefix),
  * every prefill layer quantizes the chunk's new K/V rows into this 8-bit pool (same batch and capacity as the
  * bf16 one) and replaces them in the bf16 pool by their dequantized values before attending, so the chunk
- * attends to its prefix and to itself in quantized form.  codes == NULL switches the write-through off;
- * binding a pool switches it off too. */
+ * attends to its prefix and to itself in quantized form.  The target is the row selected now, in every layer.
+ * codes == NULL switches the write-through off; every bind and a change of the selected row switch it off too. */
 int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size);
 /* Lock-step batch pool of kv_bits=8, the reference's batch rule (generate/ar.py:751-859 `_make_cache`: a
  * BatchQuantizedKVCache for every layer where models/cache.py:8-21 `should_quantize_kv_layer` holds, a BatchKVCache
@@ -215,7 +217,8 @@ int b200_engine_bind_batch_kvq(b200_engine* e, void* codes, void* scales, void* 
 /* b200_engine_set_prefill_kvq into ROW `row` of an 8-bit batch pool of `rows` rows and capacity `cap` holding layers
  * 0 .. n_q8_layers-1 (the layout of b200_engine_bind_batch_kvq): the prefill of one admitted row writes its K/V rows
  * of those layers through to the batch pool (quantized before they are attended, BatchQuantizedKVCache.update_and_fetch
- * on a prefill chunk); the other layers stay bf16 in the bound pool.  Reset like b200_engine_set_prefill_kvq. */
+ * on a prefill chunk); the other layers stay bf16 in the bound pool.  Needs a bf16 pool bound; switched off like
+ * b200_engine_set_prefill_kvq. */
 int b200_engine_set_prefill_kvq_row(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int rows,
                                     int cap, int row, int n_q8_layers);
 /* One 8-bit decode attention step (the kernel of the per-phase decode step) on caller buffers, synchronous:
@@ -380,7 +383,8 @@ int b200_gemm_wt_f32(const void* X, long ldx, const void* W, long ldw, const voi
 /* ------------------------------------------------------------------------- */
 /* The bound KV pool is (layers, 2, rows, kv heads, capacity, head_dim); every row keeps its own
  * length (no left padding).  b200_engine_set_kv_row selects the row that b200_engine_prefill /
- * b200_engine_decode read and write (admission of a request = a batch-1 prefill into a free row). */
+ * b200_engine_decode read and write (admission of a request = a batch-1 prefill into a free row).  A bind resets it
+ * to 0 when the new pool has fewer rows; selecting another row switches a prefill write-through off. */
 int b200_engine_set_kv_row(b200_engine* e, int row);
 /* (Re)arm rows 0..B-1: next input token, cached length, rope position (length + M-RoPE delta) and
  * an active flag per row (host arrays).  B <= 16. */

@@ -4,6 +4,7 @@
 // workspace and the KV pool (torch-allocated device memory).
 #include <stdarg.h>
 
+#include <optional>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -30,6 +31,33 @@ struct VBlk {
   const bf16 *ln1w, *ln1b, *ln2w, *ln2b, *qkvw, *qkvb, *projw, *projb, *fc1w, *fc1b, *fc2w, *fc2b;
 };
 
+// Offset, in head rows (one position of one kv head), of the (layer, side, row) plane of a pool laid out
+// (layers, 2, rows, n_kv, cap, ...).  Times head_dim: the element offset of a bf16 pool or of 8-bit codes; times
+// head_dim / group_size: that of 8-bit scales and biases.
+static long plane_off(int layer, int side, int row, int rows, int n_kv, int cap) {
+  return (((long)layer * 2 + side) * rows + row) * n_kv * (long)cap;
+}
+
+// The KV cache the engine is bound to (caller-owned).  The kind decides which calls may use it: prefill needs bf16,
+// single-request decode bf16 or q8, the lock-step batch decoder bf16 or q8_batch.
+enum class KvKind { none, bf16, q8, q8_batch };
+struct KvBinding {
+  KvKind kind = KvKind::none;
+  bf16* kv = nullptr;  // bf16 pool; q8_batch: layers n_q8 .. n_layers-1 (nullptr when every layer is 8-bit)
+  KvqPlanes q8 = {};   // 8-bit pool of layers 0 .. n_q8-1
+  int n_q8 = 0, rows = 0, cap = 0;  // rows and capacity of both pools
+  bool operator==(const KvBinding& o) const {
+    return kind == o.kind && kv == o.kv && q8.codes == o.q8.codes && q8.scales == o.q8.scales &&
+           q8.biases == o.q8.biases && q8.gs == o.q8.gs && n_q8 == o.n_q8 && rows == o.rows && cap == o.cap;
+  }
+};
+// Prefill write-through: every prefill layer below n_layers quantizes its chunk's K/V rows into row `row` of an
+// 8-bit pool of `rows` rows and capacity `cap` (the b200_engine_bind_kvq layout) before they are attended
+struct KvWriteThrough {
+  KvqPlanes q8;
+  int rows, cap, row, n_layers;
+};
+
 }  // namespace b200
 
 using namespace b200;
@@ -53,21 +81,12 @@ struct b200_engine {
   // workspace (caller-owned)
   uint8_t* ws = nullptr;
   long ws_bytes = 0;
-  // kv pool (caller-owned)
-  bf16* kv = nullptr;
-  int kv_batch = 0, kv_cap = 0;
-  int kv_row = 0;        // row of the pool that prefill / single-row decode read and write
-  // 8-bit pool (b200_engine_bind_kvq; replaces `kv` while bound) and the engine-owned bf16 staging planes
-  // [2][n_kv][cap][hd] where the decode QKV kernel leaves the new K/V row before it is quantized
-  KvqPlanes q8 = {};
-  KvqPlanes pre_q8 = {};  // b200_engine_set_prefill_kvq: prefill writes its rows through to this 8-bit pool
-  // b200_engine_set_prefill_kvq_row: the write-through pool is a batch pool of its own geometry (pre_rows x pre_cap,
-  // target row pre_row) holding layers 0 .. pre_layers-1 only; pre_layers = 0: the bound pool's geometry, every layer
-  int pre_rows = 0, pre_cap = 0, pre_row = 0, pre_layers = 0;
-  // b200_engine_bind_batch_kvq: the lock-step batch pool of kv_bits=8.  Layers 0 .. bq8_layers-1 in this 8-bit pool,
-  // the others in the bf16 pool `kv` (nullptr when every layer is 8-bit)
-  KvqPlanes bq8 = {};
-  int bq8_layers = 0;
+  // KV binding (set by bind() only) and the row of it that prefill / single-row decode read and write
+  KvBinding kvb;
+  int kv_row = 0;
+  std::optional<KvWriteThrough> wt;  // cleared by every bind and by a change of kv_row
+  // q8 kind: engine-owned bf16 staging planes [2][n_kv][cap][hd] where the decode QKV kernel leaves the new K/V row
+  // before it is quantized
   bf16* q8_stage = nullptr;
   long q8_stage_elems = 0;
   void* batch = nullptr; // lock-step batched decoder (decode_batch.cu)
@@ -134,34 +153,20 @@ struct b200_engine {
   DecodeDims dims() const {
     DecodeDims d;
     d.hidden = cfg.hidden; d.inter = cfg.inter; d.n_heads = cfg.n_heads; d.n_kv = cfg.n_kv_heads;
-    d.hd = cfg.head_dim; d.vocab = cfg.vocab; d.cap = kv_cap; d.eps = cfg.rms_eps;
+    d.hd = cfg.head_dim; d.vocab = cfg.vocab; d.cap = kvb.cap; d.eps = cfg.rms_eps;
     d.scale_bf = __bfloat162float(__float2bfloat16_rn(1.0f / sqrtf((float)cfg.head_dim)));
     return d;
   }
-  bf16* kptr(int layer, int row) const {
-    return kv + (((long)layer * 2 + 0) * kv_batch + row) * cfg.n_kv_heads * (long)kv_cap * cfg.head_dim;
+  // element offset of the (layer, side, row) plane of a pool of the bound geometry (bf16 or 8-bit codes)
+  long kv_off(int layer, int side, int row) const {
+    return plane_off(layer, side, row, kvb.rows, cfg.n_kv_heads, kvb.cap) * cfg.head_dim;
   }
-  bf16* vptr(int layer, int row) const {
-    return kv + (((long)layer * 2 + 1) * kv_batch + row) * cfg.n_kv_heads * (long)kv_cap * cfg.head_dim;
-  }
-  bool pre_q8_layer(int layer) const { return pre_q8.codes && (pre_layers == 0 || layer < pre_layers); }
-  int pre_q8_cap() const { return pre_layers ? pre_cap : kv_cap; }
-  KvqPlanes pre_q8_plane(int layer, int side) const {
-    if (!pre_layers) return q8_plane(layer, side, kv_row, pre_q8);
-    const long plane = (((long)layer * 2 + side) * pre_rows + pre_row) * cfg.n_kv_heads;
-    KvqPlanes p = pre_q8;
-    p.codes += plane * pre_cap * cfg.head_dim;
-    p.scales += plane * pre_cap * (cfg.head_dim / pre_q8.gs);
-    p.biases += plane * pre_cap * (cfg.head_dim / pre_q8.gs);
-    return p;
-  }
-  KvqPlanes q8_plane(int layer, int side, int row, const KvqPlanes& pool) const {
-    const long plane = (((long)layer * 2 + side) * kv_batch + row) * cfg.n_kv_heads;
-    KvqPlanes p = pool;
-    p.codes += plane * kv_cap * cfg.head_dim;
-    p.scales += plane * kv_cap * (cfg.head_dim / pool.gs);
-    p.biases += plane * kv_cap * (cfg.head_dim / pool.gs);
-    return p;
+  bf16* kptr(int layer, int row) const { return kvb.kv + kv_off(layer, 0, row); }
+  bf16* vptr(int layer, int row) const { return kvb.kv + kv_off(layer, 1, row); }
+  KvqPlanes q8_plane(const KvqPlanes& pool, int layer, int side, int row, int rows, int cap) const {
+    const long off = plane_off(layer, side, row, rows, cfg.n_kv_heads, cap);
+    return KvqPlanes{pool.codes + off * cfg.head_dim, pool.scales + off * (cfg.head_dim / pool.gs),
+                     pool.biases + off * (cfg.head_dim / pool.gs), pool.gs};
   }
 };
 
@@ -253,7 +258,8 @@ static void invalidate_graph(b200_engine* e) {
 static int mega_prepare(b200_engine* e, cudaStream_t s) {
   const auto& c = e->cfg;
   B200_REQUIRE(c.n_layers <= MEGA_MAX_LAYERS, "mega: %d layers > %d", c.n_layers, MEGA_MAX_LAYERS);
-  B200_REQUIRE(!e->q8.codes, "mega: the persistent kernel reads a bf16 KV pool; an 8-bit pool runs the per-phase kernels");
+  B200_REQUIRE(e->kvb.kind == KvKind::bf16,
+               "mega: the persistent kernel reads a bf16 KV pool; an 8-bit pool runs the per-phase kernels");
   if (!e->bar) {
     B200_CUDA(cudaMalloc(&e->bar, sizeof(unsigned long long)));
     B200_CUDA(cudaMemset(e->bar, 0, sizeof(unsigned long long)));
@@ -273,8 +279,8 @@ static int mega_prepare(b200_engine* e, cudaStream_t s) {
   p.h = e->h; p.qbuf = e->qbuf; p.attn = e->attn; p.act = e->act;
   p.logits = e->logits; p.logprobs = e->logprobs;
   p.kv = e->kptr(0, e->kv_row);
-  p.kv_layer_stride = 2L * e->kv_batch * c.n_kv_heads * (long)e->kv_cap * c.head_dim;
-  p.kv_v_offset = (long)e->kv_batch * c.n_kv_heads * (long)e->kv_cap * c.head_dim;
+  p.kv_layer_stride = e->kv_off(1, 0, 0);
+  p.kv_v_offset = e->kv_off(0, 1, 0);
   p.partials = e->partials; p.st = e->st; p.token_log = e->token_log; p.log_cap = e->log_cap;
   p.force = e->force; p.inv_freq = e->lm_inv_freq; p.bar = e->bar; p.advance = 1;
   p.dbg = e->dbg;
@@ -295,16 +301,18 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
   const auto& c = e->cfg;
   int rc;
   if (e->active_mega()) return mega_launch(e->mp, e->sm_count, s);
-  if (e->q8.codes) {
+  if (e->kvb.kind == KvKind::q8) {
+    const KvBinding& b = e->kvb;
     bf16* sk = e->q8_stage;
-    bf16* sv = sk + (long)c.n_kv_heads * e->kv_cap * c.head_dim;
+    bf16* sv = sk + (long)c.n_kv_heads * b.cap * c.head_dim;
     for (int l = 0; l < c.n_layers; ++l) {
       const LayerW& lw = e->layers[l];
       if ((rc = launch_qkv(d, lw, e->h, e->qbuf, sk, sv, e->st, e->lm_inv_freq, s, e->qk_norm ? e->qn[l] : nullptr,
                            e->qk_norm ? e->kn[l] : nullptr)))
         return rc;
-      if ((rc = launch_attn_q8(d, e->qbuf, e->q8_plane(l, 0, e->kv_row, e->q8), e->q8_plane(l, 1, e->kv_row, e->q8), sk, sv,
-                               e->attn, e->st, e->attn_cluster, s)))
+      if ((rc = launch_attn_q8(d, e->qbuf, e->q8_plane(b.q8, l, 0, e->kv_row, b.rows, b.cap),
+                               e->q8_plane(b.q8, l, 1, e->kv_row, b.rows, b.cap), sk, sv, e->attn, e->st,
+                               e->attn_cluster, s)))
         return rc;
       if ((rc = launch_res(lw.wo, e->attn, e->h, c.hidden, c.n_heads * c.head_dim, s))) return rc;
       if ((rc = launch_gateup(d, lw, e->h, e->act, s))) return rc;
@@ -677,12 +685,12 @@ static int prefill_layers(b200_engine* e, const void* embeds, const int* pos3, i
     B200_CUDA(cudaEventSynchronize(e->kvref_ev));
   }
   e->kvref_host->k0 = e->kptr(0, e->kv_row);
-  e->kvref_host->v_off = (long)e->kv_batch * c.n_kv_heads * (long)e->kv_cap * c.head_dim;
-  e->kvref_host->layer_stride = 2L * e->kvref_host->v_off;
-  e->kvref_host->cap = e->kv_cap;
+  e->kvref_host->v_off = e->kv_off(0, 1, 0);
+  e->kvref_host->layer_stride = e->kv_off(1, 0, 0);
+  e->kvref_host->cap = e->kvb.cap;
   B200_CUDA(cudaMemcpyAsync(e->kvref, e->kvref_host, sizeof(KvRef), cudaMemcpyHostToDevice, s));
   B200_CUDA(cudaEventRecord(e->kvref_ev, s));
-  if (all_logits_out || ctx0 != 0 || e->pre_q8.codes)  // all-row logits / a later chunk / 8-bit write-through: plain launches
+  if (all_logits_out || ctx0 != 0 || e->wt)  // all-row logits / a later chunk / 8-bit write-through: plain launches
     return prefill_layers_body(e, pos_stage, T, ctx0, all_logits_out, s);
   const std::vector<long> key = {(long)(uintptr_t)e->ws, (long)e->ws_bytes, (long)T};
   return seq_run(e, e->pre_graphs, key, s, [&]() { return prefill_layers_body(e, pos_stage, T, 0, nullptr, s); });
@@ -712,7 +720,7 @@ static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0,
   e->launches += 1;
   const float scale = 1.0f / sqrtf((float)hd);
   const float scale_bf = __bfloat162float(__float2bfloat16_rn(scale));
-  const int S = ctx0 + T;
+  const int S = ctx0 + T, cap = e->kvb.cap;
   for (int l = 0; l < c.n_layers; ++l) {
     const LayerW& lw = e->layers[l];
     bf16* kc = e->kptr(l, e->kv_row);
@@ -725,13 +733,13 @@ static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0,
     // the pipelined kernel needs V^T of EVERY key: available for a fresh prompt (ctx0 == 0).  It then
     // reads the chunk's own rotated K copy and V^T from the workspace, and the cache is addressed through
     // e->kvref: nothing about the KV pool is baked into the captured graph.
-    const bool fa = ctx0 == 0 && !e->pre_q8.codes && attention_fa_supported(qkv, QKV, hd, kws, hd, (long)T * hd, vt, (long)hd * t_ld,
+    const bool fa = ctx0 == 0 && !e->wt && attention_fa_supported(qkv, QKV, hd, kws, hd, (long)T * hd, vt, (long)hd * t_ld,
                                                         t_ld, att, QH, hd);
     if (segs) {
       B200_REQUIRE(fa, "prefill_batch: the pipelined attention kernel does not support this geometry");
-      const long row_stride = (long)c.n_kv_heads * e->kv_cap * hd;
-      if ((rc = mrope_kv_write(qkv, pos3, e->lm_inv_freq, e->axis_sel, e->kptr(l, 0), e->vptr(l, 0), T, 0, e->kv_cap,
-                               c.n_heads, c.n_kv_heads, hd, s, scale_bf, vt, t_ld, nullptr, l, kws, tok_loc, row_stride)))
+      if ((rc = mrope_kv_write(qkv, pos3, e->lm_inv_freq, e->axis_sel, e->kptr(l, 0), e->vptr(l, 0), T, 0, cap,
+                               c.n_heads, c.n_kv_heads, hd, s, scale_bf, vt, t_ld, nullptr, l, kws, tok_loc,
+                               e->kv_off(0, 0, 1))))
         return rc;
       // all sequences in ONE launch: the (q0, Lq, k0, S) table follows the (row, position) table in `tok_loc`
       int longest = 0;
@@ -741,15 +749,16 @@ static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0,
         return rc;
       e->launches += 2;
     } else {
-    if ((rc = mrope_kv_write(qkv, pos3, e->lm_inv_freq, e->axis_sel, kc, vc, T, ctx0, e->kv_cap, c.n_heads,
+    if ((rc = mrope_kv_write(qkv, pos3, e->lm_inv_freq, e->axis_sel, kc, vc, T, ctx0, cap, c.n_heads,
                              c.n_kv_heads, hd, s, fa ? scale_bf : 0.f, fa ? vt : nullptr, t_ld,
                              fa ? e->kvref : nullptr, l, fa ? kws : nullptr)))
       return rc;
-    if (e->pre_q8_layer(l)) {  // an 8-bit layer: the chunk's rows are quantized before they are attended
-      if ((rc = kvq_quantize_rows(kc, e->kv_cap, e->pre_q8_plane(l, 0), e->pre_q8_cap(), c.n_kv_heads, ctx0, T, hd,
-                                  true, s)) ||
-          (rc = kvq_quantize_rows(vc, e->kv_cap, e->pre_q8_plane(l, 1), e->pre_q8_cap(), c.n_kv_heads, ctx0, T, hd,
-                                  true, s)))
+    if (e->wt && l < e->wt->n_layers) {  // an 8-bit layer: the chunk's rows are quantized before they are attended
+      const KvWriteThrough& w8 = *e->wt;
+      if ((rc = kvq_quantize_rows(kc, cap, e->q8_plane(w8.q8, l, 0, w8.row, w8.rows, w8.cap), w8.cap, c.n_kv_heads,
+                                  ctx0, T, hd, true, s)) ||
+          (rc = kvq_quantize_rows(vc, cap, e->q8_plane(w8.q8, l, 1, w8.row, w8.rows, w8.cap), w8.cap, c.n_kv_heads,
+                                  ctx0, T, hd, true, s)))
         return rc;
       e->launches += 2;
     }
@@ -757,7 +766,7 @@ static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0,
       rc = attention_fa(qkv, QKV, hd, kws, hd, (long)T * hd, vt, (long)hd * t_ld, t_ld, att, QH, c.n_heads,
                         c.n_kv_heads, hd, T, S, 1, s, 0, T, 0, S);
     } else {
-      rc = attention(qkv, QKV, hd, kc, hd, (long)e->kv_cap * hd, vc, hd, (long)e->kv_cap * hd, att, QH, c.n_heads,
+      rc = attention(qkv, QKV, hd, kc, hd, (long)cap * hd, vc, hd, (long)cap * hd, att, QH, c.n_heads,
                      c.n_kv_heads, hd, T, S, 1, scale, s);
     }
     if (rc) return rc;
@@ -785,6 +794,42 @@ static int prefill_layers_body(b200_engine* e, const int* pos3, int T, int ctx0,
                      B200_EPI_NONE, s)))
       return rc;
   }
+  return B200_OK;
+}
+
+static bool kvq_group_ok(const b200_engine* e, int gs) {
+  return (gs == 32 || gs == 64 || gs == 128) && e->cfg.head_dim % gs == 0;
+}
+
+// The one place the KV binding changes (the entry points have checked their arguments).  The decode graph is dropped
+// when the binding differs from the bound one, a write-through is cleared, the 8-bit decode staging planes exist for
+// the q8 kind only, and a selected row the new pool does not have goes back to row 0.
+static int bind(b200_engine* e, const KvBinding& b) {
+  if (!(b == e->kvb)) invalidate_graph(e);  // a row reset below also changes the rows
+  e->wt.reset();
+  if (e->kv_row >= b.rows) e->kv_row = 0;
+  const long stage = b.kind == KvKind::q8 ? 2L * e->cfg.n_kv_heads * b.cap * e->cfg.head_dim : 0;
+  if (stage > e->q8_stage_elems || (stage == 0 && e->q8_stage)) {
+    e->kvb = KvBinding{};  // nothing is bound until the staging planes are in place
+    if (e->q8_stage) B200_CUDA(cudaFree(e->q8_stage));
+    e->q8_stage = nullptr;
+    e->q8_stage_elems = 0;
+    if (stage) B200_CUDA(cudaMalloc(&e->q8_stage, (size_t)stage * sizeof(bf16)));
+    e->q8_stage_elems = stage;
+  }
+  e->kvb = b;
+  return B200_OK;
+}
+
+static int set_write_through(b200_engine* e, const char* fn, void* codes, void* scales, void* biases, int group_size,
+                             int rows, int cap, int row, int n_layers) {
+  B200_REQUIRE(e->kvb.kind == KvKind::bf16, "%s: bind the bf16 pool first", fn);
+  B200_REQUIRE(codes && scales && biases && rows >= 1 && cap >= 1 && row >= 0 && row < rows, "%s: bad arguments", fn);
+  B200_REQUIRE(n_layers >= 1 && n_layers <= e->cfg.n_layers, "%s: %d 8-bit layers of %d", fn, n_layers,
+               e->cfg.n_layers);
+  B200_REQUIRE(kvq_group_ok(e, group_size), "%s: group size %d must be 32, 64 or 128 and divide head_dim %d", fn,
+               group_size, e->cfg.head_dim);
+  e->wt = KvWriteThrough{KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size}, rows, cap, row, n_layers};
   return B200_OK;
 }
 
@@ -952,21 +997,17 @@ int b200_engine_set_workspace(b200_engine* e, void* ptr, long bytes) {
 int b200_engine_bind_kv(b200_engine* e, void* pool, int batch, int cap) {
   B200_REQUIRE(e && pool && batch >= 1 && cap >= 1 && ((uintptr_t)pool & 15) == 0,
                "bind_kv: bad arguments");
-  if (pool != e->kv || batch != e->kv_batch || cap != e->kv_cap || e->q8.codes) invalidate_graph(e);
-  if (e->q8_stage) {  // the 8-bit decode staging planes are not needed while a bf16 pool is bound
-    B200_CUDA(cudaFree(e->q8_stage));
-    e->q8_stage = nullptr;
-    e->q8_stage_elems = 0;
-  }
-  e->kv = (bf16*)pool;
-  e->kv_batch = batch;
-  e->kv_cap = cap;
-  e->q8 = KvqPlanes{};
-  e->pre_q8 = KvqPlanes{};
-  e->pre_layers = 0;
-  e->bq8 = KvqPlanes{};
-  e->bq8_layers = 0;
-  return B200_OK;
+  return bind(e, KvBinding{KvKind::bf16, (bf16*)pool, {}, 0, batch, cap});
+}
+
+int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases, int batch, int cap,
+                         int group_size) {
+  B200_REQUIRE(e && codes && scales && biases && batch >= 1 && cap >= 1 && ((uintptr_t)codes & 15) == 0,
+               "bind_kvq: bad arguments");
+  B200_REQUIRE(kvq_group_ok(e, group_size), "bind_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d",
+               group_size, e->cfg.head_dim);
+  const KvqPlanes q8{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
+  return bind(e, KvBinding{KvKind::q8, nullptr, q8, e->cfg.n_layers, batch, cap});
 }
 
 int b200_engine_bind_batch_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int n_q8_layers,
@@ -975,83 +1016,29 @@ int b200_engine_bind_batch_kvq(b200_engine* e, void* codes, void* scales, void* 
                    ((uintptr_t)bf16_pool & 15) == 0,
                "bind_batch_kvq: bad arguments");
   const auto& c = e->cfg;
-  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && c.head_dim % group_size == 0,
+  B200_REQUIRE(kvq_group_ok(e, group_size),
                "bind_batch_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size, c.head_dim);
   B200_REQUIRE(n_q8_layers >= 1 && n_q8_layers <= c.n_layers && (bf16_pool != nullptr) == (n_q8_layers < c.n_layers),
                "bind_batch_kvq: %d of %d layers 8-bit needs a bf16 pool for the rest (and only then)", n_q8_layers,
                c.n_layers);
-  B200_REQUIRE(e->kv_row < batch, "bind_batch_kvq: bound row %d of %d", e->kv_row, batch);
-  if (bf16_pool != e->kv || batch != e->kv_batch || cap != e->kv_cap || e->q8.codes) invalidate_graph(e);
-  e->kv = (bf16*)bf16_pool;
-  e->kv_batch = batch;
-  e->kv_cap = cap;
-  e->q8 = KvqPlanes{};
-  e->pre_q8 = KvqPlanes{};
-  e->pre_layers = 0;
-  e->bq8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
-  e->bq8_layers = n_q8_layers;
-  return B200_OK;
+  const KvqPlanes q8{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
+  return bind(e, KvBinding{KvKind::q8_batch, (bf16*)bf16_pool, q8, n_q8_layers, batch, cap});
 }
 
 int b200_engine_set_prefill_kvq_row(b200_engine* e, void* codes, void* scales, void* biases, int group_size, int rows,
                                     int cap, int row, int n_q8_layers) {
-  B200_REQUIRE(e && codes && scales && biases && rows >= 1 && cap >= 1 && row >= 0 && row < rows,
-               "set_prefill_kvq_row: bad arguments");
-  B200_REQUIRE(n_q8_layers >= 1 && n_q8_layers <= e->cfg.n_layers, "set_prefill_kvq_row: %d 8-bit layers of %d",
-               n_q8_layers, e->cfg.n_layers);
-  B200_REQUIRE(e->kv, "set_prefill_kvq_row: bind the bf16 pool first");
-  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && e->cfg.head_dim % group_size == 0,
-               "set_prefill_kvq_row: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size,
-               e->cfg.head_dim);
-  // every argument is checked: only now does the engine state change
-  e->pre_q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
-  e->pre_rows = rows;
-  e->pre_cap = cap;
-  e->pre_row = row;
-  e->pre_layers = n_q8_layers;
-  return B200_OK;
+  B200_REQUIRE(e, "set_prefill_kvq_row: null engine");
+  return set_write_through(e, "set_prefill_kvq_row", codes, scales, biases, group_size, rows, cap, row, n_q8_layers);
 }
 
 int b200_engine_set_prefill_kvq(b200_engine* e, void* codes, void* scales, void* biases, int group_size) {
   B200_REQUIRE(e, "set_prefill_kvq: null engine");
-  e->pre_layers = 0;
   if (!codes) {
-    e->pre_q8 = KvqPlanes{};
+    e->wt.reset();
     return B200_OK;
   }
-  B200_REQUIRE(e->kv && scales && biases, "set_prefill_kvq: bind the bf16 pool first");
-  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && e->cfg.head_dim % group_size == 0,
-               "set_prefill_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size,
-               e->cfg.head_dim);
-  e->pre_q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
-  return B200_OK;
-}
-
-int b200_engine_bind_kvq(b200_engine* e, void* codes, void* scales, void* biases, int batch, int cap,
-                         int group_size) {
-  B200_REQUIRE(e && codes && scales && biases && batch >= 1 && cap >= 1 && ((uintptr_t)codes & 15) == 0,
-               "bind_kvq: bad arguments");
-  const auto& c = e->cfg;
-  B200_REQUIRE((group_size == 32 || group_size == 64 || group_size == 128) && c.head_dim % group_size == 0,
-               "bind_kvq: group size %d must be 32, 64 or 128 and divide head_dim %d", group_size, c.head_dim);
-  B200_REQUIRE(e->kv_row < batch, "bind_kvq: bound row %d of %d", e->kv_row, batch);
-  const long stage = 2L * c.n_kv_heads * cap * c.head_dim;
-  if (stage > e->q8_stage_elems) {
-    if (e->q8_stage) B200_CUDA(cudaFree(e->q8_stage));
-    e->q8_stage = nullptr;
-    e->q8_stage_elems = 0;
-    B200_CUDA(cudaMalloc(&e->q8_stage, (size_t)stage * sizeof(bf16)));
-    e->q8_stage_elems = stage;
-  }
-  if (codes != e->q8.codes || batch != e->kv_batch || cap != e->kv_cap || group_size != e->q8.gs)
-    invalidate_graph(e);
-  e->kv = nullptr;
-  e->kv_batch = batch;
-  e->kv_cap = cap;
-  e->bq8 = KvqPlanes{};
-  e->bq8_layers = 0;
-  e->q8 = KvqPlanes{(uint8_t*)codes, (bf16*)scales, (bf16*)biases, group_size};
-  return B200_OK;
+  return set_write_through(e, "set_prefill_kvq", codes, scales, biases, group_size, e->kvb.rows, e->kvb.cap, e->kv_row,
+                           e->cfg.n_layers);
 }
 
 int b200_engine_vision(b200_engine* e, const float* pixel_values, const int* grid_thw_host,
@@ -1081,11 +1068,12 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   B200_REQUIRE(e && embeds && pos3 && T > 0 && ctx0 >= 0, "engine_prefill: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv && !e->bq8.codes, "engine_prefill: KV pool not bound (a lock-step 8-bit batch pool is decode-only)");
-  B200_REQUIRE(ctx0 + T <= e->kv_cap, "engine_prefill: ctx0+T=%d exceeds cache capacity %d",
-               ctx0 + T, e->kv_cap);
-  B200_REQUIRE(!e->pre_q8.codes || !e->pre_layers || ctx0 + T <= e->pre_cap,
-               "engine_prefill: ctx0+T=%d exceeds the capacity %d of the 8-bit write-through pool", ctx0 + T, e->pre_cap);
+  B200_REQUIRE(e->kvb.kind == KvKind::bf16, "engine_prefill: no bf16 KV pool bound (an 8-bit pool is decode-only)");
+  B200_REQUIRE(ctx0 + T <= e->kvb.cap, "engine_prefill: ctx0+T=%d exceeds cache capacity %d",
+               ctx0 + T, e->kvb.cap);
+  B200_REQUIRE(!e->wt || ctx0 + T <= e->wt->cap,
+               "engine_prefill: ctx0+T=%d exceeds the capacity %d of the 8-bit write-through pool", ctx0 + T,
+               e->wt->cap);
   B200_REQUIRE(e->ws && b200_engine_workspace_bytes(e, T, 1) <= e->ws_bytes,
                "engine_prefill: workspace too small for %d tokens", T);
   B200_CUDA(cudaSetDevice(e->device));
@@ -1095,9 +1083,9 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   const bf16* h = (const bf16*)(e->ws + lm_ws(c, T).h);
   // last row through the fused head + sampler; arms the decode state
   const DecodeDims d = e->dims();
-  if (e->prepared_cap != e->kv_cap || e->prepared_cluster != e->attn_cluster) {
+  if (e->prepared_cap != e->kvb.cap || e->prepared_cluster != e->attn_cluster) {
     if ((rc = decode_prepare(d, e->attn_cluster))) return rc;
-    e->prepared_cap = e->kv_cap;
+    e->prepared_cap = e->kvb.cap;
     e->prepared_cluster = e->attn_cluster;
   }
   e->ctx_host = ctx0 + T;
@@ -1124,14 +1112,14 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_REQUIRE(e && embeds && pos3 && n_seq > 0 && seq_len && rows, "engine_prefill_batch: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv && !e->bq8.codes, "engine_prefill_batch: KV pool not bound / 8-bit batch pool bound");
-  B200_REQUIRE(!e->pre_q8.codes, "engine_prefill_batch: no 8-bit write-through in the batched prefill");
+  B200_REQUIRE(e->kvb.kind == KvKind::bf16, "engine_prefill_batch: no bf16 KV pool bound (an 8-bit pool is decode-only)");
+  B200_REQUIRE(!e->wt, "engine_prefill_batch: no 8-bit write-through in the batched prefill");
   long T = 0;
   std::vector<PreSeg> segs(n_seq);
   for (int g = 0; g < n_seq; ++g) {
-    B200_REQUIRE(seq_len[g] > 0 && seq_len[g] <= e->kv_cap && rows[g] >= 0 && rows[g] < e->kv_batch,
+    B200_REQUIRE(seq_len[g] > 0 && seq_len[g] <= e->kvb.cap && rows[g] >= 0 && rows[g] < e->kvb.rows,
                  "engine_prefill_batch: sequence %d: %d tokens into row %d (capacity %d, %d rows)", g, seq_len[g], rows[g],
-                 e->kv_cap, e->kv_batch);
+                 e->kvb.cap, e->kvb.rows);
     segs[g] = PreSeg{(int)T, seq_len[g], rows[g]};
     T += round8(seq_len[g]);   // every sequence starts at a multiple of 8 tokens: the V^T tiles are loaded by TMA
                                // with tokens innermost, and a box must start on a 16-byte boundary
@@ -1160,9 +1148,9 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_CUDA(cudaEventRecord(e->loc_ev, s));   // the table (and its staging copy) may be rewritten after this point
   if (rc) return rc;
   const DecodeDims d = e->dims();
-  if (e->prepared_cap != e->kv_cap || e->prepared_cluster != e->attn_cluster) {
+  if (e->prepared_cap != e->kvb.cap || e->prepared_cluster != e->attn_cluster) {
     if ((rc = decode_prepare(d, e->attn_cluster))) return rc;
-    e->prepared_cap = e->kv_cap;
+    e->prepared_cap = e->kvb.cap;
     e->prepared_cluster = e->attn_cluster;
   }
   for (int g = 0; g < n_seq; ++g) {   // first token of every sequence: fused head + sampler on its last row
@@ -1195,11 +1183,11 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   B200_REQUIRE(e && n_steps > 0, "engine_decode: bad arguments");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE((e->kv || e->q8.codes) && !e->bq8.codes, "engine_decode: KV pool not bound (a lock-step 8-bit batch pool "
-               "serves b200_batch_decode only)");
-  B200_REQUIRE(e->ctx_host + n_steps <= e->kv_cap,
+  B200_REQUIRE(e->kvb.kind == KvKind::bf16 || e->kvb.kind == KvKind::q8, "engine_decode: KV pool not bound (a "
+               "lock-step 8-bit batch pool serves b200_batch_decode only)");
+  B200_REQUIRE(e->ctx_host + n_steps <= e->kvb.cap,
                "engine_decode: %d cached + %d steps exceeds cache capacity %d", e->ctx_host,
-               n_steps, e->kv_cap);
+               n_steps, e->kvb.cap);
   B200_REQUIRE(n_steps < e->log_cap, "engine_decode: too many steps per call");
   B200_CUDA(cudaSetDevice(e->device));
   cudaStream_t s = (cudaStream_t)stream;
@@ -1213,9 +1201,9 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   if ((rc = launch_set_state(e->st, 0, e->ctx_host, e->pos_host, force_tokens_host ? 1 : 0, 0,
                              e->embed, e->h, e->cfg.hidden, s)))
     return rc;
-  if (e->prepared_cap != e->kv_cap || e->prepared_cluster != e->attn_cluster) {
+  if (e->prepared_cap != e->kvb.cap || e->prepared_cluster != e->attn_cluster) {
     if ((rc = decode_prepare(e->dims(), e->attn_cluster))) return rc;
-    e->prepared_cap = e->kv_cap;
+    e->prepared_cap = e->kvb.cap;
     e->prepared_cluster = e->attn_cluster;
   }
   if (e->use_mega && e->mega_fits && !e->mega_ready) {
@@ -1227,7 +1215,7 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
       e->mega_fits = false;
     }
   }
-  if (e->q8.codes && !(e->use_graph && e->gexec))
+  if (e->kvb.kind == KvKind::q8 && !(e->use_graph && e->gexec))
     if ((rc = kvq_decode_prepare(e->dims(), e->attn_cluster))) return rc;
   if (e->use_graph && !e->gexec) {
     // capture one step on the engine's own stream (capture does not execute)
@@ -1337,9 +1325,12 @@ int b200_engine_fetch_tokens(b200_engine* e, long start, int n, int* host_out, v
   return B200_OK;
 }
 int b200_engine_set_kv_row(b200_engine* e, int row) {
-  B200_REQUIRE(e && row >= 0 && (e->kv_batch == 0 || row < e->kv_batch), "set_kv_row: row %d of %d", row,
-               e ? e->kv_batch : 0);
-  if (row != e->kv_row) invalidate_graph(e);
+  B200_REQUIRE(e && row >= 0 && (e->kvb.kind == KvKind::none || row < e->kvb.rows), "set_kv_row: row %d of %d", row,
+               e ? e->kvb.rows : 0);
+  if (row != e->kv_row) {  // the decode graph and a write-through were set up for the old row
+    invalidate_graph(e);
+    e->wt.reset();
+  }
   e->kv_row = row;
   return B200_OK;
 }
@@ -1351,16 +1342,21 @@ static void bd_model(b200_engine* e, BdModel* m) {
   m->layers = e->layers.data();
   m->embed = e->embed; m->head = e->head; m->final_norm = e->norm;
   m->inv_freq = e->lm_inv_freq;
-  m->kv = e->kv;
-  m->row_stride = (long)c.n_kv_heads * e->kv_cap * c.head_dim;
-  m->v_off = (long)e->kv_batch * m->row_stride;
-  m->layer_stride = 2L * m->v_off;
-  m->kv_batch = e->kv_batch;
+  const KvBinding& b = e->kvb;
+  m->kv = b.kv;
+  m->row_stride = e->kv_off(0, 0, 1);
+  m->v_off = e->kv_off(0, 1, 0);
+  m->layer_stride = e->kv_off(1, 0, 0);
+  m->kv_batch = b.rows;
   m->sm_count = e->sm_count;
   m->qn = e->qk_norm ? e->qn.data() : nullptr;
   m->kn = e->qk_norm ? e->kn.data() : nullptr;
-  m->q8_codes = e->bq8.codes; m->q8_scales = e->bq8.scales; m->q8_biases = e->bq8.biases;
-  m->q8_gs = e->bq8.gs; m->q8_layers = e->bq8_layers;
+  m->q8_codes = b.q8.codes; m->q8_scales = b.q8.scales; m->q8_biases = b.q8.biases;
+  m->q8_gs = b.q8.gs; m->q8_layers = b.n_q8;
+}
+
+static bool batch_kind(const b200_engine* e) {
+  return e->kvb.kind == KvKind::bf16 || e->kvb.kind == KvKind::q8_batch;
 }
 
 int b200_batch_begin(b200_engine* e, int B, const int* tok, const int* ctx, const int* pos, const int* active,
@@ -1368,7 +1364,7 @@ int b200_batch_begin(b200_engine* e, int B, const int* tok, const int* ctx, cons
   B200_REQUIRE(e && tok && ctx && pos && active, "batch_begin: null argument");
   int rc = resolve(e);
   if (rc) return rc;
-  B200_REQUIRE(e->kv || e->bq8.codes, "batch_begin: KV pool not bound");
+  B200_REQUIRE(batch_kind(e), "batch_begin: KV pool not bound (bf16 or a lock-step 8-bit batch pool)");
   B200_CUDA(cudaSetDevice(e->device));
   BdModel m;
   bd_model(e, &m);
@@ -1381,10 +1377,11 @@ int b200_batch_begin(b200_engine* e, int B, const int* tok, const int* ctx, cons
 
 int b200_batch_decode(b200_engine* e, int n_steps, int want_logprobs, void* stream) {
   B200_REQUIRE(e && e->batch && n_steps > 0, "batch_decode: batch_begin first");
+  B200_REQUIRE(batch_kind(e), "batch_decode: KV pool not bound (bf16 or a lock-step 8-bit batch pool)");
   for (size_t b = 0; b < e->b_ctx.size(); ++b)
-    B200_REQUIRE(!e->b_active[b] || e->b_ctx[b] + n_steps <= e->kv_cap,
+    B200_REQUIRE(!e->b_active[b] || e->b_ctx[b] + n_steps <= e->kvb.cap,
                  "batch_decode: row %zu: %d cached + %d steps exceeds cache capacity %d", b, e->b_ctx[b], n_steps,
-                 e->kv_cap);
+                 e->kvb.cap);
   B200_CUDA(cudaSetDevice(e->device));
   BdModel m;
   bd_model(e, &m);
@@ -1422,8 +1419,8 @@ int b200_kv_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, co
   const size_t w = (size_t)n_tokens * hd * 2;
   for (int l = 0; l < n_layers; ++l)
     for (int kv = 0; kv < 2; ++kv) {
-      const char* sp = (const char*)src_pool + ((((size_t)l * 2 + kv) * src_batch + src_row) * n_kv) * (size_t)src_cap * hd * 2;
-      char* dp = (char*)dst_pool + ((((size_t)l * 2 + kv) * dst_batch + dst_row) * n_kv) * (size_t)dst_cap * hd * 2;
+      const char* sp = (const char*)src_pool + plane_off(l, kv, src_row, src_batch, n_kv, src_cap) * hd * 2;
+      char* dp = (char*)dst_pool + plane_off(l, kv, dst_row, dst_batch, n_kv, dst_cap) * hd * 2;
       B200_CUDA(cudaMemcpy2DAsync(dp, (size_t)dst_cap * hd * 2, sp, (size_t)src_cap * hd * 2, w, n_kv,
                                   cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     }

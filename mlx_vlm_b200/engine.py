@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _native as N
-from .models.cache import BatchKVQPool, KVPool
+from .models.cache import BatchKVQPool, KVPool, QuantizedKVPool
 
 
 def _inv_freq(dim: int, base: float) -> np.ndarray:
@@ -96,60 +96,45 @@ class Engine:
             raise N.B200Error(f"KV pool (layers, kv heads, head_dim) = {(pool.n_layers, pool.n_kv, pool.hd)} does not "
                               f"match the engine's {(c.n_layers, c.n_kv_heads, c.head_dim)}")
 
-    def bind_pool(self, pool: KVPool):
-        # keyed on the device buffer itself (not id(pool): CPython reuses ids of collected pools);
-        # the engine keeps a strong reference to the bound buffer so its address cannot be recycled
+    def bind_pool(self, pool):
+        """bind a KVPool (bf16), a QuantizedKVPool (8-bit, single-request decode: the per-phase kernels with the
+        8-bit attention) or a BatchKVQPool (the lock-step batch pool of kv_bits=8); see b200_engine_bind_kv"""
+        # keyed on the device buffers themselves (not id(pool): CPython reuses ids of collected pools);
+        # the engine keeps a strong reference to the bound buffers so their addresses cannot be recycled
+        self._check_pool_shape(pool)
         if isinstance(pool, BatchKVQPool):
-            return self.bind_batch_kvq(pool)
-        self._check_pool_shape(pool)
-        key = (pool.buf.data_ptr(), pool.batch, pool.capacity)
+            q, bf = pool.q, (None if pool.bf is None else pool.bf.buf)
+            bufs = (q.codes, q.scales, q.biases, bf)
+            args = (q.codes.data_ptr(), q.scales.data_ptr(), q.biases.data_ptr(), pool.group_size, pool.n_q,
+                    N.ptr(bf), pool.batch, pool.capacity)
+            fn = "bind_batch_kvq"
+        elif isinstance(pool, QuantizedKVPool):
+            bufs = (pool.codes, pool.scales, pool.biases)
+            args = (pool.codes.data_ptr(), pool.scales.data_ptr(), pool.biases.data_ptr(), pool.batch, pool.capacity,
+                    pool.group_size)
+            fn = "bind_kvq"
+        else:
+            bufs = (pool.buf,)
+            args = (pool.buf.data_ptr(), pool.batch, pool.capacity)
+            fn = "bind_kv"
+        key = (type(pool),) + args
         if key != self._bound:
-            N.check(self.lib.b200_engine_bind_kv(self.h, pool.buf.data_ptr(), pool.batch,
-                                                 pool.capacity), "bind_kv")
+            N.check(getattr(self.lib, "b200_engine_" + fn)(self.h, *args), fn)
             self._bound = key
-            self._bound_buf = pool.buf
+            self._bound_buf = bufs
 
-    def bind_kvq(self, pool):
-        """bind an 8-bit pool (models/cache.py QuantizedKVPool) in place of the bf16 one: decode steps then run
-        the per-phase kernels with the 8-bit attention (csrc/kvq.cu)"""
-        self._check_pool_shape(pool)
-        key = ("q8", pool.codes.data_ptr(), pool.batch, pool.capacity, pool.group_size)
-        if key != self._bound:
-            N.check(self.lib.b200_engine_bind_kvq(self.h, pool.codes.data_ptr(), pool.scales.data_ptr(),
-                                                  pool.biases.data_ptr(), pool.batch, pool.capacity,
-                                                  pool.group_size), "bind_kvq")
-            self._bound = key
-            self._bound_buf = (pool.codes, pool.scales, pool.biases)
-
-    def bind_batch_kvq(self, pool: BatchKVQPool):
-        """bind the lock-step batch pool of kv_bits=8 (8-bit layers + a bf16 last layer, models/cache.py
-        BatchKVQPool); see b200_engine_bind_batch_kvq"""
-        self._check_pool_shape(pool)
-        q, bf = pool.q, pool.bf
-        key = ("bq8", q.codes.data_ptr(), N.ptr(None if bf is None else bf.buf), pool.batch, pool.capacity,
-               pool.group_size)
-        if key != self._bound:
-            N.check(self.lib.b200_engine_bind_batch_kvq(self.h, q.codes.data_ptr(), q.scales.data_ptr(),
-                                                        q.biases.data_ptr(), pool.group_size, pool.n_q,
-                                                        N.ptr(None if bf is None else bf.buf), pool.batch,
-                                                        pool.capacity), "bind_batch_kvq")
-            self._bound = key
-            self._bound_buf = (q.codes, q.scales, q.biases, None if bf is None else bf.buf)
-
-    def set_prefill_kvq_row(self, pool: BatchKVQPool, row: int):
-        """the next prefill calls write the 8-bit layers' K/V rows through to row `row` of the batch pool"""
-        q = pool.q
-        N.check(self.lib.b200_engine_set_prefill_kvq_row(self.h, q.codes.data_ptr(), q.scales.data_ptr(),
-                                                         q.biases.data_ptr(), pool.group_size, pool.batch,
-                                                         pool.capacity, int(row), pool.n_q), "set_prefill_kvq_row")
-
-    def set_prefill_kvq(self, pool):
-        """prefill calls write their K/V rows through to this 8-bit pool (None: off); see b200_engine_set_prefill_kvq"""
+    def set_prefill_kvq(self, pool, row: int = 0):
+        """the next prefill calls quantize their K/V rows of the layers this 8-bit pool holds (a QuantizedKVPool:
+        every layer; a BatchKVQPool: its 8-bit layers) into row `row` of it before they are attended; None: off.
+        Any bind and a change of the selected row switch it off too (b200_engine_set_prefill_kvq_row)"""
         if pool is None:
             N.check(self.lib.b200_engine_set_prefill_kvq(self.h, None, None, None, 0), "set_prefill_kvq")
             return
-        N.check(self.lib.b200_engine_set_prefill_kvq(self.h, pool.codes.data_ptr(), pool.scales.data_ptr(),
-                                                     pool.biases.data_ptr(), pool.group_size), "set_prefill_kvq")
+        q = pool.q if isinstance(pool, BatchKVQPool) else pool
+        N.check(self.lib.b200_engine_set_prefill_kvq_row(self.h, q.codes.data_ptr(), q.scales.data_ptr(),
+                                                         q.biases.data_ptr(), q.group_size, q.batch, q.capacity,
+                                                         int(row), q.n_layers), "set_prefill_kvq_row")
+        self._bound = None   # the next bind_pool reaches the engine, which switches the write-through off
 
     # -- calls ---------------------------------------------------------------
     def vision(self, pixel_values: torch.Tensor, grid_thw: np.ndarray) -> torch.Tensor:

@@ -156,8 +156,16 @@ class LanguageModel:
                 # a batched pool moves as a whole: keep every row's live prefix
                 live = c0.offset if pool.batch == 1 else pool.capacity
                 pool.reserve(need_tokens, live_tokens=live)
+        return self._bind_row(pool, c0._row or 0)
+
+    def _bind_row(self, pool, row: int, q8=None, q8_row: int = 0):
+        """bind `pool` and select its row `row`; with an 8-bit pool `q8` the next prefill writes its rows of the 8-bit
+        layers through to row `q8_row` of it, quantized before they are attended"""
+        eng = self._engine()
         eng.bind_pool(pool)
-        eng.set_kv_row(c0._row or 0)
+        eng.set_kv_row(row)
+        if q8 is not None:
+            eng.set_prefill_kvq(q8, q8_row)
         return pool
 
     def _bind_q8(self, cache, need_tokens: int, decode: bool):
@@ -172,15 +180,10 @@ class LanguageModel:
         if pool.capacity < need_tokens:
             eng.stream.synchronize()
             pool.reserve(need_tokens, live_tokens=c0.offset)
+        row = c0._row or 0
         if decode:
-            eng.bind_kvq(pool)
-            eng.set_kv_row(c0._row or 0)
-            return pool
-        prefix = pool.to_bf16_pool(int(c0.offset))
-        eng.bind_pool(prefix)
-        eng.set_kv_row(c0._row or 0)
-        eng.set_prefill_kvq(pool)
-        return prefix
+            return self._bind_row(pool, row)
+        return self._bind_row(pool.to_bf16_pool(int(c0.offset)), row, pool, row)
 
     def _bind_batch_row(self, cache, need_tokens: int, decode: bool, chunk_end: Optional[int]):
         """the prefill of a row admitted to a kv_bits=8 batch pool (BatchKVQPool): the chunks run on a batch-1 bf16
@@ -210,10 +213,7 @@ class LanguageModel:
                     tmp.reserve(chunk_end, live_tokens=off)
         if bp.capacity < need_tokens:
             raise ValueError(f"kv_bits=8 batch pool holds {bp.capacity} positions per row, the row needs {need_tokens}")
-        eng.bind_pool(tmp)
-        eng.set_kv_row(0)
-        eng.set_prefill_kvq_row(bp, row)
-        return tmp
+        return self._bind_row(tmp, 0, bp, row)
 
     def _finish_batch_row(self, cache, n_tokens: int):
         """after a prefill chunk of a kv_bits=8 batch row: its bf16 layers move to the batch pool's row"""
