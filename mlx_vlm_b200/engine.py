@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _native as N
-from .models.cache import BatchKVQPool, KVPool, QuantizedKVPool
+from .models.cache import BATCH_LOG_STEPS, BatchKVQPool, KVPool, QuantizedKVPool
 
 
 def _inv_freq(dim: int, base: float) -> np.ndarray:
@@ -206,7 +206,7 @@ class Engine:
         ldv = (self.cfg.vocab + 7) // 8 * 8      # rows are padded to 16-byte multiples (tail = -inf)
         return self._view(p, self._batch_B * ldv, torch.bfloat16).view(self._batch_B, ldv)[:, :self.cfg.vocab]
 
-    BATCH_LOG_STEPS, BATCH_LOG_ROWS = 4096, 16
+    BATCH_LOG_STEPS, BATCH_LOG_ROWS = BATCH_LOG_STEPS, 16
 
     def batch_token_log_view(self) -> torch.Tensor:
         """int32 (steps since the last batch_begin, 16) view of the batched decoder's token log"""

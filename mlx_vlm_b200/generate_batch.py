@@ -11,10 +11,10 @@ How the rows run on the CUDA engine: LOCK STEP on the device (csrc/decode_batch.
 rows live in ONE batched KV pool (layers, 2, rows, kv heads, capacity, head_dim), each with its own
 length (no left padding); a decode step is one captured CUDA graph that streams the weights ONCE
 for all rows (weight-major wgmma GEMMs with the rows as a 16-wide token tile), so B rows cost
-about one batch-1 step.  Admission of a request = a batch-1 prefill straight into a free row of
-the pool; a finished row is replaced by the last row (one row copy); the device state is re-armed
-only when the set of rows changes.  Tokens are produced in slices of `decode_slice` steps and
-surfaced one per row per `next()` call.  Scheduling policy is the reference's: decode-first, then
+about one batch-1 step.  `models/cache.py::BatchRows` owns the pool's rows: admission of a request =
+a prefill straight into the next free row; after rows finish the remaining rows move down (row
+copies); every row's length; and when the device state is re-armed (`BatchRows.arm`).  Tokens are
+produced in slices of `decode_slice` steps and surfaced one per row per `next()` call.  Scheduling policy is the reference's: decode-first, then
 admit up to `prefill_batch_size` waiting prompts (shortest first) while fewer than
 `completion_batch_size` rows are active.  Engines without the batched decoder (the CPU stand-in
 of the host-logic tests) run the rows time-multiplexed over the batch-1 path instead.
@@ -108,7 +108,6 @@ class _Row:
     last_token: int = -1       # last computed token (input of the next decode step)
     buffer: List[Tuple[int, float]] = field(default_factory=list)
     reserve: int = 0
-    ctx: int = 0               # tokens in the row's KV cache (lock-step mode)
 
 
 class GenerationBatch:
@@ -222,9 +221,7 @@ class BatchGenerator:
                 "than hidden / heads), whose 8-bit policy is the single-request one")
         if self._lockstep:
             self.completion_batch_size = min(self.completion_batch_size, 16)
-        self._pool = None          # the shared batched KV pool (lock-step mode)
-        self._armed_key = None     # (uids, live flags) the device state was armed for
-        self._steps_since_begin = 0
+        self._rows: Optional[cache_mod.BatchRows] = None   # the rows of the shared batched KV pool (lock-step mode)
         self.uid_count = 0
         self._unprocessed_sequences: List[_Row] = []
         self._generation_batch = GenerationBatch.empty()
@@ -255,6 +252,11 @@ class BatchGenerator:
     def _active(self) -> List[_Row]:
         return self._generation_batch.rows
 
+    @property
+    def _pool(self):
+        """the shared batched KV pool of lock-step mode (owned by `_rows`; None before the first admission)"""
+        return None if self._rows is None else self._rows.pool
+
     def remove(self, uid) -> bool:
         for i, r in enumerate(self._unprocessed_sequences):   # waiting in the queue
             if r.uid == uid:
@@ -262,11 +264,15 @@ class BatchGenerator:
                 return True
         if uid in self._generation_batch.uids:                 # already decoding
             idx = self._generation_batch.uids.index(uid)
-            self._generation_batch.filter([i for i in range(len(self._generation_batch)) if i != idx])
-            if self._lockstep:
-                self._compact()
+            self._keep([i for i in range(len(self._generation_batch)) if i != idx])
             return True
         return False
+
+    def _keep(self, keep: List[int]):
+        """the active rows `keep` (ascending) stay; in lock-step mode their pool rows move down to stay compact"""
+        self._generation_batch.filter(keep)
+        if self._rows is not None:
+            self._rows.filter(keep)
 
     @property
     def unprocessed_prompts(self):
@@ -298,7 +304,7 @@ class BatchGenerator:
         return s
 
     def close(self):
-        self._generation_batch.filter([])
+        self._keep([])
         self._unprocessed_sequences.clear()
 
     # ------------------------------------------------------------------ device work
@@ -308,33 +314,50 @@ class BatchGenerator:
         with torch.cuda.stream(eng.stream):   # ordered after the snapshot copy; .item() syncs it
             return float(lp.view(-1)[tok].float().item())
 
-    def _prefill(self, row: _Row) -> PromptProgress:
-        """Embeddings + prefill for one row; the fused head + sampler leave the first token in
-        the engine's token log."""
-        model, lm, eng = self.model, self.model.language_model, self.model.engine
-        tic = time.perf_counter()
+    def _embed(self, row: _Row):
+        """the row's prompt embeddings (vision tower + merge unless the request brings `inputs_embeds`); sets the
+        row's `reserve` and M-RoPE `delta`.  Returns (ids, embeddings, position_ids, rope_deltas)."""
         kw = dict(row.kwargs)
         ids = np.asarray([row.ids])
         emb = kw.pop("inputs_embeds", None)
         pos, deltas = kw.pop("position_ids", None), kw.pop("rope_deltas", None)
         if emb is None:
-            out = model.get_input_embeddings(ids, kw.pop("pixel_values", None), mask=kw.pop("mask", None), **kw)
+            out = self.model.get_input_embeddings(ids, kw.pop("pixel_values", None), mask=kw.pop("mask", None), **kw)
             emb, pos, deltas = out.inputs_embeds, out.position_ids, out.rope_deltas
-        T = emb.shape[1]
-        row.reserve = T + row.max_tokens + 1
-        if self._lockstep:
-            row.cache = lm.make_cache_row(self._pool_for(row.reserve), len(self._active) + self._admitting)
-            self._admitting += 1
-        else:
-            row.cache = cache_mod.make_prompt_cache(lm)
+        row.reserve = emb.shape[1] + row.max_tokens + 1
         row.delta = int(np.asarray(deltas).reshape(-1)[0]) if deltas is not None else 0
+        return ids, emb, pos, deltas
+
+    def _pool_rows(self, need_tokens: int) -> cache_mod.BatchRows:
+        """the rows of the shared batched pool, with room for `need_tokens` positions per row: allocated with
+        `completion_batch_size` rows at the first admission, grown (capacity doubling) when a row needs more"""
+        if self._rows is None:
+            lm = self.model.language_model
+            self._rows = cache_mod.BatchRows.allocate(self.model.engine, lm.args.num_hidden_layers, lm.n_kv_heads,
+                                                      lm.head_dim, self.completion_batch_size, need_tokens,
+                                                      self.kv_bits, self.kv_group_size)
+        else:
+            self._rows.ensure(self._rows.B, need_tokens)
+        return self._rows
+
+    def _prefill(self, row: _Row) -> PromptProgress:
+        """Embeddings + prefill for one row; the fused head + sampler leave the first token in
+        the engine's token log.  In lock-step mode the row is prefilled into the next free row of the pool."""
+        lm, eng = self.model.language_model, self.model.engine
+        tic = time.perf_counter()
+        ids, emb, pos, deltas = self._embed(row)
+        if self._lockstep:
+            rows = self._pool_rows(row.reserve)
+            cache = lm.make_cache_row(rows.pool, rows.B)
+        else:
+            cache = row.cache = cache_mod.make_prompt_cache(lm)
         step = self.prefill_step_size
         ids_left = ids
         while step is not None and emb.shape[1] > step + 1:   # chunked prefill (ar.py:426-472)
-            lm(ids_left[:, :step], inputs_embeds=emb[:, :step], cache=row.cache, position_ids=pos,
+            lm(ids_left[:, :step], inputs_embeds=emb[:, :step], cache=cache, position_ids=pos,
                rope_deltas=deltas, logits_to_keep=1, reserve_tokens=row.reserve)
             emb, ids_left = emb[:, step:], ids_left[:, step:]
-        out = lm(ids_left, inputs_embeds=emb, cache=row.cache, position_ids=pos, rope_deltas=deltas,
+        out = lm(ids_left, inputs_embeds=emb, cache=cache, position_ids=pos, rope_deltas=deltas,
                  logits_to_keep=1, reserve_tokens=row.reserve)
         if self.greedy_sampling:
             host = _host_buf(1)
@@ -345,10 +368,11 @@ class BatchGenerator:
         else:
             tok, lp = self._sample(out.logits[:, -1, :])
         row.last_token, row.n_decoded = tok, 1
-        row.ctx = int(row.cache[0].offset)
         row.buffer.append((tok, lp))
-        if self.kv_bits is not None and self._lockstep:
-            self._pool._admit = None   # the bf16 pool of the admission (csrc: prefill write-through) is done
+        if self._lockstep:
+            rows.admit(int(cache[0].offset))
+            if self.kv_bits is not None:
+                rows.pool.end_admission()
         dt = time.perf_counter() - tic
         self._prompt_tokens_counter += len(row.ids)
         self._prompt_time_counter += dt
@@ -359,31 +383,18 @@ class BatchGenerator:
         """`PromptProcessingBatch` (ar.py:1581-2175): the rows admitted together are prefilled in ONE pass over the
         weights (tokens concatenated, block-diagonal causal attention, every token scattered to its own pool row);
         embeddings (vision tower + merge) are still produced per request."""
-        model, lm, eng = self.model, self.model.language_model, self.model.engine
+        lm = self.model.language_model
         tic = time.perf_counter()
-        ids_l, emb_l, pos_l, del_l = [], [], [], []
-        for row in rows:
-            kw = dict(row.kwargs)
-            ids = np.asarray([row.ids])
-            emb = kw.pop("inputs_embeds", None)
-            pos, deltas = kw.pop("position_ids", None), kw.pop("rope_deltas", None)
-            if emb is None:
-                out = model.get_input_embeddings(ids, kw.pop("pixel_values", None), mask=kw.pop("mask", None), **kw)
-                emb, pos, deltas = out.inputs_embeds, out.position_ids, out.rope_deltas
-            row.reserve = emb.shape[1] + row.max_tokens + 1
-            row.delta = int(np.asarray(deltas).reshape(-1)[0]) if deltas is not None else 0
-            ids_l.append(ids); emb_l.append(emb); pos_l.append(pos); del_l.append(deltas)
-        pool = self._pool_for(max(r.reserve for r in rows))
-        base = len(self._active)
-        for i, row in enumerate(rows):
-            row.cache = lm.make_cache_row(pool, base + i)
-        toks = lm.prefill_rows(ids_l, emb_l, [r.cache for r in rows], pos_l, del_l,
-                               reserve_tokens=max(r.reserve for r in rows))
+        ids_l, emb_l, pos_l, del_l = zip(*[self._embed(row) for row in rows])
+        reserve = max(r.reserve for r in rows)
+        pool_rows = self._pool_rows(reserve)
+        caches = [lm.make_cache_row(pool_rows.pool, pool_rows.B + i) for i in range(len(rows))]
+        toks = lm.prefill_rows(list(ids_l), list(emb_l), caches, list(pos_l), list(del_l), reserve_tokens=reserve)
         dt = time.perf_counter() - tic
         out = []
-        for row, tok in zip(rows, toks):
+        for row, tok, cache in zip(rows, toks, caches):
             row.last_token, row.n_decoded = tok, 1
-            row.ctx = int(row.cache[0].offset)
+            pool_rows.admit(int(cache[0].offset))
             row.buffer.append((tok, 0.0))
             self._prompt_tokens_counter += len(row.ids)
             out.append(PromptProgress(uid=row.uid, prompt_tokens=len(row.ids), prompt_time=dt / len(rows),
@@ -401,87 +412,43 @@ class BatchGenerator:
             return tok, float(logprobs.reshape(-1)[tok].float().item())
 
     # ------------------------------------------------------------------ lock-step rows
-    _admitting = 0
-
-    def _pool_for(self, need_tokens: int):
-        """the shared batched pool, with room for `need_tokens` positions per row"""
-        lm, eng = self.model.language_model, self.model.engine
-        step = cache_mod.KVPool.step
-        cap = ((need_tokens + step - 1) // step) * step
-        if self._pool is None and self.kv_bits is not None:
-            self._pool = cache_mod.BatchKVQPool(lm.args.num_hidden_layers, lm.n_kv_heads, lm.head_dim, eng.device,
-                                                group_size=self.kv_group_size, batch=self.completion_batch_size,
-                                                capacity=cap, stream=eng.stream)
-        elif self._pool is None:
-            self._pool = cache_mod.KVPool(lm.args.num_hidden_layers, lm.n_kv_heads, lm.head_dim, eng.device,
-                                          batch=self.completion_batch_size, capacity=cap)
-        elif cap > self._pool.capacity:
-            import contextlib
-            eng.stream.synchronize()
-            on = torch.cuda.stream(eng.stream) if torch.cuda.is_available() else contextlib.nullcontext()
-            with on:
-                self._pool.reserve(cap, live_tokens=self._pool.capacity)
-            self._armed_key = None
-        return self._pool
-
-    def _compact(self):
-        """rows are pool rows 0..B-1 in `_active` order: after a filter, move rows down"""
-        eng = self.model.engine
-        for slot, row in enumerate(self._active):
-            cur = row.cache[0]._row
-            if cur != slot:
-                eng.kv_copy_row(self._pool, slot, self._pool, cur, row.ctx)
-                for c in row.cache:
-                    c._row = slot
-                self._armed_key = None
-
     def _lockstep_slice(self):
         """one slice of lock-step decode steps for every row that still has tokens to compute"""
-        eng = self.model.engine
-        rows = self._active
-        live = [r.n_decoded < r.max_tokens for r in rows]
+        eng, rows = self.model.engine, self._rows
+        active = self._active
+        live = [r.n_decoded < r.max_tokens for r in active]
         if not any(live):
             return
-        k = min([self.decode_slice] + [r.max_tokens - r.n_decoded for r, a in zip(rows, live) if a])
+        k = min([self.decode_slice] + [r.max_tokens - r.n_decoded for r, a in zip(active, live) if a])
         greedy = self.greedy_sampling
         if not greedy:
             k = 1
-        key = (tuple(r.uid for r in rows), tuple(live))
-        if key != self._armed_key or self._steps_since_begin + k > 4000 or not greedy:
-            eng.bind_pool(self._pool)
-            eng.batch_begin([r.last_token for r in rows], [r.ctx for r in rows],
-                            [r.ctx + (r.delta or 0) for r in rows], [int(a) for a in live])
-            self._armed_key = key
-            self._steps_since_begin = 0
+        # greedy: the device feeds each step's tokens to the next; otherwise the host's sampled tokens are uploaded
+        rows.arm(k, [r.last_token for r in active], [r.delta or 0 for r in active], live, fed_back=greedy)
+        first = rows.steps
         eng.batch_decode(k, want_logprobs=not greedy)
-        B = len(rows)
+        rows.advance(k, live)
+        B = len(active)
         if greedy:
             toks = _host_buf(k * B).view(k, B)
             lps = torch.empty(k, B, dtype=torch.float32)
             lps = lps.pin_memory() if torch.cuda.is_available() else lps
-            eng.batch_fetch(self._steps_since_begin, k, toks, lps)
+            eng.batch_fetch(first, k, toks, lps)
             eng.stream.synchronize()
-            self._steps_since_begin += k
-            for b, (r, a) in enumerate(zip(rows, live)):
+            for b, (r, a) in enumerate(zip(active, live)):
                 if not a:
                     continue
                 col = toks[:, b].tolist()
                 r.buffer.extend((int(t), float(l)) for t, l in zip(col, lps[:, b].tolist()))
-                r.last_token, r.n_decoded, r.ctx = int(col[-1]), r.n_decoded + k, r.ctx + k
-                for c in r.cache:
-                    c.offset = r.ctx
+                r.last_token, r.n_decoded = int(col[-1]), r.n_decoded + k
         else:   # sampler on the host-visible logits of every row (one step at a time)
             logits = eng.batch_logits_view("logits")
-            self._steps_since_begin += 1
-            for b, (r, a) in enumerate(zip(rows, live)):
+            for b, (r, a) in enumerate(zip(active, live)):
                 if not a:
                     continue
                 tok, lp = self._sample(logits[b:b + 1])
                 r.buffer.append((tok, lp))
-                r.last_token, r.n_decoded, r.ctx = tok, r.n_decoded + 1, r.ctx + 1
-                for c in r.cache:
-                    c.offset = r.ctx
-            self._armed_key = None
+                r.last_token, r.n_decoded = tok, r.n_decoded + 1
 
     def _decode_slice(self, row: _Row):
         """Refill the row's token buffer: hand the engine to this row for up to `decode_slice`
@@ -543,28 +510,24 @@ class BatchGenerator:
             self._gen_tokens_counter += len(self._active)
             self._gen_time_counter += time.perf_counter() - tic
             if len(keep) < len(self._generation_batch):
-                self._generation_batch.filter(keep)
-                if self._lockstep:
-                    self._compact()
+                self._keep(keep)
         # 2. admit waiting prompts while there is room (shortest first)
         room = self.completion_batch_size - len(self._active)
-        n_admit = min(room, self.prefill_batch_size, len(self._unprocessed_sequences))
+        n_new = min(room, self.prefill_batch_size, len(self._unprocessed_sequences))
         admitted = []
-        self._admitting = 0
         # kv_bits=8 rows are admitted one at a time (the grouped prefill has no 8-bit write-through)
-        group = (self._lockstep and n_admit >= 2 and self.greedy_sampling and not self.compute_logprobs
+        group = (self._lockstep and n_new >= 2 and self.greedy_sampling and not self.compute_logprobs
                  and self.kv_bits is None
                  and hasattr(self.model.language_model, "prefill_rows") and self.batched_prefill
                  and (self.prefill_step_size is None
-                      or all(len(r.ids) <= self.prefill_step_size + 1 for r in self._unprocessed_sequences[:n_admit])))
+                      or all(len(r.ids) <= self.prefill_step_size + 1 for r in self._unprocessed_sequences[:n_new])))
         if group:
-            admitted = [self._unprocessed_sequences.pop(0) for _ in range(n_admit)]
+            admitted = [self._unprocessed_sequences.pop(0) for _ in range(n_new)]
             prompt_responses.extend(self._prefill_group(admitted))
-        for _ in range(0 if group else max(0, n_admit)):
+        for _ in range(0 if group else max(0, n_new)):
             row = self._unprocessed_sequences.pop(0)
             prompt_responses.append(self._prefill(row))
             admitted.append(row)
-        self._admitting = 0
         if admitted:
             self._generation_batch.extend(GenerationBatch(admitted))
         return prompt_responses, generation_responses

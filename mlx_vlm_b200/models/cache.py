@@ -17,7 +17,14 @@ from __future__ import annotations
 from contextlib import nullcontext
 from typing import Any, List, Optional
 
+import numpy as np
 import torch
+
+
+def _on(stream):
+    """make `stream` current for the enclosed allocations and copies (no-op without a CUDA stream, as on the CPU
+    stand-in engine of the host tests)"""
+    return torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else nullcontext()
 
 
 class KVPool:
@@ -95,7 +102,7 @@ class QuantizedKVPool:
         cap = ((max(n_tokens, 2 * self.capacity) + self.step - 1) // self.step) * self.step
         lead = (self.n_layers, 2, self.batch, self.n_kv, cap)
         ng = self.hd // self.group_size
-        with torch.cuda.stream(self.stream) if self.stream is not None else nullcontext():
+        with _on(self.stream):
             new = (torch.zeros(lead + (self.hd,), dtype=torch.uint8, device=self.device),
                    torch.zeros(lead + (ng,), dtype=torch.bfloat16, device=self.device),
                    torch.zeros(lead + (ng,), dtype=torch.bfloat16, device=self.device))
@@ -123,7 +130,7 @@ class QuantizedKVPool:
         """A bf16 pool of the same capacity holding the dequantized first n_tokens positions (the prefix a
         prefill chunk over this cache attends to)."""
         from .. import _native as N
-        with torch.cuda.stream(self.stream) if self.stream is not None else nullcontext():
+        with _on(self.stream):
             out = KVPool(self.n_layers, self.n_kv, self.hd, self.device, batch=self.batch, capacity=self.capacity,
                          stream=self.stream)
         assert out.capacity == self.capacity
@@ -165,6 +172,28 @@ class BatchKVQPool:
                                  capacity=capacity, stream=stream)
         self.bf = (KVPool(n_layers - self.n_q, n_kv_heads, head_dim, device, batch=batch, capacity=capacity,
                           stream=stream) if self.n_q < n_layers else None)
+        # (row, batch-1 bf16 KVPool) of the row being admitted: the prefill chunks of the admission run on that pool
+        # and write the 8-bit layers through to the row (DESIGN §3); None between admissions
+        self.admission = None
+
+    def admission_pool(self, row: int, done: int, chunk_end: int) -> KVPool:
+        """the bf16 pool of row `row`'s admission for a prefill chunk that starts at position `done` and ends at
+        `chunk_end`: a fresh pool for the first chunk, the same pool (grown to hold the chunk) for the next ones"""
+        if done == 0:
+            with _on(self.stream):
+                self.admission = (row, KVPool(self.n_layers, self.n_kv, self.hd, self.device, batch=1,
+                                              capacity=chunk_end, stream=self.stream))
+        elif self.admission is None or self.admission[0] != row:
+            raise NotImplementedError("a prefill chunk of a kv_bits=8 batch row must continue that row's admission")
+        elif self.admission[1].capacity < chunk_end:
+            self.stream.synchronize()
+            with _on(self.stream):
+                self.admission[1].reserve(chunk_end, live_tokens=done)
+        return self.admission[1]
+
+    def end_admission(self):
+        """the admitted row is complete in this pool: release its bf16 pool"""
+        self.admission = None
 
     @property
     def capacity(self) -> int:
@@ -181,7 +210,7 @@ class BatchKVQPool:
     def reserve(self, n_tokens: int, live_tokens: int = 0) -> bool:
         moved = self.q.reserve(n_tokens, live_tokens=live_tokens)
         if self.bf is not None:
-            with torch.cuda.stream(self.stream) if self.stream is not None else nullcontext():
+            with _on(self.stream):
                 self.bf.reserve(n_tokens, live_tokens=live_tokens)
             assert self.bf.capacity == self.q.capacity
         return moved
@@ -196,11 +225,9 @@ class BatchKVQPool:
 
     def row_caches(self, row: int) -> list:
         """per-layer views of row `row`: QuantizedKVCache on the 8-bit layers, KVCache on the bf16 one"""
-        out = [QuantizedKVCache(self.group_size, 8, pool=self.q, layer=l, row=row) for l in range(self.n_q)]
-        out += [KVCache(self.bf, l - self.n_q, row=row) for l in range(self.n_q, self.n_layers)]
-        for c in out:
-            c._batch_pool = self
-        return out
+        return ([QuantizedKVCache(self.group_size, 8, pool=self.q, layer=l, row=row, batch_pool=self)
+                 for l in range(self.n_q)] +
+                [KVCache(self.bf, l - self.n_q, row=row, batch_pool=self) for l in range(self.n_q, self.n_layers)])
 
 
 class _BaseCache:
@@ -221,10 +248,11 @@ class _BaseCache:
 class KVCache(_BaseCache):
     step = 256
 
-    def __init__(self, pool: Optional[KVPool] = None, layer: int = 0, row: Optional[int] = None):
+    def __init__(self, pool: Optional[KVPool] = None, layer: int = 0, row: Optional[int] = None, batch_pool=None):
         self._pool = pool
         self._layer = layer
         self._row = row   # None: the whole (batch-1) pool; r: row r of a batched pool
+        self.batch_pool = batch_pool   # the BatchKVQPool whose row this view is (its bf16 part), else None
         self.offset = 0
         self._own = None  # standalone storage when used without a pool (API parity)
 
@@ -350,12 +378,13 @@ class QuantizedKVCache(_BaseCache):
     step = 256
 
     def __init__(self, group_size: int = 64, bits: int = 8, pool: Optional[QuantizedKVPool] = None,
-                 layer: int = 0, row: Optional[int] = None):
+                 layer: int = 0, row: Optional[int] = None, batch_pool=None):
         _kvq_check(group_size, bits)
         self.group_size, self.bits = group_size, bits
         self._pool = pool
         self._layer = layer
         self._row = row
+        self.batch_pool = batch_pool   # the BatchKVQPool whose row this view is (its 8-bit part), else None
         self.offset = 0
 
     def _side(self, side: int):
@@ -646,11 +675,18 @@ class BatchKVCache(_BaseCache):
 # ------------------------------------------------------------------------------------------------
 # Device-resident batch cache of the lock-step decoder (csrc/decode_batch.cu)
 # ------------------------------------------------------------------------------------------------
+# steps the lock-step decoder's token log holds (csrc/decode_batch.cu `log_cap`), counted from the last
+# `b200_batch_begin`: a decode or fetch past it is refused
+BATCH_LOG_STEPS = 4096
+
+
 class BatchRows:
-    """Row bookkeeping of ONE batched device pool (layers, 2, rows, kv heads, capacity, head_dim)
-    shared by the per-layer `RowBatchKVCache` views.  Row b of the logical batch is row b of the
-    pool (live rows are kept compact); every row has its own length — there is no left padding
-    and no common write index, the kernels read the per-row lengths from device arrays.
+    """The one owner of the rows of ONE batched device pool (layers, 2, rows, kv heads, capacity, head_dim): its
+    allocation and growth, admission into the next free row, compaction after rows leave, every row's length, and
+    the arming of the lock-step decoder over them.  Row b of the logical batch is row b of the pool (live rows are
+    kept compact); every row has its own length — there is no left padding and no common write index, the kernels
+    read the per-row lengths from device arrays.  The per-layer `RowBatchKVCache` / `BatchQuantizedKVCache` views
+    share it.
 
     `filter / extend / extract / trim` are the reference's BatchKVCache operations
     (cache.py:1077-1201) as row copies inside / between pools (`b200_kv_copy_row`)."""
@@ -660,6 +696,22 @@ class BatchRows:
         self.eng = engine
         self.lengths: List[int] = list(lengths or [])
         self.version = 0   # bumped by every structural change (the decoder re-arms its rows)
+        self.steps = 0     # lock-step steps since the last batch_begin (the next row of the engine's token log)
+        self._armed = None  # (version, allocation key, live flags) the device state was armed for
+        self._sweep = None  # (state, 8-bit pool, layers served) of the current extract sweep
+
+    @classmethod
+    def allocate(cls, engine, n_layers: int, n_kv_heads: int, head_dim: int, rows: int, capacity: int = 0,
+                 kv_bits=None, group_size: int = 64) -> "BatchRows":
+        """an empty batch of `rows` rows of at least `capacity` positions (rounded up to whole 256-position steps):
+        a bf16 `KVPool`, or with kv_bits=8 a `BatchKVQPool` (the reference's batch rule)"""
+        capacity = max(capacity, KVPool.step)
+        if kv_bits is not None:
+            pool = BatchKVQPool(n_layers, n_kv_heads, head_dim, engine.device, group_size=group_size, batch=rows,
+                                capacity=capacity, stream=engine.stream)
+        else:
+            pool = KVPool(n_layers, n_kv_heads, head_dim, engine.device, batch=rows, capacity=capacity)
+        return cls(pool, engine)
 
     @property
     def B(self) -> int:
@@ -677,7 +729,7 @@ class BatchRows:
             else:
                 new = KVPool(p.n_layers, p.n_kv, p.hd, p.device, batch=rows, capacity=max(p.capacity, tokens),
                              dtype=p.dtype)
-            with torch.cuda.stream(self.eng.stream):
+            with _on(self.eng.stream):
                 for b, n in enumerate(self.lengths):
                     self.eng.kv_copy_row(new, b, p, b, n)
             new.generation = p.generation + 1
@@ -685,9 +737,16 @@ class BatchRows:
             self._touch()
         elif tokens > p.capacity:
             self.eng.stream.synchronize()
-            with torch.cuda.stream(self.eng.stream):
+            with _on(self.eng.stream):
                 p.reserve(tokens, live_tokens=max(self.lengths) if self.lengths else 0)
             self._touch()
+
+    def admit(self, length: int) -> int:
+        """the next free row, already filled in place with `length` positions (a prefill into it), joins the rows;
+        returns its index"""
+        self.lengths.append(int(length))
+        self._touch()
+        return self.B - 1
 
     def filter(self, keep):
         keep = [int(i) for i in keep]
@@ -709,15 +768,35 @@ class BatchRows:
     def append_row(self, src_pool: KVPool, src_row: int, length: int) -> int:
         self.ensure(self.B + 1, max(self.lengths + [length]))
         self.eng.kv_copy_row(self.pool, self.B, src_pool, src_row, length)
-        self.lengths.append(int(length))
-        self._touch()
-        return self.B - 1
+        return self.admit(length)
 
     def trim(self, n: int) -> int:
         n = min([n] + self.lengths) if self.lengths else 0
         self.lengths = [ln - n for ln in self.lengths]
         self._touch()
         return n
+
+    def arm(self, k: int, tokens, deltas, live, fed_back: bool) -> bool:
+        """Make the lock-step decoder ready to run `k` steps over these rows, arming it (bind the pool, batch_begin
+        with each row's next token, length, rope position = length + delta, and live flag) unless it is still armed
+        for them: re-arms when the rows or the live flags changed, when the pool's allocation changed, when the `k`
+        steps would run past the engine's token log, and when the next tokens come from the host (`fed_back` False)
+        rather than from the device's own feedback.  A re-arm uploads the values the device already holds.  Returns
+        whether it armed."""
+        live = [int(a) for a in live]
+        state = (self.version, self.key(), tuple(live))
+        if fed_back and state == self._armed and self.steps + k <= BATCH_LOG_STEPS:
+            return False
+        self.eng.bind_pool(self.pool)
+        self.eng.batch_begin(tokens, self.lengths, [n + int(d) for n, d in zip(self.lengths, deltas)], live)
+        self._armed, self.steps = state, 0
+        return True
+
+    def advance(self, k: int, live=None):
+        """`k` lock-step steps ran: the live rows (all rows when `live` is None) grew by k positions"""
+        live = [1] * self.B if live is None else live
+        self.lengths = [n + k if a else n for n, a in zip(self.lengths, live)]
+        self.steps += k
 
     def layer_caches(self) -> list:
         p = self.pool
@@ -733,13 +812,30 @@ class BatchRows:
             return (p.q.codes.data_ptr() if p.q.codes is not None else 0, p.capacity)
         return (p.buf.data_ptr() if p.buf is not None else 0,)
 
+    def extract_pool(self, idx: int, layer: int) -> QuantizedKVPool:
+        """The single-request 8-bit pool that 8-bit layer `layer`'s extract of row `idx` views.  The reference calls
+        extract on every layer in turn; as the layers of a request share one pool here, the extract of layer 0 copies
+        the row's 8-bit layers into a FRESH single-request pool and the extracts of the other 8-bit layers of that
+        same sweep (same rows state, row and length) view it.  Every sweep gets its own pool, so caches extracted
+        twice never share storage."""
+        state = (self.version, self.key(), idx, self.lengths[idx])
+        if layer == 0 or self._sweep is None or self._sweep[0] != state or layer in self._sweep[2]:
+            bp, n = self.pool, self.lengths[idx]
+            one = QuantizedKVPool(bp.n_q, bp.n_kv, bp.hd, bp.device, group_size=bp.group_size, batch=1,
+                                  capacity=max(n, 1), stream=self.eng.stream)
+            with _on(self.eng.stream):
+                self.eng.kvq_copy_row(one, 0, bp.q, idx, n)
+            self._sweep = (state, one, set())
+        self._sweep[2].add(layer)
+        return self._sweep[1]
 
-class RowBatchKVCache(_BaseCache):
-    """One layer's view of a `BatchRows` pool with the reference batch-cache surface
-    (`offset`, `keys`, `values`, `state`, `filter`, `extend`, `extract`, `trim`, `merge`, `size`,
-    `empty`, `nbytes`).  The pool is shared by all layers, so the structural operations act on the
-    WHOLE pool when invoked on layer 0 and are no-ops on the other layers (the reference calls them
-    on every layer's object in a loop; the net effect is the same)."""
+
+class _BatchLayerCache(_BaseCache):
+    """One layer's view of a `BatchRows` pool: the reference batch-cache row surface (`offset` = the per-row
+    lengths, `left_padding` zeros — rows here are not padded —, `size`, `empty`, `batch_size`, `trim`, `filter`,
+    `extend`, `make_mask`).  The pool is shared by all layers, so the structural operations act on the WHOLE pool
+    when invoked on layer 0 and are no-ops on the other layers (the reference calls them on every layer's object in
+    a loop; the net effect is the same)."""
 
     def __init__(self, rows: BatchRows, layer: int):
         self._rows = rows
@@ -747,13 +843,46 @@ class RowBatchKVCache(_BaseCache):
 
     @property
     def offset(self):
-        import numpy as np
         return np.asarray(self._rows.lengths, dtype=np.int64)
 
     @property
     def left_padding(self):
-        import numpy as np
         return np.zeros(self._rows.B, dtype=np.int64)
+
+    def size(self):
+        return max(self._rows.lengths) if self._rows.lengths else 0
+
+    def empty(self):
+        return self._rows.B == 0
+
+    def is_trimmable(self):
+        return True
+
+    @property
+    def batch_size(self) -> int:
+        return self._rows.B
+
+    def trim(self, n):
+        if self._layer == 0:
+            return self._rows.trim(n)
+        return min([n] + [ln + n for ln in self._rows.lengths]) if self._rows.lengths else 0
+
+    def filter(self, batch_indices):
+        if self._layer == 0:
+            idx = batch_indices.tolist() if hasattr(batch_indices, "tolist") else list(batch_indices)
+            self._rows.filter(idx)
+
+    def extend(self, other: "_BatchLayerCache"):
+        if self._layer == 0:
+            self._rows.extend(other._rows)
+
+    def make_mask(self, N: int, return_array: bool = False, **kwargs):
+        return None if N == 1 else "causal"   # per-row lengths are applied by the kernels
+
+
+class RowBatchKVCache(_BatchLayerCache):
+    """One bf16 layer's view of a `BatchRows` pool with the reference batch-cache surface (`keys`, `values`,
+    `state`, `extract`, `merge`, `nbytes` here, the row surface in `_BatchLayerCache`)."""
 
     def _planes(self):
         p = self._rows.pool
@@ -772,43 +901,12 @@ class RowBatchKVCache(_BaseCache):
         n = self.size()
         return self.keys[..., :n, :], self.values[..., :n, :], self.offset, self.left_padding
 
-    def size(self):
-        return max(self._rows.lengths) if self._rows.lengths else 0
-
-    def empty(self):
-        return self._rows.B == 0
-
-    def is_trimmable(self):
-        return True
-
-    @property
-    def batch_size(self) -> int:
-        return self._rows.B
-
-    def trim(self, n):
-        if self._layer == 0:
-            self._trimmed = self._rows.trim(n)
-            return self._trimmed
-        return min([n] + [ln + n for ln in self._rows.lengths]) if self._rows.lengths else 0
-
-    def filter(self, batch_indices):
-        if self._layer == 0:
-            idx = batch_indices.tolist() if hasattr(batch_indices, "tolist") else list(batch_indices)
-            self._rows.filter(idx)
-
-    def extend(self, other: "RowBatchKVCache"):
-        if self._layer == 0:
-            self._rows.extend(other._rows)
-
     def extract(self, idx: int) -> KVCache:
         """row `idx` as a standalone single-request KVCache of this layer (a copy)"""
         n = self._rows.lengths[idx]
         out = KVCache()
         out.update_and_fetch(self.keys[idx:idx + 1, :, :n].clone(), self.values[idx:idx + 1, :, :n].clone())
         return out
-
-    def make_mask(self, N: int, return_array: bool = False, **kwargs):
-        return None if N == 1 else "causal"   # per-row lengths are applied by the kernels
 
     @property
     def nbytes(self):
@@ -834,31 +932,19 @@ class RowBatchKVCache(_BaseCache):
         return cls(rows, c0._layer)
 
 
-class BatchQuantizedKVCache(_BaseCache):
+class BatchQuantizedKVCache(_BatchLayerCache):
     """One 8-bit layer's view of a `BatchRows` over a `BatchKVQPool`, with the reference's observable surface
     (models/cache.py:1747-1960): `keys` / `values` are (codes as uint32 (B, n_kv, S, head_dim / 4), scales, biases)
-    in mx.quantize's packing, `offset` the per-row lengths, `left_padding` zeros (rows here are not padded).  Rows
-    sit on the pool rows exactly as for `RowBatchKVCache`; `filter` / `extend` act on the whole pool from layer 0 and
-    move every plane byte for byte.  `extract` returns a single-request `QuantizedKVCache`."""
+    in mx.quantize's packing.  Rows sit on the pool rows exactly as for `RowBatchKVCache`; `filter` / `extend` move
+    every plane byte for byte.  `extract` returns a single-request `QuantizedKVCache`."""
 
     def __init__(self, rows: BatchRows, layer: int):
-        self._rows = rows
-        self._layer = layer
+        super().__init__(rows, layer)
         self.bits = 8
 
     @property
     def group_size(self) -> int:
         return self._rows.pool.group_size
-
-    @property
-    def offset(self):
-        import numpy as np
-        return np.asarray(self._rows.lengths, dtype=np.int64)
-
-    @property
-    def left_padding(self):
-        import numpy as np
-        return np.zeros(self._rows.B, dtype=np.int64)
 
     def _side(self, side: int):
         q = self._rows.pool.q
@@ -880,57 +966,12 @@ class BatchQuantizedKVCache(_BaseCache):
         k, v = self.keys, self.values
         return (tuple(x[..., :n, :] for x in k), tuple(x[..., :n, :] for x in v), self.offset, self.left_padding)
 
-    def size(self):
-        return max(self._rows.lengths) if self._rows.lengths else 0
-
-    def empty(self):
-        return self._rows.B == 0
-
-    def is_trimmable(self):
-        return True
-
-    @property
-    def batch_size(self) -> int:
-        return self._rows.B
-
-    def trim(self, n):
-        if self._layer == 0:
-            return self._rows.trim(n)
-        return min([n] + [ln + n for ln in self._rows.lengths]) if self._rows.lengths else 0
-
-    def filter(self, batch_indices):
-        if self._layer == 0:
-            idx = batch_indices.tolist() if hasattr(batch_indices, "tolist") else list(batch_indices)
-            self._rows.filter(idx)
-
-    def extend(self, other: "BatchQuantizedKVCache"):
-        if self._layer == 0:
-            self._rows.extend(other._rows)
-
     def extract(self, idx: int) -> QuantizedKVCache:
         """row `idx` as a single-request QuantizedKVCache of this layer (a byte copy of its first offset[idx]
-        positions).  The reference calls extract on every layer in turn; as the layers of a request share one pool
-        here, the extract of layer 0 copies the row's 8-bit layers into a FRESH single-request pool and the extracts
-        of the other 8-bit layers of that same sweep (same rows state, row and length) view it.  Every sweep gets its
-        own pool, so caches extracted twice never share storage."""
-        rows = self._rows
-        key = (rows.version, rows.key(), idx, rows.lengths[idx])
-        cached = getattr(rows, "_extracted", None)
-        if self._layer == 0 or cached is None or cached[0] != key or self._layer in cached[2]:
-            bp, n = rows.pool, rows.lengths[idx]
-            one = QuantizedKVPool(bp.n_q, bp.n_kv, bp.hd, bp.device, group_size=bp.group_size, batch=1,
-                                  capacity=max(n, 1), stream=rows.eng.stream)
-            with torch.cuda.stream(rows.eng.stream) if rows.eng.stream is not None else nullcontext():
-                rows.eng.kvq_copy_row(one, 0, bp.q, idx, n)
-            cached = (key, one, set())
-            rows._extracted = cached
-        cached[2].add(self._layer)
-        out = QuantizedKVCache(self.group_size, 8, pool=cached[1], layer=self._layer)
-        out.offset = rows.lengths[idx]
+        positions, in the pool of this extract sweep: `BatchRows.extract_pool`)"""
+        out = QuantizedKVCache(self.group_size, 8, pool=self._rows.extract_pool(idx, self._layer), layer=self._layer)
+        out.offset = self._rows.lengths[idx]
         return out
-
-    def make_mask(self, N: int, return_array: bool = False, **kwargs):
-        return None if N == 1 else "causal"
 
     @property
     def nbytes(self):

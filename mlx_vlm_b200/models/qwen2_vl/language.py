@@ -16,7 +16,7 @@ import torch
 
 from ..base import LanguageModelOutput
 from ..cache import (BatchKVQPool, BatchQuantizedKVCache, BatchRows, KVCache, KVPool, QuantizedKVCache,
-                     QuantizedKVPool, RowBatchKVCache)
+                     RowBatchKVCache)
 from .config import ModelConfig, TextConfig
 
 
@@ -127,17 +127,11 @@ class LanguageModel:
     def make_batch_cache(self, rows: int, capacity: int = 0, kv_bits=None, kv_group_size: int = 64):
         """device-resident batch cache for `rows` requests: (BatchRows, per-layer caches) — RowBatchKVCache, or with
         kv_bits=8 the reference's batch rule (BatchQuantizedKVCache where `should_quantize_kv_layer` holds)"""
-        eng = self._engine()
         if kv_bits is not None:
             from ..cache import _kvq_check
             _kvq_check(kv_group_size, kv_bits, self.head_dim)
-            pool = BatchKVQPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
-                                group_size=kv_group_size, batch=rows, capacity=max(capacity, KVPool.step),
-                                stream=eng.stream)
-        else:
-            pool = KVPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
-                          batch=rows, capacity=max(capacity, KVPool.step))
-        r = BatchRows(pool, eng)
+        r = BatchRows.allocate(self._engine(), self.args.num_hidden_layers, self.n_kv_heads, self.head_dim, rows,
+                               capacity, kv_bits, kv_group_size)
         return r, r.layer_caches()
 
     def _bind(self, cache, need_tokens: int, decode: bool = False, chunk_end: Optional[int] = None) -> KVPool:
@@ -146,7 +140,7 @@ class LanguageModel:
         if pool is None:
             raise ValueError("b200 LanguageModel needs caches from make_prompt_cache(language_model)")
         eng = self._engine()
-        if getattr(c0, "_batch_pool", None) is not None:
+        if c0.batch_pool is not None:
             return self._bind_batch_row(cache, need_tokens, decode, chunk_end)
         if any(isinstance(c, QuantizedKVCache) for c in cache):
             return self._bind_q8(cache, need_tokens, decode)
@@ -193,24 +187,10 @@ class LanguageModel:
         the prompt only (`chunk_end`: the end of this chunk), grown chunk by chunk; `need_tokens` (which includes
         the tokens still to be generated) sizes the batch pool"""
         c0 = cache[0]
-        bp, row, off = c0._batch_pool, c0._row, int(c0.offset)
+        bp, row = c0.batch_pool, c0._row
         if decode or chunk_end is None:
             raise NotImplementedError("a row of a kv_bits=8 batch pool decodes in the lock-step batch only")
-        eng = self._engine()
-        adm = getattr(bp, "_admit", None)
-        if off == 0 or adm is None or adm[0] != row:
-            if off != 0:
-                raise NotImplementedError("a prefill chunk of a kv_bits=8 batch row must continue that row's admission")
-            with torch.cuda.stream(eng.stream):
-                tmp = KVPool(self.args.num_hidden_layers, self.args.num_key_value_heads, self.head_dim, eng.device,
-                             batch=1, capacity=chunk_end, stream=eng.stream)
-            bp._admit = (row, tmp)
-        else:
-            tmp = adm[1]
-            if tmp.capacity < chunk_end:
-                eng.stream.synchronize()
-                with torch.cuda.stream(eng.stream):
-                    tmp.reserve(chunk_end, live_tokens=off)
+        tmp = bp.admission_pool(row, int(c0.offset), chunk_end)
         if bp.capacity < need_tokens:
             raise ValueError(f"kv_bits=8 batch pool holds {bp.capacity} positions per row, the row needs {need_tokens}")
         return self._bind_row(tmp, 0, bp, row)
@@ -218,12 +198,12 @@ class LanguageModel:
     def _finish_batch_row(self, cache, n_tokens: int):
         """after a prefill chunk of a kv_bits=8 batch row: its bf16 layers move to the batch pool's row"""
         eng = self._engine()
-        bp = cache[0]._batch_pool
+        bp = cache[0].batch_pool
         eng.set_prefill_kvq(None)
         if bp.bf is None:
             return
         from ... import _native as Nn
-        tmp = bp._admit[1]
+        tmp = bp.admission[1]
         src = tmp.buf[bp.n_q:]
         Nn.check(eng.lib.b200_pool_copy_row(bp.bf.buf.data_ptr(), bp.batch, bp.capacity, int(cache[0]._row),
                                             src.data_ptr(), 1, tmp.capacity, 0, bp.n_layers - bp.n_q, bp.n_kv,
@@ -282,7 +262,7 @@ class LanguageModel:
             Vp = (V + 7) // 8 * 8     # device rows are 16-byte aligned for any vocabulary
             all_logits = eng.empty((L, Vp)) if keep_all else None
             eng.prefill(emb.contiguous(), pos3, cache_offset, delta0, all_logits)
-            if getattr(cache[0], "_batch_pool", None) is not None:
+            if cache[0].batch_pool is not None:
                 self._finish_batch_row(cache, cache_offset + L)
             elif isinstance(cache[0], QuantizedKVCache):
                 eng.set_prefill_kvq(None)
@@ -429,18 +409,20 @@ class LanguageModel:
         return out
 
     # ----------------------------------------------------------- batched rows
-    def _arm_batch(self, rows: BatchRows, toks, deltas, need: int):
+    def _batch_step(self, rows: BatchRows, toks, deltas, reserve_tokens: int, fed_back: bool) -> int:
+        """one lock-step step of every row (all live) with room for it, the decoder armed as `BatchRows.arm`
+        decides; returns the step's row of the batched token log"""
         eng = self._engine()
         B = rows.B
         d = np.zeros(B, dtype=np.int64) if deltas is None else np.asarray(deltas, dtype=np.int64).reshape(-1)[:B]
         if d.shape[0] < B:
             d = np.resize(d, B)
-        rows.ensure(B, need)
-        eng.bind_pool(rows.pool)
-        ctx = np.asarray(rows.lengths, dtype=np.int64)
-        eng.batch_begin(np.asarray(toks).reshape(-1)[:B], ctx, ctx + d, np.ones(B, dtype=np.int32))
-        self._batch_key = (id(rows), rows.version, rows.key())
-        self._batch_step = 0
+        rows.ensure(B, max(max(rows.lengths) + 1, int(reserve_tokens)))
+        rows.arm(1, np.asarray(toks).reshape(-1)[:B], d, [1] * B, fed_back)
+        step = rows.steps
+        eng.batch_decode(1)
+        rows.advance(1)
+        return step
 
     def _fused_greedy_batch(self, ids, cache, **kwargs):
         """B > 1 rows in lock step (csrc/decode_batch.cu): ONE weight stream per step for all rows.
@@ -448,21 +430,13 @@ class LanguageModel:
         rows = getattr(cache[0], "_rows", None)
         if rows is None or rows.B != ids.shape[0]:
             return None
-        eng = self._engine()
         inputs = kwargs.get("_inputs_tensor", None)
         last = getattr(self, "_fused_last", None)
-        key = (id(rows), rows.version, rows.key())
-        chained = (last is not None and isinstance(inputs, torch.Tensor) and inputs.is_cuda and
-                   inputs.data_ptr() == last.data_ptr() and getattr(self, "_batch_key", None) == key and
-                   self._batch_step + 1 < eng.BATCH_LOG_STEPS and
-                   max(rows.lengths) + 1 <= rows.pool.capacity)
-        if not chained:
-            self._arm_batch(rows, ids[:, 0], kwargs.get("rope_deltas", None),
-                            max(max(rows.lengths) + 1, int(kwargs.get("reserve_tokens", 0))))
-        eng.batch_decode(1)
-        out = eng.batch_token_log_view()[self._batch_step, :rows.B]
-        self._batch_step += 1
-        rows.lengths = [n + 1 for n in rows.lengths]
+        fed_back = (last is not None and isinstance(inputs, torch.Tensor) and inputs.device == last.device and
+                    inputs.data_ptr() == last.data_ptr())
+        step = self._batch_step(rows, ids[:, 0], kwargs.get("rope_deltas", None),
+                                int(kwargs.get("reserve_tokens", 0)), fed_back)
+        out = self._engine().batch_token_log_view()[step, :rows.B]
         self._fused_last = out
         return out
 
@@ -476,12 +450,8 @@ class LanguageModel:
         V = self.args.vocab_size
         if L == 1 and inputs_embeds is None:
             assert B == rows.B, (B, rows.B)
-            self._arm_batch(rows, ids_host[:, 0], rope_deltas_kw,
-                            max(max(rows.lengths) + 1, int(reserve_tokens)))
-            eng.batch_decode(1)
-            self._batch_step = 1
+            self._batch_step(rows, ids_host[:, 0], rope_deltas_kw, reserve_tokens, fed_back=False)
             self._fused_last = None
-            rows.lengths = [n + 1 for n in rows.lengths]
             rows_logits = eng.empty((B, V))
             from ... import _native as Nn
             Nn.check(eng.lib.b200_memcpy_d2d(rows_logits.data_ptr(), eng.lib.b200_batch_logits(eng.h), B * V * 2,
