@@ -927,7 +927,7 @@ size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap) {
           (size_t)ATT_MAXCL * ATT_MAXG * d.hd + (size_t)8 * ATT_MAXG * d.hd) * 4;
 }
 
-int decode_prepare(const DecodeDims& d, int cluster) {
+int decode_prepare() {
   int rc;
   if ((rc = set_stream_attr<SM_QKV, 2>()) || (rc = set_stream_attr<SM_QKV, 6>()) ||
       (rc = set_stream_attr<SM_QKV, 10>()) || (rc = set_stream_attr<SM_ORES, 2>()) ||
@@ -938,6 +938,14 @@ int decode_prepare(const DecodeDims& d, int cluster) {
       (rc = set_stream_attr<SM_HEAD, 2>()) || (rc = set_stream_attr<SM_HEAD, 6>()) ||
       (rc = set_stream_attr<SM_HEAD, 10>()))
     return rc;
+  if ((rc = set_carveout(k_sample, 0)) || (rc = set_carveout(k_set_state, 0)) ||
+      (rc = set_carveout(k_qk_norm_rope<4>, 0)) || (rc = set_carveout(k_qk_norm_rope<2>, 0)))
+    return rc;
+  return B200_OK;
+}
+
+int attn_prepare(const DecodeDims& d, int cluster) {
+  int rc;
   if (d.cap <= ATT1_MAX_CAP) {
     const size_t smem = attn1_smem(d);
     B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
@@ -948,9 +956,6 @@ int decode_prepare(const DecodeDims& d, int cluster) {
     B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
     if ((rc = set_carveout(k_attn, (int)smem))) return rc;
   }
-  if ((rc = set_carveout(k_sample, 0)) || (rc = set_carveout(k_set_state, 0)) ||
-      (rc = set_carveout(k_qk_norm_rope<4>, 0)) || (rc = set_carveout(k_qk_norm_rope<2>, 0)))
-    return rc;
   return B200_OK;
 }
 

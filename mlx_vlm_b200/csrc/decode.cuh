@@ -106,7 +106,11 @@ void batch_decoder_destroy(void* handle);
 
 void decode_set_sm_count(int n);
 void decode_set_pdl(bool on);
-int decode_prepare(const DecodeDims& d, int cluster);
+// kernel attributes of the decode step that do not depend on the cache (once per engine)
+int decode_prepare();
+// the per-phase bf16 attention (k_attn1 up to 4096 positions, else k_attn on clusters of `cluster` CTAs): refuses a
+// capacity its shared memory cannot hold; run before the steps it serves
+int attn_prepare(const DecodeDims& d, int cluster);
 int head_grid();
 size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap);
 // qn / kn (Qwen3-VL q_norm / k_norm weights, both or neither): the QKV kernel leaves q / k unrotated and a second

@@ -138,7 +138,8 @@ struct b200_engine {
   int last_steps = 0;
   bool timing_valid = false;
   int attn_cluster = 8;
-  int prepared_cap = -1, prepared_cluster = -1;
+  bool decode_prepared = false;  // decode_prepare() has run for this engine
+  int attn_prepared_cap = -1, attn_prepared_cluster = -1;  // attn_prepare() has run for this capacity and cluster
   // megakernel
   int use_mega = 1;  // 0: one kernel per phase, 1: k_mega
   bool mega_fits = true;  // false: this shape / cache capacity does not fit the persistent kernel
@@ -1083,10 +1084,9 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   const bf16* h = (const bf16*)(e->ws + lm_ws(c, T).h);
   // last row through the fused head + sampler; arms the decode state
   const DecodeDims d = e->dims();
-  if (e->prepared_cap != e->kvb.cap || e->prepared_cluster != e->attn_cluster) {
-    if ((rc = decode_prepare(d, e->attn_cluster))) return rc;
-    e->prepared_cap = e->kvb.cap;
-    e->prepared_cluster = e->attn_cluster;
+  if (!e->decode_prepared) {
+    if ((rc = decode_prepare())) return rc;
+    e->decode_prepared = true;
   }
   e->ctx_host = ctx0 + T;
   e->pos_host = ctx0 + T + rope_delta;
@@ -1148,10 +1148,9 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_CUDA(cudaEventRecord(e->loc_ev, s));   // the table (and its staging copy) may be rewritten after this point
   if (rc) return rc;
   const DecodeDims d = e->dims();
-  if (e->prepared_cap != e->kvb.cap || e->prepared_cluster != e->attn_cluster) {
-    if ((rc = decode_prepare(d, e->attn_cluster))) return rc;
-    e->prepared_cap = e->kvb.cap;
-    e->prepared_cluster = e->attn_cluster;
+  if (!e->decode_prepared) {
+    if ((rc = decode_prepare())) return rc;
+    e->decode_prepared = true;
   }
   for (int g = 0; g < n_seq; ++g) {   // first token of every sequence: fused head + sampler on its last row
     if ((rc = launch_set_state(e->st, 0, segs[g].T, segs[g].T, 0, 0, e->embed, e->h, c.hidden, s))) return rc;
@@ -1201,10 +1200,9 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   if ((rc = launch_set_state(e->st, 0, e->ctx_host, e->pos_host, force_tokens_host ? 1 : 0, 0,
                              e->embed, e->h, e->cfg.hidden, s)))
     return rc;
-  if (e->prepared_cap != e->kvb.cap || e->prepared_cluster != e->attn_cluster) {
-    if ((rc = decode_prepare(e->dims(), e->attn_cluster))) return rc;
-    e->prepared_cap = e->kvb.cap;
-    e->prepared_cluster = e->attn_cluster;
+  if (!e->decode_prepared) {
+    if ((rc = decode_prepare())) return rc;
+    e->decode_prepared = true;
   }
   if (e->use_mega && e->mega_fits && !e->mega_ready) {
     if ((rc = mega_prepare(e, s))) {
@@ -1215,8 +1213,18 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
       e->mega_fits = false;
     }
   }
-  if (e->kvb.kind == KvKind::q8 && !(e->use_graph && e->gexec))
-    if ((rc = kvq_decode_prepare(e->dims(), e->attn_cluster))) return rc;
+  if (!(e->use_graph && e->gexec)) {
+    // the per-phase attention kernel: its capacity limit and shared memory apply to the steps it serves only, so a
+    // cache that k_mega holds is not refused for being too long for k_attn
+    if (e->kvb.kind == KvKind::q8) {
+      if ((rc = kvq_decode_prepare(e->dims(), e->attn_cluster))) return rc;
+    } else if (!e->active_mega() &&
+               (e->attn_prepared_cap != e->kvb.cap || e->attn_prepared_cluster != e->attn_cluster)) {
+      if ((rc = attn_prepare(e->dims(), e->attn_cluster))) return rc;
+      e->attn_prepared_cap = e->kvb.cap;
+      e->attn_prepared_cluster = e->attn_cluster;
+    }
+  }
   if (e->use_graph && !e->gexec) {
     // capture one step on the engine's own stream (capture does not execute)
     cudaGraph_t graph = nullptr;

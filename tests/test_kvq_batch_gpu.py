@@ -44,19 +44,30 @@ def _dequant(codes, scales, biases, gs):
     return _bf(s * codes.float() + b)
 
 
-@pytest.mark.parametrize("B", [1, 3, 16])
+# cap None: the largest capacity the kernel's scores fit (bd_attn_smem(d, 4) <= 200 KiB, decode_batch.cu), with 8 q heads
+# per kv head so that bd_attn_heads_per_cta picks 4 heads per CTA, and the last two rows near the capacity
+@pytest.mark.parametrize("B,cap", [(1, 512), (3, 512), (16, 512), (16, None)], ids=["1", "3", "16", "16-cap_limit"])
 @pytest.mark.parametrize("hd,gs", [(64, 32), (64, 64), (128, 32), (128, 64), (128, 128)])
-def test_batch_kvq_attention_op(B, hd, gs):
+def test_batch_kvq_attention_op(B, cap, hd, gs):
     from mlx_vlm_b200 import _native as N
     from oracle import mlx_semantics as S
     from _util import cmp_bf16
     lib = N.lib()
     torch.manual_seed(B * 1000 + hd + gs)
-    nkv, nh, cap = 2, (4 if hd == 64 else 8), 512
+    nkv, nh = 2, (4 if hd == 64 else 8)
+    limit = cap is None
+    if limit:
+        cap = (200 * 1024 // 4 - 6 * hd - 32 * hd) // 4 // 256 * 256
+        assert cap == (12032 if hd == 64 else 11520)
+        nkv, nh = 4, 32
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        assert nkv * 4 * B > sms >= nkv * 2 * B, "bd_attn_heads_per_cta must pick 4 heads per CTA"
     QKV = (nh + 2 * nkv) * hd
     rng = np.random.default_rng(B + hd + gs)
     ctx = rng.integers(0, 400, size=B).astype(np.int32)
     ctx[0] = 0 if B > 1 else ctx[0]
+    if limit:
+        ctx[-2:] = cap - 257, cap - 1
     # cache content of every row, quantized by the conversion kernel
     cache = (torch.randn(2, B, nkv, cap, hd, device="cuda") * 0.8).to(torch.bfloat16)
     codes, scales, biases = (t.view(2, B, nkv, cap, -1).contiguous()

@@ -115,7 +115,8 @@ def _check_pool(model, c, pool, ref, n):
 
 
 @pytest.mark.parametrize("hd,gs", [(64, 32), (64, 64), (128, 32), (128, 64), (128, 128)])
-@pytest.mark.parametrize("ctx,cluster", [(5, 1), (300, 8), (1000, 4)])
+# past 4096 positions: trailing ranks of 8 with few keys, one rank holding 4600, two ranks of 4500
+@pytest.mark.parametrize("ctx,cluster", [(5, 1), (300, 8), (1000, 4), (4500, 8), (4600, 1), (9000, 2)])
 def test_decode_attention_kernel(hd, gs, ctx, cluster):
     """k_attn_q8 on its own: the new row (staging plane, position ctx) is appended bit-exact to what the reference
     quantize gives, the rows before it are untouched, and the output is sdpa over the dequantized K/V (the new
