@@ -32,7 +32,7 @@ extern "C" {
 #define B200_ERR_UNSUPPORTED 3 /* device is not sm_90 (Hopper)                */
 #define B200_ERR_STATE 4       /* engine used before weights / cache bound    */
 
-#define B200_ABI_VERSION 1
+#define B200_ABI_VERSION 2
 
 const char* b200_last_error(void);
 int b200_abi_version(void);
@@ -46,7 +46,6 @@ int b200_device_check(int device, int* sm_count);
 /* qwen2_vl.py:44-45  pixel_values.astype(weight dtype) */
 int b200_cast_f32_bf16(const float* src, void* dst, long n, void* stream);
 
-/* epilogues of b200_gemm_bf16_tn */
 /* gemm_wt output modes / finish_rows normalisation kinds */
 #define B200_WT_BF16 0    /* C[t][n] = epi(bf16(acc + bias)) (+ residual), bf16            */
 #define B200_WT_PARTIAL 1 /* fp32 split-K partial tiles P[split][t][n] (finish_rows adds them) */
@@ -57,24 +56,17 @@ int b200_cast_f32_bf16(const float* src, void* dst, long n, void* stream);
 #define B200_NORM_RMS 1   /* mx.fast.rms_norm   (language.py:139-140)                      */
 #define B200_NORM_LN 2    /* mx.fast.layer_norm (vision.py:180-181)                        */
 
+/* epilogues of b200_gemm_wt */
 #define B200_EPI_NONE 0
 #define B200_EPI_GELU_FAST 1  /* nn.GELU(approx="fast")  vision.py:167          */
 #define B200_EPI_GELU_EXACT 2 /* nn.GELU()               vision.py:112          */
 #define B200_EPI_GELU_TANH 3  /* nn.GELU(approx="precise") (fp32 towers only)   */
 
-/* nn.Linear / nn.Conv3d(kernel==stride) / Embedding.as_linear:
- *   C[M,N] = epi( bf16( A[M,K] . W[N,K]^T + bias[N] ) )  then, if residual,
- *   C = bf16(residual + C).   A row pitch lda, C/residual row pitch ldc/ldr
- *   (elements).  Hopper tensor cores (wgmma), TMA-fed, fp32 accumulate in registers.
- *   Replaces every nn.Linear in models/qwen2_vl/{vision,language}.py and
- *   PatchEmbed.proj (vision.py:83-102).  K*2 bytes and lda*2 bytes must be
- *   multiples of 16. */
-int b200_gemm_bf16_tn(const void* A, long lda, const void* W, const void* bias,
-                      const void* residual, long ldr, void* C, long ldc,
-                      int M, int N, int K, int epilogue, void* stream);
-
-/* The same Linear, weight-major (gemm_wt.cu): weight rows on the UMMA M side, TN tokens
- * (16..256) on the N side, optional split-K.  mode B200_WT_BF16 as b200_gemm_bf16_tn;
+/* nn.Linear / nn.Conv3d(kernel==stride) / Embedding.as_linear, weight-major (gemm_wt.cu): Hopper tensor
+ * cores (wgmma), TMA-fed, fp32 accumulate in registers; weight rows on the wgmma M side, TN tokens (16..256)
+ * on the N side, optional split-K.  Replaces every nn.Linear in models/qwen2_vl/{vision,language}.py and
+ * PatchEmbed.proj (vision.py:83-102).  mode B200_WT_BF16: C[T,N] = epi( bf16( X[T,K] . W[N,K]^T + bias[N] ) )
+ * then, if residual, C = bf16(residual + C); row pitches ldx / ldc / ldr in elements (K and ldx multiples of 8).
  * B200_WT_PARTIAL: fp32 tiles partial[split][T][N] (bias / residual applied by
  * b200_finish_rows); B200_WT_SWIGLU: W = [gate; up] (N == 2*inter), C[T][inter] =
  * swiglu (mlp.py:9-15, activations.py:8-10).  cfg4 = {TN, k-blocks per stage, stages,
@@ -414,20 +406,16 @@ int b200_batch_kvq_attention(const float* qkv, const void* bias, const float* in
                              void* codes, void* scales, void* biases, int group_size, int pool_rows, int cap, void* out,
                              int B, int n_heads, int n_kv, int head_dim, const void* q_norm, const void* k_norm, float eps,
                              void* stream);
-/* BatchQuantizedKVCache.filter / extend / extract (models/cache.py:1747-1960) on 8-bit pools: b200_kv_copy_row for
- * any per-position plane set — bytes_per_position = head_dim (codes), 2 * head_dim / group_size (scales, biases) or
- * 2 * head_dim (bf16 K/V).  The bytes move unchanged. */
+/* BatchKVCache / BatchQuantizedKVCache.filter / extend / extract (models/cache.py:1077-1201, 1747-1960) on device
+ * pools: copy the first n_tokens positions of one row of a plane set (n_layers, 2, rows, n_kv, cap,
+ * bytes_per_position) into a row of another (or the same) one.  A bf16 pool is bytes_per_position = 2 * head_dim;
+ * the planes of an 8-bit pool are head_dim (codes) and 2 * head_dim / group_size (scales, biases).  The bytes move
+ * unchanged. */
 int b200_pool_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool, int src_batch,
                        int src_cap, int src_row, int n_layers, int n_kv, int bytes_per_position, int n_tokens,
                        void* stream);
-/* BatchKVCache.filter / extend / extract (cache.py:1077-1201) on device pools: copy the first
- * n_tokens positions of one row of a pool into a row of another (or the same) pool */
-int b200_kv_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool,
-                     int src_batch, int src_cap, int src_row, int n_layers, int n_kv, int hd,
-                     int n_tokens, void* stream);
 
 int b200_memcpy_d2d(void* dst, const void* src, long bytes, void* stream);
-int b200_memcpy_h2d(void* dst, const void* src_host, long bytes, void* stream);
 
 /* timing helper for bench.py: average device duration (ms) of the decode-step
  * graph over the last b200_engine_decode call, measured with CUDA events on the

@@ -39,7 +39,6 @@ SIGNATURES = {
     "b200_abi_version": (_I, []),
     "b200_device_check": (_I, [_I, C.POINTER(_I)]),
     "b200_cast_f32_bf16": (_I, [_P, _P, _L, _P]),
-    "b200_gemm_bf16_tn": (_I, [_P, _L, _P, _P, _P, _L, _P, _L, _I, _I, _I, _I, _P]),
     "b200_gemm_wt": (_I, [_P, _L, _P, _P, _P, _L, _P, _L, _P, _I, _I, _I, _I, _I, _I, _P, C.c_uint, _P]),
     "b200_gemm_wt_auto_config": (_I, [_I, _I, _I, _I, _I, _P]),
     "b200_finish_rows": (_I, [_P, _I, _P, _P, _L, _P, _L, _I, _P, _P, _F, _P, _L, _I, _I, _P]),
@@ -101,7 +100,6 @@ SIGNATURES = {
     "b200_batch_logits": (_P, [_P]),
     "b200_batch_logprobs": (_P, [_P]),
     "b200_batch_token_log": (_P, [_P]),
-    "b200_kv_copy_row": (_I, [_P, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "b200_engine_bind_kvq": (_I, [_P, _P, _P, _P, _I, _I, _I]),
     "b200_engine_set_prefill_kvq": (_I, [_P, _P, _P, _P, _I]),
     "b200_engine_bind_batch_kvq": (_I, [_P, _P, _P, _P, _I, _I, _P, _I, _I]),
@@ -112,7 +110,6 @@ SIGNATURES = {
     "b200_kvq_quantize": (_I, [_P, _I, _P, _P, _P, _I, _L, _I, _I, _I, _P]),
     "b200_kvq_dequantize": (_I, [_P, _P, _P, _I, _P, _I, _L, _I, _I, _I, _P]),
     "b200_memcpy_d2d": (_I, [_P, _P, _L, _P]),
-    "b200_memcpy_h2d": (_I, [_P, _P, _L, _P]),
     "b200_engine_last_decode_ms": (_F, [_P]),
 }
 
@@ -132,7 +129,7 @@ def lib() -> C.CDLL:
             fn = getattr(l, name)  # AttributeError if the .so lacks a declared symbol
             fn.restype = res
             fn.argtypes = args
-        if l.b200_abi_version() != 1:
+        if l.b200_abi_version() != 2:
             raise B200Error("libb200vlm.so ABI version mismatch")
         _lib = l
     return _lib

@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200vlm.so")
-SOURCES = ["engine.cu", "gemm_tn.cu", "rowops.cu", "attention.cu", "decode.cu", "decode_mega.cu",
+SOURCES = ["engine.cu", "rowops.cu", "attention.cu", "decode.cu", "decode_mega.cu",
            "attention_tc.cu", "gemm_wt.cu", "attention_fa.cu", "decode_batch.cu", "tower_f32.cu", "kvq.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -14,9 +14,6 @@
 //                   by the 4 threads of a quad), O += P . V with P as the register A operand
 // V is consumed as V^T ([head][dim][key], keys contiguous): a K-major B operand that TMA can
 // load directly; the rotary kernels emit it (rowops.cu: *_qkv_post).
-#include <mutex>
-#include <unordered_map>
-
 #include "common.cuh"
 #include "decode.cuh"
 #include "wgmma.cuh"
@@ -292,77 +289,12 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 }
 
 // ---- host: 3-D tensor maps ----------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn fa_get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-struct FaKey {
-  const void* ptr;
-  long s1, s2;
-  int d0, d1, d2, b0, b1, b2;
-  bool operator==(const FaKey& o) const {
-    return ptr == o.ptr && s1 == o.s1 && s2 == o.s2 && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && b0 == o.b0 &&
-           b1 == o.b1 && b2 == o.b2;
-  }
-};
-struct FaHash {
-  size_t operator()(const FaKey& k) const {
-    size_t h = std::hash<const void*>()(k.ptr);
-    for (long v : {k.s1, k.s2, (long)k.d0, (long)k.d1, (long)k.d2, (long)k.b0, (long)k.b1, (long)k.b2})
-      h = h * 1000003u ^ std::hash<long>()(v);
-    return h;
-  }
-};
 // bf16 tensor: dims (d0 contiguous, d1 with stride s1 elements, d2 with stride s2), box (b0, b1, b2)
 int fa_tmap3(const void* ptr, int d0, int d1, long s1, int d2, long s2, int b0, int b1, int b2, CUtensorMap* out) {
-  static std::unordered_map<FaKey, CUtensorMap, FaHash> cache;
-  static std::mutex mu;
-  FaKey key{ptr, s1, s2, d0, d1, d2, b0, b1, b2};
-  {
-    std::lock_guard<std::mutex> g(mu);
-    auto it = cache.find(key);
-    if (it != cache.end()) {
-      *out = it->second;
-      return B200_OK;
-    }
-  }
-  EncodeTiledFn enc = fa_get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled unavailable");
-    return B200_ERR_CUDA;
-  }
-  cuuint64_t gdim[3] = {(cuuint64_t)d0, (cuuint64_t)d1, (cuuint64_t)d2};
-  cuuint64_t gstr[2] = {(cuuint64_t)s1 * 2, (cuuint64_t)s2 * 2};
-  cuuint32_t box[3] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUtensorMap tm;
-  CUresult r = enc(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), gdim, gstr, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled(3d) failed (%d) ptr=%p dims=(%d,%d,%d) strides=(%ld,%ld) box=(%d,%d,%d)", (int)r,
-              ptr, d0, d1, d2, s1, s2, b0, b1, b2);
-    return B200_ERR_CUDA;
-  }
-  {
-    std::lock_guard<std::mutex> g(mu);
-    if (cache.size() > 16384) cache.clear();
-    cache[key] = tm;
-  }
-  *out = tm;
-  return B200_OK;
+  const cuuint64_t dims[3] = {(cuuint64_t)d0, (cuuint64_t)d1, (cuuint64_t)d2};
+  const cuuint64_t strides[2] = {(cuuint64_t)s1 * 2, (cuuint64_t)s2 * 2};
+  const cuuint32_t box[3] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2};
+  return bf16_tmap(3, ptr, dims, strides, box, out);
 }
 
 }  // namespace

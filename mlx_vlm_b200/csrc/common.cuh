@@ -145,19 +145,6 @@ inline bool first_use_on_device(unsigned long long* mask) {
   return true;
 }
 
-// Ask the L2 for [base, base + bytes) in 64 KB pieces, piece c by participant c mod n (fire and forget).  Used by the
-// latency-bound kernels of the lock-step decode step (attention, split-K finish) to pull the weights of the GEMMs that
-// FOLLOW them out of HBM while HBM is otherwise idle; weights are never written during a step, so no ordering is needed.
-__device__ __forceinline__ void l2_prefetch_span(const void* base, long bytes, int id, int n) {
-  constexpr long CH = 65536;
-  const char* b = reinterpret_cast<const char*>(base);
-  for (long c = id; c * CH < bytes; c += n) {
-    const long left = bytes - c * CH;
-    const unsigned sz = (unsigned)((left < CH ? left : CH) & ~15L);
-    if (sz) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(b + c * CH), "r"(sz) : "memory");
-  }
-}
-
 // ---- programmatic dependent launch -------------------------------------------------
 // Every kernel of the prefill / vision / batched-decode sequences starts with pdl_prologue():
 // it lets the NEXT kernel of the stream begin (its barrier set-up and the prefetch of its

@@ -167,8 +167,6 @@ int swiglu(const void* gu, void* out, int rows, int inter, cudaStream_t st);
 int embed_merge(const int* ids, int B, int T, const void* table, int hidden, const void* feats,
                 int n_feats, int image_token, int video_token, void* out, int* src_out,
                 cudaStream_t st);
-int gemm_bf16_tn(const void* A, long lda, const void* W, const void* bias, const void* residual,
-                 long ldr, void* C, long ldc, int M, int N, int K, int epilogue, cudaStream_t st);
 // weight-major wgmma GEMM (gemm_wt.cu) + the row op that finishes its split-K partials
 struct WtConfig {
   int TN, KS, stages, split;
@@ -195,8 +193,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
                   const WtExt* ext = nullptr);
 int finish_rows(const float* P, int S, const void* bias, const void* resid, long ldr, void* h_out,
                 long ldh, int norm_kind, const void* nw, const void* nb, float eps, void* xn, long ldx,
-                int T, int N, cudaStream_t st, const void* l2_prefetch = nullptr, long l2_prefetch_bytes = 0);
-void gemm_wt_set_pdl(bool on);
+                int T, int N, cudaStream_t st);
 int attention(const void* q, long q_ts, long q_hs, const void* k, long k_ts, long k_hs,
               const void* v, long v_ts, long v_hs, void* out, long o_ts, int n_heads, int n_kv,
               int hd, int Lq, int S, int causal, float scale, cudaStream_t st);

@@ -96,10 +96,6 @@ struct BdAttnP {
   float scale_bf;
   const bf16 *qn, *kn;  // Qwen3-VL q_norm / k_norm weights of the layer (nullptr: no q/k norm)
   float eps;
-  // weights of the GEMMs that follow (o_proj, gate/up, down): this kernel is a chain of dependent round trips that
-  // leaves HBM idle, so its CTAs ask the L2 for them up front (l2_prefetch_span; weights are static during a step)
-  const void* pf[3];
-  long pf_bytes[3];
   // 8-bit layer (Q8 variant): the layer's K codes / scales / biases of row 0.  Codes sit at the same element
   // offsets as the bf16 planes (row_stride, v_off); scales and biases at those offsets / gs.
   uint8_t* q8c;
@@ -163,12 +159,6 @@ __device__ __forceinline__ void bd_q8_val(const uint8_t* codes, const bf16* sc, 
 template <int HD, int AG, bool Q8>
 __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   bd_pdl_launch();
-  if (threadIdx.x == 0) {
-    const int n = gridDim.x * gridDim.y, id = blockIdx.y * gridDim.x + blockIdx.x;
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-      if (p.pf_bytes[i] > 0) l2_prefetch_span(p.pf[i], p.pf_bytes[i], id, n);
-  }
   extern __shared__ __align__(16) uint8_t bd_sm[];
   constexpr int NCH = HD / 8, half = HD / 2;
   constexpr int SEG = HD / 8;   // dims per lane in the P.V phase (lane = key sub-index x dim segment)
@@ -719,21 +709,6 @@ static int bd_set_smem_attrs() {
   return B200_OK;
 }
 
-// L2 prefetch budget of the latency-bound kernels of a step, in bytes (B200_BD_PREFETCH_MB).  DEFAULT 0 = off: the
-// prefetch traffic can lengthen the attention kernel's dependent round trips by more than the L2-resident weights save
-// the GEMMs (not measured on the H100, whose L2 is 50 MB).  Kept as a tuning knob.
-static long bd_prefetch_budget() {
-  static long v = -1;
-  if (v < 0) {
-    const char* e = getenv("B200_BD_PREFETCH_MB");
-    long mb = e ? atol(e) : 0;
-    if (mb < 0) mb = 0;
-    if (mb > 120) mb = 120;
-    v = mb << 20;
-  }
-  return v;
-}
-
 // one lock-step step as plain launches on `s` (also what gets captured)
 static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, long* launches) {
   const DecodeDims& dd = m.d;
@@ -761,16 +736,6 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
     ap.row_stride = m.row_stride; ap.out = d->att; ap.n_heads = dd.n_heads; ap.n_kv = dd.n_kv; ap.cap = dd.cap;
     ap.hsplit = hs; ap.scale_bf = dd.scale_bf;
     ap.qn = m.qn ? m.qn[l] : nullptr; ap.kn = m.kn ? m.kn[l] : nullptr; ap.eps = dd.eps;
-    {  // o_proj, then gate/up, then down, as far as the budget goes
-      long left = bd_prefetch_budget();
-      const void* w[3] = {lw.wo, lw.wgu, lw.wd};
-      const long bytes[3] = {(long)H * QH * 2, 2L * I * H * 2, (long)H * I * 2};
-      for (int i = 0; i < 3; ++i) {
-        ap.pf[i] = w[i];
-        ap.pf_bytes[i] = bytes[i] < left ? bytes[i] : left;
-        left -= ap.pf_bytes[i];
-      }
-    }
     if ((rc = bd_attn_dispatch(dd, ag_heads, dim3(dd.n_kv * hs, B), s, ap, q8))) return rc;
     if ((rc = gemm_wt_tuned(d->att, QH, lw.wo, nullptr, nullptr, 0, nullptr, 0, d->partial, d->partial_bytes, B, H, QH,
                             B200_EPI_NONE, B200_WT_PARTIAL, 0, true, m.sm_count, &split, s)))
@@ -785,11 +750,8 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
                             B200_EPI_NONE, B200_WT_PARTIAL, 0, true, m.sm_count, &split, s)))
       return rc;
     const bf16* nw = (l + 1 == m.n_layers) ? m.final_norm : m.layers[l + 1].ln1;
-    // the finish of `down` is the other HBM-idle spot: it asks for the next layer's qkv weights
-    const void* nq = (l + 1 == m.n_layers) ? nullptr : (const void*)m.layers[l + 1].wqkv;
-    const long nq_bytes = nq ? ((long)QKV * H * 2 < bd_prefetch_budget() ? (long)QKV * H * 2 : bd_prefetch_budget()) : 0;
     if ((rc = finish_rows(d->partial, split, nullptr, d->h, H, d->h, H, B200_NORM_RMS, nw, nullptr, dd.eps, d->xn, H, B,
-                          H, s, nq, nq_bytes)))
+                          H, s)))
       return rc;
     *launches += 7;
   }

@@ -38,6 +38,28 @@ static long plane_off(int layer, int side, int row, int rows, int n_kv, int cap)
   return (((long)layer * 2 + side) * rows + row) * n_kv * (long)cap;
 }
 
+// The reference's BatchKVCache.filter / extend / extract (models/cache.py:1077-1201) move rows between arrays: copy the
+// first n_tokens positions of one row of a plane set (layers, 2, rows, n_kv, cap, bytes_per_position) into a row of
+// another (or the same) one, byte for byte.  A bf16 pool is bytes_per_position = 2 * head_dim; the planes of an 8-bit
+// pool are head_dim (codes) and 2 * head_dim / group_size (scales, biases).
+extern "C" int b200_pool_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool,
+                                  int src_batch, int src_cap, int src_row, int n_layers, int n_kv, int bytes_per_position,
+                                  int n_tokens, void* stream) {
+  B200_REQUIRE(dst_pool && src_pool && dst_row >= 0 && dst_row < dst_batch && src_row >= 0 && src_row < src_batch &&
+                   n_tokens >= 0 && n_tokens <= dst_cap && n_tokens <= src_cap && bytes_per_position > 0,
+               "pool_copy_row: bad arguments");
+  if (n_tokens == 0) return B200_OK;
+  const size_t bp = (size_t)bytes_per_position;
+  for (int l = 0; l < n_layers; ++l)
+    for (int kv = 0; kv < 2; ++kv) {
+      const char* sp = (const char*)src_pool + plane_off(l, kv, src_row, src_batch, n_kv, src_cap) * bp;
+      char* dp = (char*)dst_pool + plane_off(l, kv, dst_row, dst_batch, n_kv, dst_cap) * bp;
+      B200_CUDA(cudaMemcpy2DAsync(dp, (size_t)dst_cap * bp, sp, (size_t)src_cap * bp, (size_t)n_tokens * bp, n_kv,
+                                  cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    }
+  return B200_OK;
+}
+
 // The KV cache the engine is bound to (caller-owned).  The kind decides which calls may use it: prefill needs bf16,
 // single-request decode bf16 or q8, the lock-step batch decoder bf16 or q8_batch.
 enum class KvKind { none, bf16, q8, q8_batch };
@@ -122,7 +144,6 @@ struct b200_engine {
     long n_launch = 0;
   };
   std::vector<SeqGraph> vis_graphs, pre_graphs;
-  bool seq_graphs = true;       // B200_SEQ_GRAPH=0: plain launches
   KvRef* kvref = nullptr;       // device: where the bound pool row lives (read by the captured prefill)
   KvRef* kvref_host = nullptr;  // pinned staging
   cudaEvent_t kvref_ev = nullptr;
@@ -509,7 +530,6 @@ static void build_pos_hw(const int* grid, int n_img, int ms, std::vector<int>* o
 template <class F>
 static int seq_run(b200_engine* e, std::vector<b200_engine::SeqGraph>& cache, const std::vector<long>& key,
                    cudaStream_t s, F body) {
-  if (!e->seq_graphs) return body();
   b200_engine::SeqGraph* g = nullptr;
   for (auto& c : cache)
     if (c.key == key) g = &c;
@@ -868,7 +888,6 @@ int b200_engine_create(const b200_qwen2vl_config* cfg, int device, b200_engine**
   e->device = device;
   e->sm_count = sm;
   decode_set_sm_count(sm);
-  if (const char* v = getenv("B200_SEQ_GRAPH")) e->seq_graphs = atoi(v) != 0;
   const auto& c = e->cfg;
   B200_CUDA(cudaMalloc(&e->st, sizeof(DecState)));
   B200_CUDA(cudaMemset(e->st, 0, sizeof(DecState)));
@@ -1415,34 +1434,9 @@ const void* b200_batch_logprobs(b200_engine* e) { return e ? batch_decoder_buffe
 /* device int32 [4096 steps][16 rows]: token of (step since the last begin, row) */
 const int* b200_batch_token_log(b200_engine* e) { return e ? (const int*)batch_decoder_buffer(e->batch, 2) : nullptr; }
 
-/* cache management of the batched pool (the reference's BatchKVCache.filter / extend / extract,
- * models/cache.py:1077-1201, move rows between arrays): copy the first n_tokens positions of one row
- * of a pool (n_layers, 2, batch, n_kv, cap, hd) into a row of another (or the same) pool */
-int b200_kv_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool, int src_batch,
-                     int src_cap, int src_row, int n_layers, int n_kv, int hd, int n_tokens, void* stream) {
-  B200_REQUIRE(dst_pool && src_pool && dst_row >= 0 && dst_row < dst_batch && src_row >= 0 && src_row < src_batch &&
-                   n_tokens >= 0 && n_tokens <= dst_cap && n_tokens <= src_cap,
-               "kv_copy_row: bad arguments");
-  if (n_tokens == 0) return B200_OK;
-  const size_t w = (size_t)n_tokens * hd * 2;
-  for (int l = 0; l < n_layers; ++l)
-    for (int kv = 0; kv < 2; ++kv) {
-      const char* sp = (const char*)src_pool + plane_off(l, kv, src_row, src_batch, n_kv, src_cap) * hd * 2;
-      char* dp = (char*)dst_pool + plane_off(l, kv, dst_row, dst_batch, n_kv, dst_cap) * hd * 2;
-      B200_CUDA(cudaMemcpy2DAsync(dp, (size_t)dst_cap * hd * 2, sp, (size_t)src_cap * hd * 2, w, n_kv,
-                                  cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-    }
-  return B200_OK;
-}
-
 int b200_memcpy_d2d(void* dst, const void* src, long bytes, void* stream) {
   B200_REQUIRE(dst && src && bytes >= 0, "memcpy_d2d: bad arguments");
   B200_CUDA(cudaMemcpyAsync(dst, src, (size_t)bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return B200_OK;
-}
-int b200_memcpy_h2d(void* dst, const void* src_host, long bytes, void* stream) {
-  B200_REQUIRE(dst && src_host && bytes >= 0, "memcpy_h2d: bad arguments");
-  B200_CUDA(cudaMemcpyAsync(dst, src_host, (size_t)bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream));
   return B200_OK;
 }
 float b200_engine_last_decode_ms(const b200_engine* e) {

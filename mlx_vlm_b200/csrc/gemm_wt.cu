@@ -22,6 +22,7 @@
 // Replaces nn.Linear of the reference (models/qwen2_vl/vision.py:83-102,108-119,132-133,168-169;
 // language.py:52-55; mlp.py:9-15; activations.py:8-10).  Rounding points follow
 // oracle/mlx_semantics.py::linear (+ activations, residual add).
+#include <array>
 #include <mutex>
 #include <unordered_map>
 #include <vector>
@@ -34,7 +35,7 @@ namespace b200 {
 
 namespace {
 
-constexpr int WT_ROWS = 128;        // weight rows per CTA (UMMA M)
+constexpr int WT_ROWS = 128;        // weight rows per CTA (the wgmma M side)
 constexpr int WT_BK = 64;           // one k-block: 64 bf16 = 128 B = one swizzle row
 constexpr int WT_WBLK = WT_ROWS * 128;  // bytes of one weight k-block tile
 constexpr int WT_MAX_STAGES = 16;
@@ -439,10 +440,9 @@ __global__ void __launch_bounds__(FIN_THREADS)
 finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ bias,
                    const bf16* __restrict__ resid, long ldr, bf16* __restrict__ h_out, long ldh,
                    int norm_kind, const bf16* __restrict__ nw, const bf16* __restrict__ nb, float eps,
-                   bf16* __restrict__ xn, long ldx, int T, int N, const void* pf, long pf_bytes) {
+                   bf16* __restrict__ xn, long ldx, int T, int N) {
   __shared__ float red[FIN_THREADS / 32];
   w_pdl_launch();
-  if (pf_bytes > 0 && threadIdx.x == 0) l2_prefetch_span(pf, pf_bytes, blockIdx.x, gridDim.x);
   w_pdl_wait();
   const int t = blockIdx.x;
   const int nv = N >> 2;
@@ -540,47 +540,49 @@ finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ 
   }
 }
 
-// ---- host: tensor maps ------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn wt_get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) ==
-            cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
+// 2-D K-major bf16 operand (rows x K, row pitch ld elements), box = box_rows x 64
+int wt_tmap(const void* ptr, long ld, int rows, int k, int box_rows, CUtensorMap* out) {
+  const cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {(cuuint32_t)WT_BK, (cuuint32_t)box_rows};
+  return bf16_tmap(2, ptr, dims, strides, box, out);
 }
-struct WtKey {
-  const void* ptr;
-  long ld;
-  int rows, k, box_rows;
-  bool operator==(const WtKey& o) const {
-    return ptr == o.ptr && ld == o.ld && rows == o.rows && k == o.k && box_rows == o.box_rows;
-  }
-};
-struct WtHash {
-  size_t operator()(const WtKey& k) const {
-    size_t h = std::hash<const void*>()(k.ptr);
-    h = h * 1000003u ^ std::hash<long>()(k.ld);
-    h = h * 1000003u ^ (size_t)k.rows;
-    h = h * 1000003u ^ (size_t)k.k;
-    h = h * 1000003u ^ (size_t)k.box_rows;
+
+// (ptr, rank, dims[3], strides[2], box[3]) of a tensor map, unused entries 0
+typedef std::array<cuuint64_t, 10> TmapKey;
+struct TmapHash {
+  size_t operator()(const TmapKey& k) const {
+    size_t h = 0;
+    for (cuuint64_t v : k) h = h * 1000003u ^ std::hash<cuuint64_t>()(v);
     return h;
   }
 };
-// 2-D K-major bf16 operand (rows x K, row pitch ld elements), box = box_rows x 64
-int wt_tmap(const void* ptr, long ld, int rows, int k, int box_rows, CUtensorMap* out) {
-  static std::unordered_map<WtKey, CUtensorMap, WtHash> cache;
+
+}  // namespace
+
+// ---- host: tensor maps (declared in wgmma.cuh; gemm_wt and attention_fa) ---------------------
+int bf16_tmap(int rank, const void* ptr, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
+              CUtensorMap* out) {
+  B200_REQUIRE(rank == 2 || rank == 3, "bf16_tmap: rank %d", rank);
+  typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static const EncodeTiledFn enc = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+                    qres == cudaDriverEntryPointSuccess;
+    return ok ? reinterpret_cast<EncodeTiledFn>(p) : nullptr;
+  }();
+  static std::unordered_map<TmapKey, CUtensorMap, TmapHash> cache;
   static std::mutex mu;
-  WtKey key{ptr, ld, rows, k, box_rows};
+  TmapKey key{};
+  key[0] = (cuuint64_t)(uintptr_t)ptr;
+  key[1] = (cuuint64_t)rank;
+  for (int i = 0; i < rank; ++i) {
+    key[2 + i] = dims[i];
+    key[7 + i] = box[i];
+    if (i > 0) key[4 + i] = strides[i - 1];
+  }
   {
     std::lock_guard<std::mutex> g(mu);
     auto it = cache.find(key);
@@ -589,22 +591,20 @@ int wt_tmap(const void* ptr, long ld, int rows, int k, int box_rows, CUtensorMap
       return B200_OK;
     }
   }
-  EncodeTiledFn enc = wt_get_encode();
   if (!enc) {
     set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
     return B200_ERR_CUDA;
   }
-  cuuint64_t gdim[2] = {(cuuint64_t)k, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)WT_BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
   CUtensorMap tm;
-  CUresult r = enc(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstr,
+  CUresult r = enc(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d) ptr=%p ld=%ld rows=%d k=%d box_rows=%d", (int)r, ptr,
-              ld, rows, k, box_rows);
+    set_error("cuTensorMapEncodeTiled failed (%d) rank=%d ptr=%p dims=(%llu,%llu,%llu) strides=(%llu,%llu) "
+              "box=(%llu,%llu,%llu)", (int)r, rank, ptr, (unsigned long long)key[2], (unsigned long long)key[3],
+              (unsigned long long)key[4], (unsigned long long)key[5], (unsigned long long)key[6],
+              (unsigned long long)key[7], (unsigned long long)key[8], (unsigned long long)key[9]);
     return B200_ERR_CUDA;
   }
   {
@@ -615,12 +615,6 @@ int wt_tmap(const void* ptr, long ld, int rows, int k, int box_rows, CUtensorMap
   *out = tm;
   return B200_OK;
 }
-
-static bool g_wt_pdl = true;
-
-}  // namespace
-
-void gemm_wt_set_pdl(bool on) { g_wt_pdl = on; }
 
 static int round16(int x) { return (x + 15) & ~15; }
 
@@ -771,7 +765,7 @@ int gemm_wt(const void* X, long ldx, const void* W, const void* bias, const void
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at;
-  lc.numAttrs = g_wt_pdl ? 1 : 0;
+  lc.numAttrs = 1;
   const bool tower = mode == B200_WT_F32 || mode == B200_WT_SPLIT, wide = cfg.TN > 128;
   if (tower) {
     B200_CUDA(cudaLaunchKernelEx(&lc, wide ? gemm_wt_kernel<true, 16> : gemm_wt_kernel<true, 8>, tw, tx, p));
@@ -1008,7 +1002,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
 
 int finish_rows(const float* P, int S, const void* bias, const void* resid, long ldr, void* h_out,
                 long ldh, int norm_kind, const void* nw, const void* nb, float eps, void* xn, long ldx,
-                int T, int N, cudaStream_t st, const void* pf, long pf_bytes) {
+                int T, int N, cudaStream_t st) {
   B200_REQUIRE(P && S >= 1 && T > 0 && N > 0 && (N % 4) == 0 && N <= FIN_N_MAX,
                "finish_rows: T=%d N=%d S=%d", T, N, S);
   B200_REQUIRE(norm_kind == B200_NORM_NONE || (xn && (norm_kind != B200_NORM_RMS || nw)),
@@ -1023,15 +1017,15 @@ int finish_rows(const float* P, int S, const void* bias, const void* resid, long
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at;
-  lc.numAttrs = g_wt_pdl ? 1 : 0;
+  lc.numAttrs = 1;
   if (few_rows) {
     B200_CUDA(cudaLaunchKernelEx(&lc, finish_rows_kernel<1024, 2>, P, S, (const bf16*)bias, (const bf16*)resid, ldr,
                                  (bf16*)h_out, ldh, norm_kind, (const bf16*)nw, (const bf16*)nb, eps,
-                                 (bf16*)xn, ldx, T, N, pf, pf_bytes));
+                                 (bf16*)xn, ldx, T, N));
   } else {
     B200_CUDA(cudaLaunchKernelEx(&lc, finish_rows_kernel<256, 8>, P, S, (const bf16*)bias, (const bf16*)resid, ldr,
                                  (bf16*)h_out, ldh, norm_kind, (const bf16*)nw, (const bf16*)nb, eps,
-                                 (bf16*)xn, ldx, T, N, pf, pf_bytes));
+                                 (bf16*)xn, ldx, T, N));
   }
   return B200_OK;
 }

@@ -396,22 +396,3 @@ int b200_batch_kvq_attention(const float* qkv, const void* bias, const float* in
                              group_size, pool_rows, cap, (bf16*)out, B, n_heads, n_kv, head_dim, (const bf16*)q_norm,
                              (const bf16*)k_norm, eps, sms, (cudaStream_t)stream);
 }
-
-/* row copy of any per-position plane set (bf16 K/V, 8-bit codes, scales or biases): byte-exact */
-int b200_pool_copy_row(void* dst_pool, int dst_batch, int dst_cap, int dst_row, const void* src_pool, int src_batch,
-                       int src_cap, int src_row, int n_layers, int n_kv, int bytes_per_position, int n_tokens,
-                       void* stream) {
-  B200_REQUIRE(dst_pool && src_pool && dst_row >= 0 && dst_row < dst_batch && src_row >= 0 && src_row < src_batch &&
-                   n_tokens >= 0 && n_tokens <= dst_cap && n_tokens <= src_cap && bytes_per_position > 0,
-               "pool_copy_row: bad arguments");
-  if (n_tokens == 0) return B200_OK;
-  const size_t bp = (size_t)bytes_per_position, w = (size_t)n_tokens * bp;
-  for (int l = 0; l < n_layers; ++l)
-    for (int kv = 0; kv < 2; ++kv) {
-      const char* sp = (const char*)src_pool + ((((size_t)l * 2 + kv) * src_batch + src_row) * n_kv) * (size_t)src_cap * bp;
-      char* dp = (char*)dst_pool + ((((size_t)l * 2 + kv) * dst_batch + dst_row) * n_kv) * (size_t)dst_cap * bp;
-      B200_CUDA(cudaMemcpy2DAsync(dp, (size_t)dst_cap * bp, sp, (size_t)src_cap * bp, w, n_kv, cudaMemcpyDeviceToDevice,
-                                  (cudaStream_t)stream));
-    }
-  return B200_OK;
-}

@@ -6,9 +6,16 @@
 // Shared-memory operands are K-major with the 128-byte swizzle TMA writes: rows of 128 B
 // (64 bf16 of K), 8-row groups 1024 B apart; a 16-wide K step advances the start address by 32 B.
 #pragma once
+#include <cuda.h>
 #include <stdint.h>
 
 namespace b200 {
+
+// Host: the TMA descriptor of a bf16 tensor of rank 2 or 3 that fills such operands: dims[0] is the contiguous
+// dimension, strides[i] the byte stride of dimension i + 1, box the tile in elements.  128-byte swizzle, 256-byte L2
+// promotion, no out-of-bounds fill.  Encoded once per (ptr, rank, dims, strides, box) and cached; B200_OK or an error.
+int bf16_tmap(int rank, const void* ptr, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
+              CUtensorMap* out);
 
 // shared-memory matrix descriptor: start address >> 4 [0,14), leading byte offset (unused for
 // swizzled K-major) [16,30), stride byte offset = 1024 >> 4 [32,46), 128-byte swizzle [62,64)

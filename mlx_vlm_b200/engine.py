@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _native as N
-from .models.cache import BATCH_LOG_STEPS, BatchKVQPool, KVPool, QuantizedKVPool
+from .models.cache import BATCH_LOG_STEPS, BatchKVQPool, QuantizedKVPool
 
 
 def _inv_freq(dim: int, base: float) -> np.ndarray:
@@ -214,23 +214,13 @@ class Engine:
         return self._view(p, self.BATCH_LOG_STEPS * self.BATCH_LOG_ROWS, torch.int32).view(self.BATCH_LOG_STEPS,
                                                                                         self.BATCH_LOG_ROWS)
 
-    def kvq_copy_row(self, dst, dst_row: int, src, src_row: int, n_tokens: int):
-        """row copy between 8-bit pools (QuantizedKVPool): codes, scales and biases, byte for byte"""
-        ng = src.hd // src.group_size
-        for plane, bpp in (("codes", src.hd), ("scales", 2 * ng), ("biases", 2 * ng)):
-            N.check(self.lib.b200_pool_copy_row(getattr(dst, plane).data_ptr(), dst.batch, dst.capacity, int(dst_row),
-                                                getattr(src, plane).data_ptr(), src.batch, src.capacity, int(src_row),
-                                                src.n_layers, src.n_kv, bpp, int(n_tokens), self.s), "pool_copy_row")
-
-    def kv_copy_row(self, dst: KVPool, dst_row: int, src: KVPool, src_row: int, n_tokens: int):
-        if isinstance(dst, BatchKVQPool):   # the 8-bit layers, then the bf16 ones
-            self.kvq_copy_row(dst.q, dst_row, src.q, src_row, n_tokens)
-            if dst.bf is not None:
-                self.kv_copy_row(dst.bf, dst_row, src.bf, src_row, n_tokens)
-            return
-        N.check(self.lib.b200_kv_copy_row(dst.buf.data_ptr(), dst.batch, dst.capacity, int(dst_row), src.buf.data_ptr(),
-                                          src.batch, src.capacity, int(src_row), dst.n_layers, dst.n_kv, dst.hd,
-                                          int(n_tokens), self.s), "kv_copy_row")
+    def kv_copy_row(self, dst, dst_row: int, src, src_row: int, n_tokens: int):
+        """the first n_tokens positions of row src_row of `src` into row dst_row of `dst`, two pools of one type and
+        layout (KVPool, QuantizedKVPool or BatchKVQPool): every plane set of the pool, byte for byte"""
+        for (d, n_layers, bpp), (s, _, _) in zip(dst.plane_sets(), src.plane_sets(), strict=True):
+            N.check(self.lib.b200_pool_copy_row(d.data_ptr(), dst.batch, dst.capacity, int(dst_row), s.data_ptr(),
+                                                src.batch, src.capacity, int(src_row), n_layers, dst.n_kv, bpp,
+                                                int(n_tokens), self.s), "pool_copy_row")
 
     def set_next(self, token: int, ctx: int, position: int):
         N.check(self.lib.b200_engine_set_next(self.h, int(token), int(ctx), int(position), self.s),

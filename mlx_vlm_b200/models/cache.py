@@ -57,6 +57,10 @@ class KVPool:
         self.generation += 1
         return True
 
+    def plane_sets(self) -> list:
+        """(tensor, layers, bytes per position) of each plane set a row copy moves (`Engine.kv_copy_row`)"""
+        return [(self.buf, self.n_layers, 2 * self.hd)]
+
 
 def _kvq_check(group_size: int, bits, head_dim: Optional[int] = None):
     if bits != 8:
@@ -113,6 +117,12 @@ class QuantizedKVPool:
         self.capacity = cap
         self.generation += 1
         return True
+
+    def plane_sets(self) -> list:
+        """(tensor, layers, bytes per position) of each plane set a row copy moves: codes, scales, biases"""
+        ng = self.hd // self.group_size
+        return [(self.codes, self.n_layers, self.hd), (self.scales, self.n_layers, 2 * ng),
+                (self.biases, self.n_layers, 2 * ng)]
 
     @classmethod
     def from_pool(cls, pool: KVPool, n_tokens: int, group_size: int) -> "QuantizedKVPool":
@@ -222,6 +232,10 @@ class BatchKVQPool:
     def bytes_per_position(self) -> int:
         """bytes of one position of one row over all layers"""
         return self.q.bytes_per_position() + (self.n_layers - self.n_q) * 2 * self.n_kv * self.hd * 2
+
+    def plane_sets(self) -> list:
+        """(tensor, layers, bytes per position) of each plane set a row copy moves: the 8-bit ones, then the bf16 one"""
+        return self.q.plane_sets() + (self.bf.plane_sets() if self.bf is not None else [])
 
     def row_caches(self, row: int) -> list:
         """per-layer views of row `row`: QuantizedKVCache on the 8-bit layers, KVCache on the bf16 one"""
@@ -689,7 +703,7 @@ class BatchRows:
     share it.
 
     `filter / extend / extract / trim` are the reference's BatchKVCache operations
-    (cache.py:1077-1201) as row copies inside / between pools (`b200_kv_copy_row`)."""
+    (cache.py:1077-1201) as row copies inside / between pools (`Engine.kv_copy_row`)."""
 
     def __init__(self, pool: KVPool, engine, lengths: Optional[List[int]] = None):
         self.pool = pool
@@ -824,7 +838,7 @@ class BatchRows:
             one = QuantizedKVPool(bp.n_q, bp.n_kv, bp.hd, bp.device, group_size=bp.group_size, batch=1,
                                   capacity=max(n, 1), stream=self.eng.stream)
             with _on(self.eng.stream):
-                self.eng.kvq_copy_row(one, 0, bp.q, idx, n)
+                self.eng.kv_copy_row(one, 0, bp.q, idx, n)
             self._sweep = (state, one, set())
         self._sweep[2].add(layer)
         return self._sweep[1]

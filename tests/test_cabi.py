@@ -23,7 +23,7 @@ def test_library_builds_and_exports_every_declared_symbol():
         assert hasattr(lib, n), f"{n} declared in include/b200vlm.h but not exported"
         assert n in N.SIGNATURES, f"{n} has no ctypes signature in _native.py"
     assert set(N.SIGNATURES) <= set(names), sorted(set(N.SIGNATURES) - set(names))
-    assert lib.b200_abi_version() == 1
+    assert lib.b200_abi_version() == 2
     assert isinstance(lib.b200_last_error(), bytes)
 
 

@@ -29,6 +29,7 @@ def _cfg(c):
     (8, 1536, 1536, 0, True, False, (16, 2, 6, 1)),     # decode batch
     (576, 1280, 1176, 0, False, False, None),           # patch embed (K tail 1176 = 18*64+24)
     (700, 1000, 520, 1, True, True, (256, 1, 2, 1)),    # large token tile, ragged N, gelu + residual
+    (272, 1536, 8960, 0, False, True, None),            # LM down + residual, no bias
 ])
 def test_gemm_wt_bf16(lib, T, N, K, epi, bias, res, cfg):
     from mlx_vlm_b200 import _native as Nn
@@ -63,6 +64,7 @@ def test_gemm_wt_bf16(lib, T, N, K, epi, bias, res, cfg):
     (576, 1280, 5120, (192, 2, 2, 4), "ln"),     # ViT fc2: split-K 4 + residual + LayerNorm
     (8, 1536, 8960, (16, 2, 6, 10), "rms"),      # decode batch
     (272, 1536, 1536, (96, 2, 3, 4), "none"),    # o_proj, no norm
+    (272, 1536, 1536, (96, 2, 3, 4), "rms_inplace"),  # o_proj, residual added in place (h_out == resid), as in the engine
 ])
 def test_gemm_wt_partial_and_finish_rows(lib, T, N, K, cfg, kind):
     from mlx_vlm_b200 import _native as Nn
@@ -77,17 +79,18 @@ def test_gemm_wt_partial_and_finish_rows(lib, T, N, K, cfg, kind):
     P = torch.full((cfg[3], T, N), 7.0, dtype=torch.float32, device="cuda")
     Nn.check(lib.b200_gemm_wt(dX.data_ptr(), K, dW.data_ptr(), 0, 0, 0, 0, 0, P.data_ptr(), T, N, K, 0, PARTIAL,
                               0, _cfg(cfg), 0, 0), "gemm_wt partial")
-    hout, xn = torch.zeros_like(dh), torch.zeros_like(dh)
-    k = {"none": 0, "rms": 1, "ln": 2}[kind]
+    norm, inplace = kind.removesuffix("_inplace"), kind.endswith("_inplace")
+    hout, xn = dh if inplace else torch.zeros_like(dh), torch.zeros_like(dh)
+    k = {"none": 0, "rms": 1, "ln": 2}[norm]
     Nn.check(lib.b200_finish_rows(P.data_ptr(), cfg[3], db.data_ptr(), dh.data_ptr(), N, hout.data_ptr(), N, k,
-                                  dnw.data_ptr(), dnb.data_ptr() if kind == "ln" else 0, 1e-6, xn.data_ptr(),
+                                  dnw.data_ptr(), dnb.data_ptr() if norm == "ln" else 0, 1e-6, xn.data_ptr(),
                                   N, T, N, 0), "finish_rows")
     torch.cuda.synchronize()
-    cmp_bf16(hout, hw, f"finish_rows h {T}x{N} split={cfg[3]}")
+    cmp_bf16(hout, hw, f"finish_rows h {T}x{N} split={cfg[3]} {kind}")
     got_h = hout.float().cpu()
-    if kind == "rms":    # the norm is checked on the kernel's own h (identical inputs)
+    if norm == "rms":    # the norm is checked on the kernel's own h (identical inputs)
         cmp_bf16(xn, S.rms_norm(r, got_h, nw, 1e-6), "finish_rows rms_norm")
-    elif kind == "ln":
+    elif norm == "ln":
         cmp_bf16(xn, S.layer_norm(r, got_h, nw, nb, 1e-6), "finish_rows layer_norm")
 
 

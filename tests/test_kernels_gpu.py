@@ -32,61 +32,6 @@ def rnd(*shape, scale=1.0, seed=0):
     return R().r(torch.randn(*shape, generator=g) * scale)
 
 
-@pytest.mark.parametrize("M,N,K,epi,bias,res", [
-    (576, 1280, 1176, 0, False, False),   # patch embed (K tail 1176 = 18*64+24)
-    (576, 3840, 1280, 0, True, False),    # ViT qkv
-    (576, 5120, 1280, 1, True, False),    # fc1 + gelu_fast
-    (576, 1280, 5120, 0, True, True),     # fc2 + residual
-    (144, 5120, 5120, 2, True, False),    # merger fc1 + exact gelu
-    (272, 2048, 1536, 0, True, False),    # LM qkv
-    (272, 1536, 8960, 0, False, True),    # down + residual
-    (1, 256, 64, 0, True, False),         # single row, tiny
-    (130, 200, 72, 1, True, True),        # ragged M/N/K (N not multiple of 32/64)
-])
-def test_gemm(lib, M, N, K, epi, bias, res):
-    from mlx_vlm_b200 import _native as Nn
-    from oracle import mlx_semantics as S
-    r = R()
-    A = rnd(M, K, seed=1)
-    W = rnd(N, K, scale=0.05, seed=2)
-    b = rnd(N, scale=0.5, seed=3) if bias else None
-    resid = rnd(M, N, seed=4) if res else None
-    want = S.linear(r, A, W, b)
-    if epi == 1:
-        want = S.gelu_fast(r, want)
-    elif epi == 2:
-        want = S.gelu_exact(r, want)
-    if res:
-        want = r.r(resid + want)
-    dA, dW = to_dev(A), to_dev(W)
-    db = to_dev(b) if bias else None
-    dr = to_dev(resid) if res else None
-    ldn = ((N + 7) // 8) * 8
-    C = torch.zeros(M, ldn, dtype=torch.bfloat16, device="cuda")
-    if res:
-        drp = torch.zeros(M, ldn, dtype=torch.bfloat16, device="cuda")
-        drp[:, :N] = dr
-        dr = drp
-    Nn.check(lib.b200_gemm_bf16_tn(dA.data_ptr(), K, dW.data_ptr(), Nn.ptr(db), Nn.ptr(dr), ldn,
-                                   C.data_ptr(), ldn, M, N, K, epi, 0), "gemm")
-    torch.cuda.synchronize()
-    cmp_bf16(C[:, :N], want, f"gemm {M}x{N}x{K} epi={epi}")
-
-
-def test_gemm_inplace_residual(lib):
-    """the engine adds the residual in place (C == residual)"""
-    from mlx_vlm_b200 import _native as Nn
-    from oracle import mlx_semantics as S
-    r = R()
-    A, W, h = rnd(272, 1536, seed=5), rnd(1536, 1536, scale=0.03, seed=6), rnd(272, 1536, seed=7)
-    want = r.r(h + S.linear(r, A, W))
-    dA, dW, dh = to_dev(A), to_dev(W), to_dev(h)
-    Nn.check(lib.b200_gemm_bf16_tn(dA.data_ptr(), 1536, dW.data_ptr(), 0, dh.data_ptr(), 1536,
-                                   dh.data_ptr(), 1536, 272, 1536, 1536, 0, 0), "gemm")
-    torch.cuda.synchronize()
-    cmp_bf16(dh, want, "gemm in-place residual")
-
-
 @pytest.mark.parametrize("rows,dim", [(576, 1280), (3, 1536), (1, 256)])
 def test_norms(lib, rows, dim):
     from mlx_vlm_b200 import _native as Nn

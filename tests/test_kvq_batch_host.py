@@ -95,18 +95,14 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "kvq
 
 
 class _HostRowCopies:
-    """the engine's row copies (b200_pool_copy_row / b200_kv_copy_row) restated with torch on host pools: this test
-    checks which rows the cache operations move where; the device copies are checked byte for byte on the GPU"""
+    """the engine's row copy (`Engine.kv_copy_row`: b200_pool_copy_row over each plane set of the pool) restated with
+    torch on host pools: this test checks which rows the cache operations move where; the device copies are checked
+    byte for byte on the GPU"""
     stream = None
 
-    def kvq_copy_row(self, dst, dst_row, src, src_row, n):
-        for name in ("codes", "scales", "biases"):
-            getattr(dst, name)[:, :, dst_row, :, :n].copy_(getattr(src, name)[:, :, src_row, :, :n].clone())
-
     def kv_copy_row(self, dst, dst_row, src, src_row, n):
-        self.kvq_copy_row(dst.q, dst_row, src.q, src_row, n)
-        if dst.bf is not None:
-            dst.bf.buf[:, :, dst_row, :, :n].copy_(src.bf.buf[:, :, src_row, :, :n].clone())
+        for (d, _, _), (s, _, _) in zip(dst.plane_sets(), src.plane_sets(), strict=True):
+            d[:, :, dst_row, :, :n].copy_(s[:, :, src_row, :, :n].clone())
 
 
 def _write_rows(pool, keys, values, gs, start=0):

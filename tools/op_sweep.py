@@ -1,7 +1,6 @@
-"""Back-to-back timing (CUDA events, warm, weights rotated over NBUF buffers so they stream from HBM
-like in a real layer loop) of the prefill-side ops at the C2 shapes, through the C ABI.
-usage: python tools/op_sweep.py [iters]   -> one line per op: us per call, TFLOP/s or GB/s"""
-import ctypes as C
+"""Back-to-back timing (CUDA events, warm) of the prefill-side attention and row ops at the C2 shapes, through
+the C ABI.  The GEMMs (gemm_wt) have their own sweep, tools/wt_sweep.py.
+usage: python tools/op_sweep.py [iters]   -> one line per op: us per call, TFLOP/s"""
 import os
 import sys
 
@@ -12,7 +11,6 @@ from mlx_vlm_b200 import _native as N
 
 lib = N.lib()
 iters = int(sys.argv[1]) if len(sys.argv) > 1 else 40
-NBUF = 6
 dev = "cuda:0"
 
 
@@ -31,22 +29,6 @@ def timeit(fn, n=iters):
     e1.record()
     torch.cuda.synchronize()
     return e0.elapsed_time(e1) * 1e3 / n
-
-
-def gemm_case(name, M, Nn, K, epi=0, bias=True, res=False):
-    A = [bf(M, K) for _ in range(2)]
-    W = [bf(Nn, K, scale=0.03) for _ in range(NBUF)]
-    b = bf(Nn) if bias else None
-    Cc = torch.empty(M, Nn, device=dev, dtype=torch.bfloat16)
-    R_ = bf(M, Nn) if res else None
-
-    def fn(i):
-        N.check(lib.b200_gemm_bf16_tn(A[i & 1].data_ptr(), K, W[i % NBUF].data_ptr(), N.ptr(b), N.ptr(R_), Nn,
-                                      Cc.data_ptr(), Nn, M, Nn, K, epi, 0), "gemm")
-    us = timeit(fn)
-    print(f"gemm {name:14s} M={M:4d} N={Nn:6d} K={K:5d}: {us:8.2f} us  {2.0 * M * Nn * K / us / 1e6:7.1f} TFLOP/s  "
-          f"(W {Nn * K * 2 / 1e6:.1f} MB -> {Nn * K * 2 / us / 1e3:.0f} GB/s)", flush=True)
-    return us
 
 
 def attn_case(name, heads, kv, hd, L, S, causal):
@@ -85,27 +67,7 @@ def rowop_cases():
 
 
 if __name__ == "__main__":
-    tot_v = 0.0
-    tot_v += 32 * gemm_case("vit.qkv", 576, 3840, 1280)
-    tot_v += 32 * gemm_case("vit.proj", 576, 1280, 1280, res=True)
-    tot_v += 32 * gemm_case("vit.fc1", 576, 5120, 1280, epi=1)
-    tot_v += 32 * gemm_case("vit.fc2", 576, 1280, 5120, res=True)
-    gemm_case("vit.patch", 576, 1280, 1176, bias=False)
-    gemm_case("merger.fc1", 144, 5120, 5120, epi=2)
-    gemm_case("merger.fc2", 144, 1536, 5120)
-    tot_l = 0.0
-    tot_l += 28 * gemm_case("lm.qkv", 272, 2048, 1536)
-    tot_l += 28 * gemm_case("lm.o", 272, 1536, 1536, bias=False, res=True)
-    tot_l += 28 * gemm_case("lm.gateup", 272, 17920, 1536, bias=False)
-    tot_l += 28 * gemm_case("lm.down", 272, 1536, 8960, bias=False, res=True)
     a_v = 32 * attn_case("vit", 16, 16, 80, 576, 576, 0)
     a_l = 28 * attn_case("lm", 12, 2, 128, 272, 272, 1)
     rowop_cases()
-    # 7B / LLaVA-ish shapes
-    gemm_case("7b.qkv T=272", 272, 4608, 3584)
-    gemm_case("7b.gateup", 272, 37888, 3584, bias=False)
-    gemm_case("7b.down", 272, 3584, 18944, bias=False, res=True)
-    gemm_case("clip.fc1 8img", 4616, 4096, 1024, epi=1)
-    gemm_case("llama.gateup", 4656, 22016, 4096, bias=False)
-    print(f"sum: vit gemm {tot_v / 1e3:.2f} ms, lm gemm {tot_l / 1e3:.2f} ms, vit attn {a_v / 1e3:.2f} ms, "
-          f"lm attn {a_l / 1e3:.2f} ms")
+    print(f"sum: vit attn {a_v / 1e3:.2f} ms, lm attn {a_l / 1e3:.2f} ms")

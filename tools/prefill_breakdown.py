@@ -1,6 +1,6 @@
 """GPU time of the C2 vision tower and LM prefill in isolation (CUDA events around N back-to-back
-calls with no Python work in between), with the captured sequence graphs on / off.
-usage: [B200_SEQ_GRAPH=0] python tools/prefill_breakdown.py"""
+calls with no Python work in between; the sequences replay as captured graphs from their second call).
+usage: python tools/prefill_breakdown.py"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -43,5 +43,5 @@ for name, fn in (("vision tower (32 blocks + merger)", vis), ("LM prefill T=272 
     e1.record(eng.stream)
     t1 = time.perf_counter()
     eng.stream.synchronize()
-    print(f"{name}: {e0.elapsed_time(e1) / n:.3f} ms GPU per call, host enqueue {1e3 * (t1 - t0) / n:.3f} ms per call "
-          f"(SEQ_GRAPH={os.environ.get('B200_SEQ_GRAPH', '1')})", flush=True)
+    print(f"{name}: {e0.elapsed_time(e1) / n:.3f} ms GPU per call, host enqueue {1e3 * (t1 - t0) / n:.3f} ms per call",
+          flush=True)
