@@ -391,6 +391,33 @@ int b200_batch_decode(b200_engine* e, int n_steps, int want_logprobs, void* stre
  * host arrays [n_steps][B] */
 int b200_batch_fetch(b200_engine* e, long first_step, int n_steps, int* tok_host, float* lp_host,
                      void* stream);
+/* Per-row logits processors and top-k logprobs of the armed rows (sample_utils.make_logits_processors applied row by
+ * row, GenerationBatch._step ar.py:1060-1121), until the next b200_batch_begin (which turns them off).  Each step,
+ * between the head and the sampler, a row with processors appends its input token to its history and then applies,
+ * in place on its bf16 logits: logit bias, repetition, presence and frequency penalty over the last context-size
+ * tokens of the history, with the rounding points of the torch ops.  Device arrays owned by the caller, row b of
+ * each at b * its row width:
+ *   params int32 [rows][8]: flags (1 bias, 2 repetition, 4 presence, 8 frequency; 0 = none), repetition, presence
+ *     and frequency context sizes, number of bias entries; penalties fp32 [rows][8]: repetition penalty,
+ *     fp32(1 / repetition penalty), presence, frequency;
+ *   bias_ids int32 / bias_vals fp32 (bf16-exact) [rows][bias_cap], ids in [0, vocab);
+ *   hist int32 [rows][hist_cap] (hist_cap <= 1024) ring of each row's tokens, hist_len int32 [rows] tokens so far;
+ *     ids outside [0, vocab) in it are skipped.
+ * params NULL: no processors (no launch).  top_k 1..20: the k largest logprobs of every row and step go to a device
+ * log (ties: lower token id first); 0: none. */
+int b200_batch_set_procs(b200_engine* e, const int* params, const float* penalties, const int* bias_ids,
+                         const float* bias_vals, int bias_cap, int* hist, int* hist_len, int hist_cap, int top_k);
+/* top-k ids and logprobs of steps [first_step, first_step+n) since the last begin: host arrays [n_steps][B][20],
+ * the first top_k of each row valid */
+int b200_batch_fetch_topk(b200_engine* e, long first_step, int n_steps, int* ids_host, float* lp_host, void* stream);
+/* The kernels of b200_batch_set_procs on caller buffers, stream-ordered (one step of B <= 16 rows, device arrays):
+ * with params non-NULL the processors run in place on logits (B, ldv) bf16, appending tok[b] to row b's history
+ * where active[b]; with top_k > 0 the top-k of logprobs (B, ldv) bf16 over [0, vocab) go to top_ids / top_lp
+ * (B, 20).  History and bias ids outside [0, vocab) are skipped. */
+int b200_batch_procs_apply(void* logits, const void* logprobs, int B, int vocab, int ldv, const int* tok,
+                           const int* active, const int* params, const float* penalties, const int* bias_ids,
+                           const float* bias_vals, int bias_cap, int* hist, int* hist_len, int hist_cap, int top_k,
+                           int* top_ids, float* top_lp, void* stream);
 /* device bf16 [B][round8(vocab)] of the last step; columns >= vocab hold -inf */
 const void* b200_batch_logits(b200_engine* e);
 const void* b200_batch_logprobs(b200_engine* e); /* same layout (want_logprobs) */

@@ -97,6 +97,9 @@ SIGNATURES = {
     "b200_batch_begin": (_I, [_P, _I, _P, _P, _P, _P, _P]),
     "b200_batch_decode": (_I, [_P, _I, _I, _P]),
     "b200_batch_fetch": (_I, [_P, _L, _I, _P, _P, _P]),
+    "b200_batch_set_procs": (_I, [_P, _P, _P, _P, _P, _I, _P, _P, _I, _I]),
+    "b200_batch_fetch_topk": (_I, [_P, _L, _I, _P, _P, _P]),
+    "b200_batch_procs_apply": (_I, [_P, _P, _I, _I, _I] + [_P] * 6 + [_I, _P, _P, _I, _I, _P, _P, _P]),
     "b200_batch_logits": (_P, [_P]),
     "b200_batch_logprobs": (_P, [_P]),
     "b200_batch_token_log": (_P, [_P]),

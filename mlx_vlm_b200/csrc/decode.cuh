@@ -101,6 +101,35 @@ int batch_decoder_begin(void** handle, const BdModel& m, int B, const int* tok, 
 int batch_decoder_step(void* handle, const BdModel& m, int n_steps, bool want_logprobs, cudaStream_t s,
                        cudaStream_t cap_stream, long* launches);
 int batch_decoder_fetch(void* handle, long first_step, int n_steps, int* tok_host, float* lp_host, cudaStream_t s);
+
+// Per-row logits processors and top-k logprobs of the lock-step batch (b200_batch_set_procs).  Device arrays owned
+// by the caller, row b at b * stride:
+//   params    int32 [rows][BD_PROC_PARAMS]: flags (BD_PROC_*; 0 = none), repetition / presence / frequency context
+//             sizes, number of bias entries
+//   penalties fp32  [rows][BD_PROC_PARAMS]: repetition penalty, fp32(1 / repetition penalty), presence, frequency
+//   bias_ids / bias_vals  [rows][bias_cap]: token ids and bf16-exact values of logit_bias
+//   hist [rows][hist_cap] ring of each row's token history, hist_len [rows] tokens appended so far
+constexpr int BD_PROC_PARAMS = 8, BD_HIST_MAX = 1024, BD_TOPK_MAX = 20;
+constexpr int BD_TOPK_SLICE = 8192, BD_TOPK_CAND_MAX = 1024;
+constexpr int BD_PROC_BIAS = 1, BD_PROC_REP = 2, BD_PROC_PRES = 4, BD_PROC_FREQ = 8;
+struct BdProcs {
+  const int* params;      // nullptr: no row has processors (no launch)
+  const float* penalties;
+  const int* bias_ids;
+  const float* bias_vals;
+  int bias_cap;
+  int* hist;
+  int* hist_len;
+  int hist_cap;
+  int top_k;              // 0 .. BD_TOPK_MAX (0: none)
+};
+// replaces the processors until the next batch_decoder_begin (which turns them off)
+int batch_decoder_set_procs(void* handle, const BdProcs& pr, int vocab);
+// top-k ids / logprobs of steps [first, first + n): host arrays [n][B][BD_TOPK_MAX]
+int batch_decoder_fetch_topk(void* handle, long first_step, int n_steps, int* ids_host, float* lp_host, cudaStream_t s);
+// the processors and the top-k of one step on caller buffers (b200_batch_procs_apply)
+int batch_procs_apply(bf16* logits, const bf16* logprobs, int B, int V, int ldv, const int* tok, const int* active,
+                      const BdProcs& pr, int* top_ids, float* top_lp, cudaStream_t s);
 const void* batch_decoder_buffer(void* handle, int which);
 void batch_decoder_destroy(void* handle);
 

@@ -586,6 +586,147 @@ __global__ void __launch_bounds__(1024) bd_sample_kernel(const BdSampleP p) {
   bd_embed_norm_row(p.embed, s_tok, p.H, p.ln0, p.eps, p.h + (long)b * p.H, p.xn + (long)b * p.H, red);
 }
 
+// ---- per-row logits processors (sample_utils.make_logits_processors), one CTA per row -------------------------------
+// Runs between the head and bd_sample, in place on the step's bf16 logits, only when some row has processors.  First
+// the step's input token joins the row's history (ar.py:1070-1074), then in the order make_logits_processors returns
+// them: logit bias, repetition, presence, frequency.  Each is a gather of the current values, then a scatter; a
+// token that occurs several times in a window writes the same value several times (penalised once).  Rounding
+// points are those of the torch ops: bias bf16(x + v); repetition bf16(x * p) for x < 0 else bf16(x * fp32(1 / p))
+// (the reciprocal of a division by a scalar); presence bf16(x - p); frequency bf16(x - sum) with sum the fp32
+// accumulation of p once per occurrence.
+struct BdProcsP {
+  bf16* logits;
+  int ldv, V;   // ids outside [0, V) in a history or a bias list are skipped
+  const int *tok, *active;
+  BdProcs pr;
+};
+
+__global__ void __launch_bounds__(1024) bd_procs_kernel(const BdProcsP p) {
+  __shared__ int win[BD_HIST_MAX];
+  const int b = blockIdx.x, t = threadIdx.x;
+  bd_pdl_wait();
+  const int* par = p.pr.params + b * BD_PROC_PARAMS;
+  const int flags = par[0];
+  if (flags == 0) return;
+  const float* pen = p.pr.penalties + b * BD_PROC_PARAMS;
+  bf16* lg = p.logits + (long)b * p.ldv;
+  int* hist = p.pr.hist + (long)b * p.pr.hist_cap;
+  const int cap = p.pr.hist_cap;
+  int len = p.pr.hist_len[b];
+  if (p.active[b]) {
+    if (t == 0) {
+      hist[len % cap] = p.tok[b];
+      p.pr.hist_len[b] = len + 1;
+    }
+    len += 1;
+  }
+  __syncthreads();
+  // the last W tokens of the history (W = the widest window in use), oldest first
+  int W = 0;
+  if (flags & BD_PROC_REP) W = max(W, par[1]);
+  if (flags & BD_PROC_PRES) W = max(W, par[2]);
+  if (flags & BD_PROC_FREQ) W = max(W, par[3]);
+  W = min(W, min(len, cap));
+  if (t < W) {
+    const int id = hist[(len - W + t) % cap];
+    win[t] = (id >= 0 && id < p.V) ? id : -1;
+  }
+  if (flags & BD_PROC_BIAS) {
+    const int nb = par[4];
+    const int* ids = p.pr.bias_ids + (long)b * p.pr.bias_cap;
+    const float* vals = p.pr.bias_vals + (long)b * p.pr.bias_cap;
+    for (int i = t; i < nb; i += blockDim.x)
+      if (ids[i] >= 0 && ids[i] < p.V) lg[ids[i]] = f2bf(bf2f(lg[ids[i]]) + vals[i]);
+  }
+  __syncthreads();
+  if (flags & BD_PROC_REP) {
+    const int w0 = W - min(par[1], W);
+    const int id = (t >= w0 && t < W) ? win[t] : -1;
+    const float x = id >= 0 ? bf2f(lg[id]) : 0.f;
+    __syncthreads();
+    if (id >= 0) lg[id] = f2bf(x < 0.f ? x * pen[0] : x * pen[1]);
+    __syncthreads();
+  }
+  if (flags & BD_PROC_PRES) {
+    const int w0 = W - min(par[2], W);
+    const int id = (t >= w0 && t < W) ? win[t] : -1;
+    const float x = id >= 0 ? bf2f(lg[id]) : 0.f;
+    __syncthreads();
+    if (id >= 0) lg[id] = f2bf(x - pen[2]);
+    __syncthreads();
+  }
+  if (flags & BD_PROC_FREQ) {
+    const int w0 = W - min(par[3], W);
+    const int id = (t >= w0 && t < W) ? win[t] : -1;
+    float x = 0.f, sub = 0.f;
+    if (id >= 0) {
+      x = bf2f(lg[id]);
+      for (int j = w0; j < W; ++j)
+        if (win[j] == id) sub += pen[3];
+    }
+    __syncthreads();
+    if (id >= 0) lg[id] = f2bf(x - sub);
+  }
+}
+
+// ---- top-k logprobs: lower token id first among equal logprobs ------------------------------------------------------
+// Keys (orderable logprob << 32 | ~id) are unique per token, so "largest key" is the order asked for.  Part kernel: one
+// CTA per (slice of BD_TOPK_SLICE tokens, row) picks its k largest keys in k rounds over shared memory; merge kernel:
+// one CTA per row ranks the slices' candidates.
+__global__ void __launch_bounds__(256) bd_topk_part_kernel(const bf16* __restrict__ lp, int ldv, int V, int k,
+                                                           unsigned long long* __restrict__ cand) {
+  __shared__ uint32_t key[BD_TOPK_SLICE];
+  __shared__ unsigned long long red[8];
+  const int s = blockIdx.x, b = blockIdx.y, S = gridDim.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  bd_pdl_wait();
+  const int base = s * BD_TOPK_SLICE, n = min(BD_TOPK_SLICE, V - base);
+  for (int i = threadIdx.x; i < n; i += 256) key[i] = bd_orderable(bf2f(lp[(long)b * ldv + base + i]));
+  __syncthreads();
+  unsigned long long prev = ~0ull;
+  for (int r = 0; r < k; ++r) {
+    unsigned long long best = 0ull;
+    for (int i = threadIdx.x; i < n; i += 256) {
+      const unsigned long long kk = ((unsigned long long)key[i] << 32) | (0xFFFFFFFFu - (uint32_t)(base + i));
+      if (kk < prev && kk > best) best = kk;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+      best = other > best ? other : best;
+    }
+    if (lane == 0) red[warp] = best;
+    __syncthreads();
+    best = 0ull;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) best = red[w] > best ? red[w] : best;
+    __syncthreads();
+    if (threadIdx.x == 0) cand[((long)b * S + s) * k + r] = best;
+    prev = best;
+  }
+}
+
+__global__ void __launch_bounds__(256) bd_topk_merge_kernel(const unsigned long long* __restrict__ cand, int S, int k,
+                                                            const int* __restrict__ n_out, int log_cap, int max_b,
+                                                            int* __restrict__ ids_log, float* __restrict__ lp_log) {
+  __shared__ unsigned long long c[BD_TOPK_CAND_MAX];
+  const int b = blockIdx.x, n = S * k;
+  bd_pdl_wait();
+  for (int i = threadIdx.x; i < n; i += 256) c[i] = cand[(long)b * n + i];
+  __syncthreads();
+  const long at = ((long)(n_out ? (n_out[b] - 1) % log_cap : 0) * max_b + b) * BD_TOPK_MAX;   // no log: [B][20]
+  for (int i = threadIdx.x; i < n; i += 256) {
+    const unsigned long long kk = c[i];
+    int rank = 0;
+    for (int j = 0; j < n; ++j) rank += c[j] > kk;
+    if (rank < k) {
+      const uint32_t ob = (uint32_t)(kk >> 32);
+      ids_log[at + rank] = (int)(0xFFFFFFFFu - (uint32_t)(kk & 0xFFFFFFFFull));
+      lp_log[at + rank] = __uint_as_float((ob & 0x80000000u) ? (ob & 0x7FFFFFFFu) : ~ob);
+    }
+  }
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
@@ -610,14 +751,24 @@ struct BatchDecoder {
   int graph_B = 0, graph_cap = 0, graph_lp = 0;
   long steps_done = 0;
   bool want_logprobs = false;
+  BdProcs procs = {}, graph_procs = {};
+  unsigned long long* topk_cand = nullptr;  // [max_b][slices][k] keys of the top-k part kernel
+  int* topk_ids = nullptr;                  // [log_cap][max_b][BD_TOPK_MAX]
+  float* topk_lp = nullptr;
 };
+
+static bool bd_same_procs(const BdProcs& a, const BdProcs& b) {
+  return a.params == b.params && a.penalties == b.penalties && a.bias_ids == b.bias_ids &&
+         a.bias_vals == b.bias_vals && a.bias_cap == b.bias_cap && a.hist == b.hist && a.hist_len == b.hist_len &&
+         a.hist_cap == b.hist_cap && a.top_k == b.top_k;
+}
 
 static void bd_free(BatchDecoder* d) {
   if (!d) return;
   if (d->gexec) cudaGraphExecDestroy(d->gexec);
   for (void* p : {(void*)d->tok, (void*)d->ctx, (void*)d->pos, (void*)d->active, (void*)d->n_out, (void*)d->token_log,
                   (void*)d->lp_log, (void*)d->h, (void*)d->xn, (void*)d->att, (void*)d->act, (void*)d->logits,
-                  (void*)d->logprobs, (void*)d->partial})
+                  (void*)d->logprobs, (void*)d->partial, (void*)d->topk_cand, (void*)d->topk_ids, (void*)d->topk_lp})
     if (p) cudaFree(p);
   if (d->stage_host) cudaFreeHost(d->stage_host);
   delete d;
@@ -758,6 +909,12 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
   if ((rc = gemm_wt_tuned(d->xn, H, m.head, nullptr, nullptr, 0, d->logits, d->ldv, nullptr, 0, B, dd.vocab, H,
                           B200_EPI_NONE, B200_WT_BF16, 0, false, m.sm_count, nullptr, s)))
     return rc;
+  if (d->procs.params) {
+    BdProcsP pp;
+    pp.logits = d->logits; pp.ldv = d->ldv; pp.V = dd.vocab; pp.tok = d->tok; pp.active = d->active; pp.pr = d->procs;
+    if ((rc = bd_launch(bd_procs_kernel, dim3(B), dim3(1024), 0, s, pp))) return rc;
+    *launches += 1;
+  }
   BdSampleP sp;
   sp.logits = d->logits; sp.logprobs = d->want_logprobs ? d->logprobs : nullptr; sp.V = dd.vocab; sp.ldv = d->ldv; sp.H = H;
   sp.tok = d->tok; sp.ctx = d->ctx; sp.pos = d->pos; sp.n_out = d->n_out; sp.active = d->active;
@@ -765,6 +922,16 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
   sp.embed = m.embed; sp.ln0 = m.layers[0].ln1; sp.eps = dd.eps; sp.h = d->h; sp.xn = d->xn;
   if ((rc = bd_launch(bd_sample_kernel, dim3(B), dim3(1024), 0, s, sp))) return rc;
   *launches += 2;
+  if (d->procs.top_k > 0) {  // over the logprob rows bd_sample wrote (want_logprobs is forced on)
+    const int S = (dd.vocab + BD_TOPK_SLICE - 1) / BD_TOPK_SLICE, k = d->procs.top_k;
+    if ((rc = bd_launch(bd_topk_part_kernel, dim3(S, B), dim3(256), 0, s, (const bf16*)d->logprobs, d->ldv, dd.vocab,
+                        k, d->topk_cand)))
+      return rc;
+    if ((rc = bd_launch(bd_topk_merge_kernel, dim3(B), dim3(256), 0, s, (const unsigned long long*)d->topk_cand, S, k,
+                        (const int*)d->n_out, d->log_cap, d->max_b, d->topk_ids, d->topk_lp)))
+      return rc;
+    *launches += 2;
+  }
   return B200_OK;
 }
 
@@ -786,6 +953,7 @@ int batch_decoder_begin(void** handle, const BdModel& m, int B, const int* tok, 
     if ((rc = bd_set_smem_attrs())) return rc;
   }
   d->B = B;
+  d->procs = BdProcs{};
   for (int b = 0; b < B; ++b) {
     B200_REQUIRE(ctx[b] >= 0 && ctx[b] < m.d.cap, "batch decode: row %d holds %d tokens, capacity %d", b, ctx[b], m.d.cap);
     d->stage_host[b] = tok[b];
@@ -810,12 +978,14 @@ int batch_decoder_step(void* handle, const BdModel& m, int n_steps, bool want_lo
   BatchDecoder* d = reinterpret_cast<BatchDecoder*>(handle);
   B200_REQUIRE(d && d->B > 0 && n_steps > 0, "batch decode: begin() first");
   B200_REQUIRE(d->steps_done + n_steps <= d->log_cap, "batch decode: fetch the tokens before step %d", d->log_cap);
+  want_logprobs = want_logprobs || d->procs.top_k > 0;
   d->want_logprobs = want_logprobs;
   int rc;
   int done = 0;
   const bool stale = !d->gexec || d->graph_kv != m.kv || d->graph_B != d->B || d->graph_cap != m.d.cap ||
                      d->graph_lp != (int)want_logprobs || d->graph_q8 != m.q8_codes ||
-                     d->graph_q8_layers != m.q8_layers || d->graph_gs != m.q8_gs;
+                     d->graph_q8_layers != m.q8_layers || d->graph_gs != m.q8_gs ||
+                     !bd_same_procs(d->graph_procs, d->procs);
   if (stale) {
     if (d->gexec) {
       cudaGraphExecDestroy(d->gexec);
@@ -840,10 +1010,12 @@ int batch_decoder_step(void* handle, const BdModel& m, int n_steps, bool want_lo
       if (ce != cudaSuccess) return cuda_fail(ce, "cudaGraphInstantiate(batch step)", __FILE__, __LINE__);
       d->graph_kv = m.kv; d->graph_B = d->B; d->graph_cap = m.d.cap; d->graph_lp = (int)want_logprobs;
       d->graph_q8 = m.q8_codes; d->graph_q8_layers = m.q8_layers; d->graph_gs = m.q8_gs;
+      d->graph_procs = d->procs;
     }
   }
   for (int i = done; i < n_steps; ++i) B200_CUDA(cudaGraphLaunch(d->gexec, s));
-  *launches += (long)(n_steps - done) * (m.n_layers * 7 + 2);
+  *launches += (long)(n_steps - done) *
+               (m.n_layers * 7 + 2 + (d->procs.params ? 1 : 0) + (d->procs.top_k > 0 ? 2 : 0));
   d->steps_done += n_steps;
   return B200_OK;
 }
@@ -857,6 +1029,63 @@ int batch_decoder_fetch(void* handle, long first_step, int n_steps, int* tok_hos
   if (lp_host)
     B200_CUDA(cudaMemcpy2DAsync(lp_host, (size_t)d->B * 4, d->lp_log + first_step * d->max_b, (size_t)d->max_b * 4,
                                 (size_t)d->B * 4, n_steps, cudaMemcpyDeviceToHost, s));
+  return B200_OK;
+}
+
+int batch_decoder_set_procs(void* handle, const BdProcs& pr, int vocab) {
+  BatchDecoder* d = reinterpret_cast<BatchDecoder*>(handle);
+  B200_REQUIRE(d && d->B > 0, "batch procs: begin() first");
+  B200_REQUIRE(pr.top_k >= 0 && pr.top_k <= BD_TOPK_MAX, "batch procs: top_k %d (0..%d)", pr.top_k, BD_TOPK_MAX);
+  B200_REQUIRE(!pr.params || (pr.penalties && pr.hist && pr.hist_len && pr.hist_cap >= 1 && pr.hist_cap <= BD_HIST_MAX &&
+                              (pr.bias_cap == 0 || (pr.bias_ids && pr.bias_vals && pr.bias_cap > 0))),
+               "batch procs: bad arguments (history capacity 1..%d)", BD_HIST_MAX);
+  const int S = (vocab + BD_TOPK_SLICE - 1) / BD_TOPK_SLICE;
+  B200_REQUIRE(pr.top_k == 0 || S * pr.top_k <= BD_TOPK_CAND_MAX, "batch procs: vocabulary %d too large for top-k", vocab);
+  if (pr.top_k > 0 && !d->topk_ids) {
+    B200_CUDA(cudaMalloc(&d->topk_cand, (size_t)d->max_b * BD_TOPK_CAND_MAX * 8));
+    B200_CUDA(cudaMalloc(&d->topk_ids, (size_t)d->log_cap * d->max_b * BD_TOPK_MAX * 4));
+    B200_CUDA(cudaMalloc(&d->topk_lp, (size_t)d->log_cap * d->max_b * BD_TOPK_MAX * 4));
+  }
+  d->procs = pr;
+  return B200_OK;
+}
+
+int batch_decoder_fetch_topk(void* handle, long first_step, int n_steps, int* ids_host, float* lp_host, cudaStream_t s) {
+  BatchDecoder* d = reinterpret_cast<BatchDecoder*>(handle);
+  B200_REQUIRE(d && d->topk_ids && first_step >= 0 && n_steps > 0 && first_step + n_steps <= d->log_cap,
+               "batch fetch top-k: bad range, or top-k never enabled");
+  const size_t w = (size_t)BD_TOPK_MAX * 4;
+  B200_CUDA(cudaMemcpy2DAsync(ids_host, d->B * w, d->topk_ids + first_step * d->max_b * BD_TOPK_MAX, d->max_b * w,
+                              d->B * w, n_steps, cudaMemcpyDeviceToHost, s));
+  B200_CUDA(cudaMemcpy2DAsync(lp_host, d->B * w, d->topk_lp + first_step * d->max_b * BD_TOPK_MAX, d->max_b * w,
+                              d->B * w, n_steps, cudaMemcpyDeviceToHost, s));
+  return B200_OK;
+}
+
+int batch_procs_apply(bf16* logits, const bf16* logprobs, int B, int V, int ldv, const int* tok, const int* active,
+                      const BdProcs& pr, int* top_ids, float* top_lp, cudaStream_t s) {
+  B200_REQUIRE(B >= 1 && B <= 16 && V > 0 && ldv >= V, "batch procs apply: bad arguments");
+  B200_REQUIRE(pr.top_k >= 0 && pr.top_k <= BD_TOPK_MAX, "batch procs apply: top_k %d", pr.top_k);
+  int rc;
+  if (pr.params) {
+    B200_REQUIRE(logits && tok && active && pr.penalties && pr.hist && pr.hist_len && pr.hist_cap >= 1 &&
+                 pr.hist_cap <= BD_HIST_MAX, "batch procs apply: bad processor arguments");
+    BdProcsP pp;
+    pp.logits = logits; pp.ldv = ldv; pp.V = V; pp.tok = tok; pp.active = active; pp.pr = pr;
+    if ((rc = bd_launch(bd_procs_kernel, dim3(B), dim3(1024), 0, s, pp))) return rc;
+  }
+  if (pr.top_k > 0) {
+    const int S = (V + BD_TOPK_SLICE - 1) / BD_TOPK_SLICE;
+    B200_REQUIRE(logprobs && top_ids && top_lp && S * pr.top_k <= BD_TOPK_CAND_MAX, "batch procs apply: bad top-k arguments");
+    unsigned long long* cand = nullptr;
+    B200_CUDA(cudaMallocAsync(&cand, (size_t)B * S * pr.top_k * 8, s));
+    rc = bd_launch(bd_topk_part_kernel, dim3(S, B), dim3(256), 0, s, logprobs, ldv, V, pr.top_k, cand);
+    if (!rc)
+      rc = bd_launch(bd_topk_merge_kernel, dim3(B), dim3(256), 0, s, (const unsigned long long*)cand, S, pr.top_k,
+                     (const int*)nullptr, 1, B, top_ids, top_lp);
+    B200_CUDA(cudaFreeAsync(cand, s));
+    if (rc) return rc;
+  }
   return B200_OK;
 }
 

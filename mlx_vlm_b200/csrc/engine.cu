@@ -1429,6 +1429,31 @@ int b200_batch_fetch(b200_engine* e, long first_step, int n_steps, int* tok_host
   return batch_decoder_fetch(e->batch, first_step, n_steps, tok_host, lp_host, (cudaStream_t)stream);
 }
 
+int b200_batch_set_procs(b200_engine* e, const int* params, const float* penalties, const int* bias_ids,
+                         const float* bias_vals, int bias_cap, int* hist, int* hist_len, int hist_cap, int top_k) {
+  B200_REQUIRE(e && e->batch, "batch_set_procs: batch_begin first");
+  BdProcs pr;
+  pr.params = params; pr.penalties = penalties; pr.bias_ids = bias_ids; pr.bias_vals = bias_vals;
+  pr.bias_cap = bias_cap; pr.hist = hist; pr.hist_len = hist_len; pr.hist_cap = hist_cap; pr.top_k = top_k;
+  return batch_decoder_set_procs(e->batch, pr, e->cfg.vocab);
+}
+
+int b200_batch_fetch_topk(b200_engine* e, long first_step, int n_steps, int* ids_host, float* lp_host, void* stream) {
+  B200_REQUIRE(e && e->batch && ids_host && lp_host, "batch_fetch_topk: batch_begin first");
+  return batch_decoder_fetch_topk(e->batch, first_step, n_steps, ids_host, lp_host, (cudaStream_t)stream);
+}
+
+int b200_batch_procs_apply(void* logits, const void* logprobs, int B, int vocab, int ldv, const int* tok,
+                           const int* active, const int* params, const float* penalties, const int* bias_ids,
+                           const float* bias_vals, int bias_cap, int* hist, int* hist_len, int hist_cap, int top_k,
+                           int* top_ids, float* top_lp, void* stream) {
+  BdProcs pr;
+  pr.params = params; pr.penalties = penalties; pr.bias_ids = bias_ids; pr.bias_vals = bias_vals;
+  pr.bias_cap = bias_cap; pr.hist = hist; pr.hist_len = hist_len; pr.hist_cap = hist_cap; pr.top_k = top_k;
+  return batch_procs_apply((bf16*)logits, (const bf16*)logprobs, B, vocab, ldv, tok, active, pr, top_ids, top_lp,
+                           (cudaStream_t)stream);
+}
+
 const void* b200_batch_logits(b200_engine* e) { return e ? batch_decoder_buffer(e->batch, 0) : nullptr; }
 const void* b200_batch_logprobs(b200_engine* e) { return e ? batch_decoder_buffer(e->batch, 1) : nullptr; }
 /* device int32 [4096 steps][16 rows]: token of (step since the last begin, row) */

@@ -201,6 +201,20 @@ class Engine:
         N.check(self.lib.b200_batch_fetch(self.h, int(first_step), int(n_steps), tok_host.data_ptr(),
                                           N.ptr(lp_host), self.s), "batch_fetch")
 
+    def batch_set_procs(self, state=None, top_k: int = 0):
+        """the armed rows' logits processors (`models/cache.py::BatchProcState`, None: none) and top-k logprobs
+        (0: none) until the next batch_begin"""
+        st = state
+        N.check(self.lib.b200_batch_set_procs(
+            self.h, N.ptr(st and st.params), N.ptr(st and st.penalties), N.ptr(st and st.bias_ids),
+            N.ptr(st and st.bias_vals), st.BIAS_CAP if st else 0, N.ptr(st and st.hist), N.ptr(st and st.hist_len),
+            st.HIST_CAP if st else 0, int(top_k)), "batch_set_procs")
+
+    def batch_fetch_topk(self, first_step: int, n_steps: int, ids_host: torch.Tensor, lp_host: torch.Tensor):
+        """async copy of the top-k ids / logprobs of steps [first, first+n) into pinned (n, B, 20) buffers"""
+        N.check(self.lib.b200_batch_fetch_topk(self.h, int(first_step), int(n_steps), ids_host.data_ptr(),
+                                               lp_host.data_ptr(), self.s), "batch_fetch_topk")
+
     def batch_logits_view(self, which: str = "logits") -> torch.Tensor:
         p = (self.lib.b200_batch_logits if which == "logits" else self.lib.b200_batch_logprobs)(self.h)
         ldv = (self.cfg.vocab + 7) // 8 * 8      # rows are padded to 16-byte multiples (tail = -inf)

@@ -29,10 +29,12 @@ import numpy as np
 import torch
 
 from .models import cache as cache_mod
+from .sample_utils import greedy_sampler, lower_logits_processors, top_logprobs
 
 DEFAULT_MAX_TOKENS = 256
 DEFAULT_COMPLETION_BATCH_SIZE = 32
 DEFAULT_PREFILL_BATCH_SIZE = 8
+TOP_LOGPROBS_MAX = 20   # the reference server's cap (server/generation.py get_top_logprobs_k) and the kernel's
 
 
 def _host_buf(n: int) -> torch.Tensor:
@@ -106,8 +108,11 @@ class _Row:
     n_tokens: int = 0          # tokens surfaced so far
     n_decoded: int = 0         # tokens computed so far (>= n_tokens: the slice buffer)
     last_token: int = -1       # last computed token (input of the next decode step)
-    buffer: List[Tuple[int, float]] = field(default_factory=list)
+    buffer: List[Tuple[int, float, Optional[list]]] = field(default_factory=list)   # (token, logprob, top-k)
     reserve: int = 0
+    procs: Optional[list] = None     # the row's logits processors (None: none)
+    lowered: Optional[dict] = None   # their device form (lock-step rows; None: torch ops on the host)
+    context: Optional[List[int]] = None   # the reference's token context of a row with processors
 
 
 class GenerationBatch:
@@ -152,6 +157,36 @@ class GenerationBatch:
             return None
         return np.asarray([[r.delta] for r in self.rows], dtype=np.int32)
 
+    # The reference keeps `logits_processors` / `token_context` as lists aligned with the rows (ar.py:995-1013):
+    # a batch that had processors when it was formed or extended tracks a context for EVERY row (the prompt when the
+    # row was admitted with processors in its group, else []), appended while any row has processors; a batch that
+    # never had any tracks none.  Here a row's `context` is None when it is not tracked.
+    @property
+    def logits_processors(self) -> list:
+        """one processor list (or None) per row; [] when the batch tracks no processors"""
+        return [r.procs for r in self.rows] if any(r.context is not None for r in self.rows) else []
+
+    @property
+    def token_context(self) -> List[List[int]]:
+        return [list(r.context) for r in self.rows] if any(r.context is not None for r in self.rows) else []
+
+    @staticmethod
+    def admitted(rows: List[_Row]) -> "GenerationBatch":
+        """rows admitted together (a prefill batch): each is seeded with its prompt when any of them has processors
+        (ar.py:1663-1667)"""
+        track = any(r.procs for r in rows)
+        for r in rows:
+            r.context = list(r.ids) if track else None
+        return GenerationBatch(rows)
+
+    def record_inputs(self, inputs: List[Tuple[_Row, List[int]]]):
+        """the input tokens of the step(s) about to run join every tracked row's context while any row has
+        processors (ar.py:1070-1074)"""
+        if any(r.procs for r in self.rows):
+            for r, toks in inputs:
+                if r.context is not None:
+                    r.context.extend(toks)
+
     def filter(self, keep: List[int]) -> None:
         self.rows = [self.rows[i] for i in keep]
 
@@ -159,6 +194,9 @@ class GenerationBatch:
         if self.rows and other.rows and (self.rows[0].delta is None) != (other.rows[0].delta is None):
             raise RuntimeError("extend() mixes MRoPE and non-MRoPE batches; both sides must carry "
                                "rope_deltas or neither side may.")
+        track = any(r.procs for r in self.rows + other.rows)   # ar.py:1181-1202
+        for r in self.rows + other.rows:
+            r.context = (r.context if r.context is not None else []) if track else None
         self.rows.extend(other.rows)
 
 
@@ -187,10 +225,10 @@ class BatchGenerator:
         self.kv_bits = kv_quant_args(kv_bits, kv_group_size, kv_quant_scheme,
                                      getattr(getattr(model, "language_model", None), "head_dim", None) or 128)
         self.kv_group_size = int(kv_group_size)
-        if logits_processors:
-            raise NotImplementedError("BatchGenerator: logits processors run on the single-request path only")
-        if top_logprobs_k:
-            raise NotImplementedError("BatchGenerator: top_logprobs_k > 0 is not supported")
+        if not 0 <= int(top_logprobs_k) <= TOP_LOGPROBS_MAX:
+            raise ValueError(f"BatchGenerator: top_logprobs_k must lie in [0, {TOP_LOGPROBS_MAX}]")
+        self.top_logprobs_k = int(top_logprobs_k)
+        self.logits_processors = list(logits_processors) if logits_processors else None   # default of every row
         self.model, self.processor = model, processor
         self.max_tokens = max_tokens
         self.sampler = sampler
@@ -232,21 +270,44 @@ class BatchGenerator:
 
     # ------------------------------------------------------------------ queueing
     def insert(self, prompts, max_tokens: Union[List[int], int, None] = None,
-               prompt_kwargs: Optional[List[dict]] = None) -> List[int]:
+               prompt_kwargs: Optional[List[dict]] = None, logits_processors=None) -> List[int]:
+        """`logits_processors`: one processor list (or None) per prompt; None gives every prompt the generator's
+        own list (ar.py:2584-2604)"""
         if max_tokens is None or isinstance(max_tokens, int):
             max_tokens = [max_tokens or self.max_tokens] * len(prompts)
         if prompt_kwargs is None:
             prompt_kwargs = [{} for _ in prompts]
+        if logits_processors is None:
+            logits_processors = [self.logits_processors] * len(prompts)
+        elif len(logits_processors) != len(prompts):
+            raise ValueError("Insufficient number of logits_processors provided")
         if len(max_tokens) != len(prompts) or len(prompt_kwargs) != len(prompts):
             raise ValueError("insert: max_tokens / prompt_kwargs must match the number of prompts")
         uids = []
-        for p, m, kw in zip(prompts, max_tokens, prompt_kwargs):
+        for p, m, kw, procs in zip(prompts, max_tokens, prompt_kwargs, logits_processors):
             ids = np.asarray(p.cpu() if isinstance(p, torch.Tensor) else p).reshape(-1).tolist()
-            self._unprocessed_sequences.append(_Row(self.uid_count, ids, int(m), dict(kw or {})))
+            row = _Row(self.uid_count, ids, int(m), dict(kw or {}), procs=list(procs) if procs else None)
+            self._check_bias(row.procs)
+            if row.procs:
+                lowered = lower_logits_processors(row.procs)
+                row.lowered = lowered if lowered is not None and cache_mod.BatchProcState.fits(lowered) else None
+            self._unprocessed_sequences.append(row)
             uids.append(self.uid_count)
             self.uid_count += 1
         self._unprocessed_sequences.sort(key=lambda r: len(r.ids))  # shortest first (ar.py:2620-2623)
         return uids
+
+    def _check_bias(self, procs):
+        """a logit bias must name tokens of the vocabulary: refused here, so only the request that brings it fails"""
+        lm = getattr(self.model, "language_model", None)
+        vocab = getattr(getattr(lm, "args", None), "vocab_size", None)
+        for p in procs or []:
+            spec = getattr(p, "lowered", None)
+            if isinstance(spec, tuple) and spec[0] == "bias":
+                bad = [i for i in spec[1] if not (isinstance(i, (int, np.integer)) and i >= 0
+                                                  and (vocab is None or i < vocab))]
+                if bad:
+                    raise ValueError(f"logit_bias: token ids {bad} outside the vocabulary [0, {vocab})")
 
     @property
     def _active(self) -> List[_Row]:
@@ -359,18 +420,20 @@ class BatchGenerator:
             emb, ids_left = emb[:, step:], ids_left[:, step:]
         out = lm(ids_left, inputs_embeds=emb, cache=cache, position_ids=pos, rope_deltas=deltas,
                  logits_to_keep=1, reserve_tokens=row.reserve)
-        if self.greedy_sampling:
+        row.context = list(row.ids) if row.procs else None   # seeded with the prompt (ar.py:1663-1667)
+        top = None
+        if self.greedy_sampling and not row.procs and not self.top_logprobs_k:
             host = _host_buf(1)
             eng.fetch_tokens(eng.tokens_launched - 1, 1, host)
             eng.stream.synchronize()
             tok = int(host[0])
             lp = self._logprob_of(tok) if self.compute_logprobs else 0.0
-        else:
-            tok, lp = self._sample(out.logits[:, -1, :])
+        else:   # the row's processors as torch ops over its prompt, as the single-request path runs them
+            tok, lp, top = self._sample(out.logits[:, -1, :], row, row.procs)
         row.last_token, row.n_decoded = tok, 1
-        row.buffer.append((tok, lp))
+        row.buffer.append((tok, lp, top))
         if self._lockstep:
-            rows.admit(int(cache[0].offset))
+            rows.admit(int(cache[0].offset), row.lowered, row.context)
             if self.kv_bits is not None:
                 rows.pool.end_admission()
         dt = time.perf_counter() - tic
@@ -395,21 +458,26 @@ class BatchGenerator:
         for row, tok, cache in zip(rows, toks, caches):
             row.last_token, row.n_decoded = tok, 1
             pool_rows.admit(int(cache[0].offset))
-            row.buffer.append((tok, 0.0))
+            row.buffer.append((tok, 0.0, None))
             self._prompt_tokens_counter += len(row.ids)
             out.append(PromptProgress(uid=row.uid, prompt_tokens=len(row.ids), prompt_time=dt / len(rows),
                                       prompt_tps=len(row.ids) * len(rows) / dt if dt > 0 else 0.0))
         self._prompt_time_counter += dt
         return out
 
-    def _sample(self, logits: torch.Tensor) -> Tuple[int, float]:
+    def _sample(self, logits: torch.Tensor, row: Optional[_Row] = None, procs=None,
+                want_top: bool = True) -> Tuple[int, float, Optional[list]]:
+        """`procs` (torch ops over the row's token context), logprobs, the sampler and the top-k of one row"""
         # torch ops on the engine's stream: ordered after the step that wrote `logits`
         with torch.cuda.stream(self.model.engine.stream):
+            for p in procs or []:
+                logits = p(row.context, logits)
             lf = logits.float()
             logprobs = logits - torch.logsumexp(lf, dim=-1, keepdim=True).to(logits.dtype)
-            y = self.sampler(logprobs)
+            y = (greedy_sampler if self.greedy_sampling or self.sampler is None else self.sampler)(logprobs)
             tok = int(y.reshape(-1)[0].item())
-            return tok, float(logprobs.reshape(-1)[tok].float().item())
+            top = top_logprobs(logprobs, self.top_logprobs_k) if self.top_logprobs_k and want_top else None
+            return tok, float(logprobs.reshape(-1)[tok].float().item()), top
 
     # ------------------------------------------------------------------ lock-step rows
     def _lockstep_slice(self):
@@ -419,36 +487,52 @@ class BatchGenerator:
         live = [r.n_decoded < r.max_tokens for r in active]
         if not any(live):
             return
-        k = min([self.decode_slice] + [r.max_tokens - r.n_decoded for r, a in zip(active, live) if a])
-        greedy = self.greedy_sampling
-        if not greedy:
-            k = 1
+        # rows whose processors do not lower run them as torch ops on their logits row, one step at a time
+        host = [a and r.procs is not None and r.lowered is None for r, a in zip(active, live)]
+        greedy = self.greedy_sampling and not any(host)
+        k = min([self.decode_slice] + [r.max_tokens - r.n_decoded for r, a in zip(active, live) if a]) if greedy else 1
         # greedy: the device feeds each step's tokens to the next; otherwise the host's sampled tokens are uploaded
+        rows.top_k = self.top_logprobs_k
         rows.arm(k, [r.last_token for r in active], [r.delta or 0 for r in active], live, fed_back=greedy)
         first = rows.steps
-        eng.batch_decode(k, want_logprobs=not greedy)
+        eng.batch_decode(k, want_logprobs=not self.greedy_sampling)
         rows.advance(k, live)
         B = len(active)
-        if greedy:
+        top_ids = top_lp = None
+        if self.top_logprobs_k:
+            top_ids = _host_buf(k * B * TOP_LOGPROBS_MAX).view(k, B, TOP_LOGPROBS_MAX)
+            top_lp = torch.empty(k, B, TOP_LOGPROBS_MAX, dtype=torch.float32)
+            top_lp = top_lp.pin_memory() if torch.cuda.is_available() else top_lp
+            eng.batch_fetch_topk(first, k, top_ids, top_lp)
+
+        def device_top(step, b):
+            if top_ids is None:
+                return None
+            n = self.top_logprobs_k
+            return list(zip(top_ids[step, b, :n].tolist(), top_lp[step, b, :n].tolist()))
+
+        if self.greedy_sampling:
             toks = _host_buf(k * B).view(k, B)
             lps = torch.empty(k, B, dtype=torch.float32)
             lps = lps.pin_memory() if torch.cuda.is_available() else lps
             eng.batch_fetch(first, k, toks, lps)
-            eng.stream.synchronize()
-            for b, (r, a) in enumerate(zip(active, live)):
-                if not a:
-                    continue
-                col = toks[:, b].tolist()
-                r.buffer.extend((int(t), float(l)) for t, l in zip(col, lps[:, b].tolist()))
-                r.last_token, r.n_decoded = int(col[-1]), r.n_decoded + k
-        else:   # sampler on the host-visible logits of every row (one step at a time)
-            logits = eng.batch_logits_view("logits")
-            for b, (r, a) in enumerate(zip(active, live)):
-                if not a:
-                    continue
-                tok, lp = self._sample(logits[b:b + 1])
-                r.buffer.append((tok, lp))
-                r.last_token, r.n_decoded = tok, r.n_decoded + 1
+        eng.stream.synchronize()
+        logits = None if greedy else eng.batch_logits_view("logits")
+        for b, (r, a) in enumerate(zip(active, live)):
+            if not a:
+                continue
+            if self.greedy_sampling and not host[b]:   # the device's tokens (its processors applied)
+                col = [int(t) for t in toks[:, b].tolist()]
+                entries = [(t, float(l), device_top(i, b)) for i, (t, l) in enumerate(zip(col, lps[:, b].tolist()))]
+            else:   # the sampler (and a host row's processors) on the row's logits
+                entries = []
+            # the step's input tokens join the token context before the processors run
+            self._generation_batch.record_inputs([(r, [r.last_token] + [t for t, _, _ in entries[:-1]])])
+            if not entries:
+                tok, lp, top = self._sample(logits[b:b + 1], r, r.procs if host[b] else None, want_top=host[b])
+                entries = [(tok, lp, top if host[b] else device_top(0, b))]
+            r.buffer.extend(entries)
+            r.last_token, r.n_decoded = entries[-1][0], r.n_decoded + len(entries)
 
     def _decode_slice(self, row: _Row):
         """Refill the row's token buffer: hand the engine to this row for up to `decode_slice`
@@ -458,7 +542,7 @@ class BatchGenerator:
         if left <= 0:
             return
         ctx = int(row.cache[0].offset)
-        if self.greedy_sampling and not self.compute_logprobs:
+        if self.greedy_sampling and not self.compute_logprobs and not row.procs and not self.top_logprobs_k:
             k = min(self.decode_slice, left)
             eng.set_next(row.last_token, ctx, ctx + row.delta)
             base = eng.tokens_launched
@@ -467,19 +551,21 @@ class BatchGenerator:
             eng.fetch_tokens(base, k, host)
             eng.stream.synchronize()
             toks = [int(t) for t in host.tolist()]
-            row.buffer.extend((t, 0.0) for t in toks)
+            row.buffer.extend((t, 0.0, None) for t in toks)
             row.last_token, row.n_decoded = toks[-1], row.n_decoded + k
         else:
             out = lm(np.asarray([[row.last_token]]), cache=row.cache,
                      rope_deltas=np.asarray([[row.delta]]), reserve_tokens=row.reserve)
-            if self.greedy_sampling:
+            self._generation_batch.record_inputs([(row, [row.last_token])])
+            top = None
+            if self.greedy_sampling and not row.procs and not self.top_logprobs_k:
                 lp = eng.snapshot("logprobs").view(-1)
                 with torch.cuda.stream(eng.stream):
                     tok = int(torch.argmax(lp.float()).item())
                     lpv = float(lp[tok].float().item())
             else:
-                tok, lpv = self._sample(out.logits[:, -1, :])
-            row.buffer.append((tok, lpv))
+                tok, lpv, top = self._sample(out.logits[:, -1, :], row, row.procs)
+            row.buffer.append((tok, lpv, top))
             row.last_token, row.n_decoded = tok, row.n_decoded + 1
 
     # ------------------------------------------------------------------ scheduling
@@ -496,7 +582,7 @@ class BatchGenerator:
             for i, row in enumerate(self._active):
                 if not row.buffer:
                     self._decode_slice(row)
-                tok, lp = row.buffer.pop(0)
+                tok, lp, top = row.buffer.pop(0)
                 row.n_tokens += 1
                 finish = None
                 if stop(tok):
@@ -504,7 +590,7 @@ class BatchGenerator:
                 elif row.n_tokens >= row.max_tokens:
                     finish = "length"
                 generation_responses.append(GenerationBatch.Response(
-                    uid=row.uid, token=tok, token_logprob=lp, finish_reason=finish))
+                    uid=row.uid, token=tok, token_logprob=lp, finish_reason=finish, top_logprobs=top))
                 if finish is None:
                     keep.append(i)
             self._gen_tokens_counter += len(self._active)
@@ -517,7 +603,8 @@ class BatchGenerator:
         admitted = []
         # kv_bits=8 rows are admitted one at a time (the grouped prefill has no 8-bit write-through)
         group = (self._lockstep and n_new >= 2 and self.greedy_sampling and not self.compute_logprobs
-                 and self.kv_bits is None
+                 and self.kv_bits is None and not self.top_logprobs_k
+                 and not any(r.procs for r in self._unprocessed_sequences[:n_new])
                  and hasattr(self.model.language_model, "prefill_rows") and self.batched_prefill
                  and (self.prefill_step_size is None
                       or all(len(r.ids) <= self.prefill_step_size + 1 for r in self._unprocessed_sequences[:n_new])))
@@ -529,7 +616,7 @@ class BatchGenerator:
             prompt_responses.append(self._prefill(row))
             admitted.append(row)
         if admitted:
-            self._generation_batch.extend(GenerationBatch(admitted))
+            self._generation_batch.extend(GenerationBatch.admitted(admitted))
         return prompt_responses, generation_responses
 
 
@@ -548,8 +635,15 @@ def batch_generate(model, processor, images=None, prompts: Optional[List[str]] =
     if images is not None and len(images) not in (0, len(prompts)):
         raise ValueError("batch_generate: give one image per prompt (or none)")
     eng = model.engine
+    # the request's penalties and logit bias become every row's processors (ar.py:2890-3097, make_logits_processors)
+    from .sample_utils import make_logits_processors
+    procs = make_logits_processors(kwargs.pop("logit_bias", None), kwargs.pop("repetition_penalty", None),
+                                   kwargs.pop("repetition_context_size", 20), kwargs.pop("presence_penalty", None),
+                                   kwargs.pop("presence_context_size", 20), kwargs.pop("frequency_penalty", None),
+                                   kwargs.pop("frequency_context_size", 20))
+    procs += list(kwargs.pop("logits_processors", None) or [])
     gen = BatchGenerator(model, processor, max_tokens=max_tokens if isinstance(max_tokens, int) else DEFAULT_MAX_TOKENS,
-                         **kwargs)
+                         logits_processors=procs or None, **kwargs)
     ids_list, kw_list, sizes = [], [], []
     for i, prompt in enumerate(prompts):
         img = images[i] if images else None

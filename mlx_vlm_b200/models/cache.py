@@ -694,6 +694,97 @@ class BatchKVCache(_BaseCache):
 BATCH_LOG_STEPS = 4096
 
 
+class BatchProcState:
+    """Device state of the lock-step rows' logits processors (the arrays of `b200_batch_set_procs`), one slot per
+    row of the lock-step batch: parameters, logit-bias lists and a ring of each row's last HIST_CAP tokens.  The
+    device appends each step's input token to the ring of every live row with processors; `move_rows` moves slots
+    with their rows (filter / extend)."""
+    ROWS, HIST_CAP, BIAS_CAP = 16, 1024, 1024
+    FLAGS = {"bias": 1, "repetition": 2, "presence": 4, "frequency": 8}
+
+    def __init__(self, device):
+        R = self.ROWS
+        self.params = torch.zeros(R, 8, dtype=torch.int32, device=device)
+        self.penalties = torch.zeros(R, 8, dtype=torch.float32, device=device)
+        self.bias_ids = torch.zeros(R, self.BIAS_CAP, dtype=torch.int32, device=device)
+        self.bias_vals = torch.zeros(R, self.BIAS_CAP, dtype=torch.float32, device=device)
+        self.hist = torch.zeros(R, self.HIST_CAP, dtype=torch.int32, device=device)
+        self.hist_len = torch.zeros(R, dtype=torch.int32, device=device)
+
+    @classmethod
+    def fits(cls, procs: dict) -> bool:
+        """whether lowered processors fit the device state (else the row runs them as torch ops)"""
+        if len(procs.get("bias", ({},))[0]) > cls.BIAS_CAP:
+            return False
+        return all(0 < int(procs[k][1]) <= cls.HIST_CAP for k in ("repetition", "presence", "frequency") if k in procs)
+
+    @staticmethod
+    def row_values(procs: dict, vocab: int):
+        """(params [8] int32, penalties [8] fp32, bias ids, bias values) of one row, values rounded as the torch ops
+        round them"""
+        par = np.zeros(8, np.int32)
+        pen = np.zeros(8, np.float32)
+        ids, vals = [], []
+        for kind, flag in BatchProcState.FLAGS.items():
+            if kind not in procs:
+                continue
+            par[0] |= flag
+            if kind == "bias":
+                bias = procs["bias"][0]
+                ids = [int(i) for i in bias.keys()]
+                if any(not 0 <= i < vocab for i in ids):
+                    raise ValueError(f"logit_bias: token ids must lie in [0, {vocab})")
+                # the bf16 values the processor adds (torch.tensor(vals, dtype=bfloat16))
+                vals = torch.tensor(list(bias.values()), dtype=torch.bfloat16).float().tolist()
+                par[4] = len(ids)
+            else:
+                p, ctx = procs[kind]
+                par[{"repetition": 1, "presence": 2, "frequency": 3}[kind]] = int(ctx)
+                if kind == "repetition":
+                    pen[0] = np.float32(p)
+                    pen[1] = np.float32(1.0) / np.float32(p)   # x / p is computed as x * fp32(1 / p)
+                else:
+                    pen[2 if kind == "presence" else 3] = np.float32(p)
+        return par, pen, ids, vals
+
+    def set_row(self, row: int, procs: dict, history: List[int], vocab: int):
+        par, pen, ids, vals = self.row_values(procs, vocab)
+        n, cap = len(history), self.HIST_CAP
+        ring = np.zeros(cap, np.int32)
+        for i in range(max(0, n - cap), n):
+            ring[i % cap] = history[i]
+        dev = self.params.device
+        self.params[row] = torch.from_numpy(par).to(dev)
+        self.penalties[row] = torch.from_numpy(pen).to(dev)
+        if ids:
+            self.bias_ids[row, :len(ids)] = torch.tensor(ids, dtype=torch.int32, device=dev)
+            self.bias_vals[row, :len(ids)] = torch.tensor(vals, dtype=torch.float32, device=dev)
+        self.hist[row] = torch.from_numpy(ring).to(dev)
+        self.hist_len[row] = n
+
+    def move_rows(self, src: "BatchProcState", dst_rows: List[int], src_rows: List[int]):
+        if not dst_rows:
+            return
+        d = torch.tensor(dst_rows, dtype=torch.long, device=self.params.device)
+        s = torch.tensor(src_rows, dtype=torch.long, device=self.params.device)
+        for a, b in ((self.params, src.params), (self.penalties, src.penalties), (self.bias_ids, src.bias_ids),
+                     (self.bias_vals, src.bias_vals), (self.hist, src.hist), (self.hist_len, src.hist_len)):
+            a[d] = b[s]
+
+    def clear_rows(self, rows: List[int]):
+        r = torch.tensor(rows, dtype=torch.long, device=self.params.device)
+        self.params[r] = 0
+        self.hist_len[r] = 0
+
+    def history(self, row: int) -> List[int]:
+        n = int(self.hist_len[row])
+        ring = self.hist[row].tolist()
+        return [ring[i % self.HIST_CAP] for i in range(max(0, n - self.HIST_CAP), n)]
+
+    def bind(self, eng, procs_on: bool, top_k: int):
+        eng.batch_set_procs(self if procs_on else None, top_k)
+
+
 class BatchRows:
     """The one owner of the rows of ONE batched device pool (layers, 2, rows, kv heads, capacity, head_dim): its
     allocation and growth, admission into the next free row, compaction after rows leave, every row's length, and
@@ -713,6 +804,9 @@ class BatchRows:
         self.steps = 0     # lock-step steps since the last batch_begin (the next row of the engine's token log)
         self._armed = None  # (version, allocation key, live flags) the device state was armed for
         self._sweep = None  # (state, 8-bit pool, layers served) of the current extract sweep
+        self.procs: List[Optional[dict]] = [None] * len(self.lengths)  # lowered processors of each row (or None)
+        self.top_k = 0      # top-k logprobs of every row and step (0: none)
+        self._pstate = None  # device processor state of the rows (BatchProcState), allocated on first use
 
     @classmethod
     def allocate(cls, engine, n_layers: int, n_kv_heads: int, head_dim: int, rows: int, capacity: int = 0,
@@ -755,12 +849,27 @@ class BatchRows:
                 p.reserve(tokens, live_tokens=max(self.lengths) if self.lengths else 0)
             self._touch()
 
-    def admit(self, length: int) -> int:
+    def admit(self, length: int, procs: Optional[dict] = None, history: Optional[List[int]] = None) -> int:
         """the next free row, already filled in place with `length` positions (a prefill into it), joins the rows;
-        returns its index"""
+        `procs` (sample_utils.lower_logits_processors) are its logits processors, applied on the device over its
+        token history, seeded with `history` (the reference's token context: the prompt ids).  Returns its index"""
+        self.procs = self._row_procs() + [procs or None]
         self.lengths.append(int(length))
+        if procs or self._pstate is not None:   # (a slot without processors is cleared)
+            with _on(self.eng.stream):   # ordered with the kernel that reads the state
+                self._state().set_row(self.B - 1, procs or {}, history or [], self.eng.cfg.vocab)
         self._touch()
         return self.B - 1
+
+    def _row_procs(self) -> List[Optional[dict]]:
+        """`procs` aligned with the rows (rows given lengths directly have none)"""
+        return (self.procs + [None] * self.B)[:self.B]
+
+    def _state(self) -> "BatchProcState":
+        if self._pstate is None:
+            with _on(self.eng.stream):
+                self._pstate = BatchProcState(self.eng.device)
+        return self._pstate
 
     def filter(self, keep):
         keep = [int(i) for i in keep]
@@ -768,7 +877,12 @@ class BatchRows:
         for new_i, old_i in enumerate(keep):
             if new_i != old_i:
                 self.eng.kv_copy_row(self.pool, new_i, self.pool, old_i, self.lengths[old_i])
+        procs = self._row_procs()
         self.lengths = [self.lengths[i] for i in keep]
+        self.procs = [procs[i] for i in keep]
+        if self._pstate is not None:
+            with _on(self.eng.stream):
+                self._pstate.move_rows(self._pstate, list(range(len(keep))), keep)
         self._touch()
 
     def extend(self, other: "BatchRows"):
@@ -776,6 +890,14 @@ class BatchRows:
         self.ensure(self.B + other.B, n)
         for b, ln in enumerate(other.lengths):
             self.eng.kv_copy_row(self.pool, self.B + b, other.pool, b, ln)
+        dst = list(range(self.B, self.B + other.B))
+        if other._pstate is not None:
+            with _on(self.eng.stream):
+                self._state().move_rows(other._pstate, dst, list(range(other.B)))
+        elif self._pstate is not None and dst:   # the slots may still hold a departed row's state
+            with _on(self.eng.stream):
+                self._pstate.clear_rows(dst)
+        self.procs = self._row_procs() + other._row_procs()
         self.lengths = self.lengths + list(other.lengths)
         self._touch()
 
@@ -783,6 +905,11 @@ class BatchRows:
         self.ensure(self.B + 1, max(self.lengths + [length]))
         self.eng.kv_copy_row(self.pool, self.B, src_pool, src_row, length)
         return self.admit(length)
+
+    def history(self, row: int) -> List[int]:
+        """the device token history of a row with processors (its last `BatchProcState.HIST_CAP` tokens at most)"""
+        self.eng.stream.synchronize()
+        return self._state().history(row)
 
     def trim(self, n: int) -> int:
         n = min([n] + self.lengths) if self.lengths else 0
@@ -798,11 +925,14 @@ class BatchRows:
         rather than from the device's own feedback.  A re-arm uploads the values the device already holds.  Returns
         whether it armed."""
         live = [int(a) for a in live]
-        state = (self.version, self.key(), tuple(live))
+        state = (self.version, self.key(), tuple(live), self.top_k)
         if fed_back and state == self._armed and self.steps + k <= BATCH_LOG_STEPS:
             return False
         self.eng.bind_pool(self.pool)
         self.eng.batch_begin(tokens, self.lengths, [n + int(d) for n, d in zip(self.lengths, deltas)], live)
+        procs_on = any(self._row_procs())
+        if procs_on or self.top_k:   # batch_begin turned them off
+            self._state().bind(self.eng, procs_on, self.top_k)
         self._armed, self.steps = state, 0
         return True
 

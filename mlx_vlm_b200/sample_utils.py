@@ -79,6 +79,7 @@ def make_logits_processors(logit_bias: Optional[Dict[int, float]] = None,
             out[:, idx] += v
             return out
 
+        logit_bias_processor.lowered = ("bias", dict(zip(keys, vals)))
         procs.append(logit_bias_processor)
     for make, pen, ctx in ((make_repetition_penalty, repetition_penalty, repetition_context_size),
                            (make_presence_penalty, presence_penalty, presence_context_size),
@@ -86,6 +87,36 @@ def make_logits_processors(logit_bias: Optional[Dict[int, float]] = None,
         if pen is not None and pen != 0:
             procs.append(make(pen, ctx))
     return procs
+
+
+def top_logprobs(logprobs: torch.Tensor, k: int):
+    """[(token id, logprob)] of the k largest entries of a (vocab,) logprob row, largest first, the lower token id
+    first among equal logprobs (the order of the lock-step batch's top-k kernel)."""
+    v, i = torch.sort(logprobs.reshape(-1).float(), descending=True, stable=True)
+    return [(int(a), float(b)) for a, b in zip(i[:k].tolist(), v[:k].tolist())]
+
+
+LOWERED_ORDER = ("bias", "repetition", "presence", "frequency")
+
+
+def lower_logits_processors(procs) -> Optional[Dict[str, tuple]]:
+    """The parameters of a processor list that the lock-step batch applies on the device (csrc/decode_batch.cu
+    `bd_procs_kernel`): {"bias": ({id: value},), "repetition" | "presence" | "frequency": (penalty, context size)}.
+    Only closures of `make_logits_processors` / `make_*_penalty` lower, each kind at most once and in the order
+    make_logits_processors returns them (the order the kernel applies them).  None when the list holds anything
+    else: that row runs its processors as torch ops."""
+    out: Dict[str, tuple] = {}
+    last = -1
+    for p in procs or []:
+        spec = getattr(p, "lowered", None)
+        if not isinstance(spec, tuple) or spec[0] not in LOWERED_ORDER:
+            return None
+        at = LOWERED_ORDER.index(spec[0])
+        if at <= last:
+            return None
+        last = at
+        out[spec[0]] = tuple(spec[1:])
+    return out
 
 
 def apply_top_k(logprobs: torch.Tensor, top_k: int) -> torch.Tensor:
@@ -190,6 +221,7 @@ def make_repetition_penalty(penalty: float, context_size: int = 20):
             logits[:, t] = sel
         return logits
 
+    repetition_penalty_processor.lowered = ("repetition", penalty, context_size)
     return repetition_penalty_processor
 
 
@@ -202,6 +234,7 @@ def make_presence_penalty(penalty: float, context_size: int = 20):
             logits[:, t] -= penalty
         return logits
 
+    presence_penalty_processor.lowered = ("presence", penalty, context_size)
     return presence_penalty_processor
 
 
@@ -214,6 +247,7 @@ def make_frequency_penalty(penalty: float, context_size: int = 20):
             logits = (logits.float() - sub[None]).to(logits.dtype)
         return logits
 
+    frequency_penalty_processor.lowered = ("frequency", penalty, context_size)
     return frequency_penalty_processor
 
 

@@ -15,11 +15,11 @@ from __future__ import annotations
 import queue
 import threading
 from dataclasses import dataclass, field
-from typing import Any, Dict, Iterator, List, Optional
+from typing import Any, Dict, Iterator, List, Optional, Tuple
 
 import numpy as np
 
-from .generate_batch import BatchGenerator
+from .generate_batch import TOP_LOGPROBS_MAX, BatchGenerator
 
 
 @dataclass
@@ -27,6 +27,25 @@ class GenerationArguments:
     max_tokens: int = 256
     temperature: float = 0.0
     logprobs: bool = False
+    top_logprobs: int = 0          # capped to [0, 20] as the reference server caps it (get_top_logprobs_k)
+    repetition_penalty: Optional[float] = None
+    repetition_context_size: int = 20
+    presence_penalty: Optional[float] = None
+    presence_context_size: int = 20
+    frequency_penalty: Optional[float] = None
+    frequency_context_size: int = 20
+    logit_bias: Optional[Dict[int, float]] = None
+
+    def logits_processors(self) -> list:
+        """the request's penalties and logit bias as processors (server/generation.py:689-761)"""
+        from .sample_utils import make_logits_processors
+        bias = {int(k): float(v) for k, v in self.logit_bias.items()} if self.logit_bias else None
+        return make_logits_processors(bias, self.repetition_penalty, self.repetition_context_size,
+                                      self.presence_penalty, self.presence_context_size, self.frequency_penalty,
+                                      self.frequency_context_size)
+
+    def top_k(self) -> int:
+        return max(0, min(int(self.top_logprobs or 0), TOP_LOGPROBS_MAX))
 
 
 @dataclass
@@ -42,6 +61,7 @@ class TokenEvent:
     logprob: float
     finish_reason: Optional[str]
     text: str = ""
+    top_logprobs: Optional[List[Tuple[int, float]]] = None
 
 
 @dataclass
@@ -195,7 +215,9 @@ class ResponseGenerator:
                         gen = self._make_batch_generator(req.args)
                     try:
                         ids, kw = self._gpu_embed(req)
-                        (uid,) = gen.insert([ids], max_tokens=req.args.max_tokens, prompt_kwargs=[kw])
+                        procs = req.args.logits_processors()
+                        (uid,) = gen.insert([ids], max_tokens=req.args.max_tokens, prompt_kwargs=[kw],
+                                            logits_processors=[procs or None])
                     except Exception as e:     # a bad request must not take the loop down
                         req.rqueue.put(e)
                         continue
@@ -204,14 +226,19 @@ class ResponseGenerator:
                 self.peak_active = max(self.peak_active, len(active))
                 if not active or gen is None:
                     continue
+                if hasattr(gen, "top_logprobs_k"):   # the widest top_logprobs any active request asks for
+                    gen.top_logprobs_k = max(r.args.top_k() for r in active.values())
                 _, responses = gen.next()
                 self.steps += 1
                 for r in responses:
                     req = active.get(r.uid)
                     if req is None:
                         continue
+                    k = req.args.top_k()
+                    top = getattr(r, "top_logprobs", None)
                     req.rqueue.put(TokenEvent(token=int(r.token), logprob=float(r.token_logprob),
-                                              finish_reason=r.finish_reason))
+                                              finish_reason=r.finish_reason,
+                                              top_logprobs=list(top[:k]) if k and top else None))
                     if r.finish_reason is not None:
                         active.pop(r.uid)
                         req.rqueue.put(None)
