@@ -11,7 +11,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from ..tower_ops import EPI_GELU_FAST, SplitBuf, TowerOps
+from ..tower_ops import EPI_GELU_FAST, SplitBuf, TowerOps, encoder, pack_encoder_layers, sanitize
 from .config import VisionConfig
 
 
@@ -33,6 +33,8 @@ def bucketed_position_ids(patch_mask: np.ndarray, side: int) -> np.ndarray:
 
 
 class VisionModel:
+    epi = EPI_GELU_FAST       # the MLP's activation: GELU(approx="fast")
+
     def __init__(self, config: VisionConfig, engine_getter):
         self.config = config
         self.model_type = config.model_type
@@ -40,15 +42,7 @@ class VisionModel:
         self.w: Dict[str, torch.Tensor] = {}
 
     def sanitize(self, weights):
-        out = {}
-        for k, v in weights.items():
-            if "position_ids" in k:
-                continue
-            if "patch_embedding.weight" in k and v.ndim == 4 and v.shape[1] == self.config.num_channels \
-                    and v.shape[-1] != self.config.num_channels:
-                v = v.permute(0, 2, 3, 1)     # PyTorch [O, C, kH, kW] -> [O, kH, kW, C]
-            out[k] = v
-        return out
+        return sanitize(weights, self.config.num_channels)
 
     def load(self, weights: Dict[str, torch.Tensor], prefix: str = "vision_model."):
         c, eng = self.config, self._engine()
@@ -65,15 +59,13 @@ class VisionModel:
         put("patch.b", weights[prefix + "embeddings.patch_embedding.bias"])
         put("pos", weights[prefix + "embeddings.position_embedding.weight"])
         put("post.w", weights[prefix + "post_layernorm.weight"]); put("post.b", weights[prefix + "post_layernorm.bias"])
-        for i in range(c.num_hidden_layers):
-            q = prefix + f"encoder.layers.{i}."
-            put(f"{i}.ln1.w", weights[q + "layer_norm1.weight"]); put(f"{i}.ln1.b", weights[q + "layer_norm1.bias"])
-            put(f"{i}.ln2.w", weights[q + "layer_norm2.weight"]); put(f"{i}.ln2.b", weights[q + "layer_norm2.bias"])
-            put(f"{i}.qkv.w", torch.cat([weights[q + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0))
-            put(f"{i}.qkv.b", torch.cat([weights[q + f"self_attn.{n}_proj.bias"] for n in "qkv"], 0))
-            put(f"{i}.out.w", weights[q + "self_attn.out_proj.weight"]); put(f"{i}.out.b", weights[q + "self_attn.out_proj.bias"])
-            put(f"{i}.fc1.w", weights[q + "mlp.fc1.weight"]); put(f"{i}.fc1.b", weights[q + "mlp.fc1.bias"])
-            put(f"{i}.fc2.w", weights[q + "mlp.fc2.weight"]); put(f"{i}.fc2.b", weights[q + "mlp.fc2.bias"])
+        pack_encoder_layers(weights, prefix, c.num_hidden_layers, put)
+
+    def patch_position_ids(self, patch_attention_mask: Optional[np.ndarray], B: int, gh: int, gw: int) -> np.ndarray:
+        """(B, gh * gw) rows of the position table"""
+        if patch_attention_mask is None:
+            patch_attention_mask = np.ones((B, gh, gw), dtype=bool)
+        return bucketed_position_ids(patch_attention_mask, self.config.image_size // self.config.patch_size)
 
     def __call__(self, x: torch.Tensor, patch_attention_mask: Optional[np.ndarray] = None,
                  output_hidden_states: Optional[bool] = None):
@@ -83,17 +75,13 @@ class VisionModel:
         c, eng = self.config, self._engine()
         ops = TowerOps(eng)
         B, H, W, C = x.shape
-        ps, E, I = c.patch_size, c.hidden_size, c.intermediate_size
+        ps, E = c.patch_size, c.hidden_size
         gh, gw = H // ps, W // ps
         P = gh * gw
         T = B * P
-        nh = c.num_attention_heads
-        hd = E // nh
         K = ps * ps * C
         w = self.w
-        if patch_attention_mask is None:
-            patch_attention_mask = np.ones((B, gh, gw), dtype=bool)
-        pos_ids = bucketed_position_ids(patch_attention_mask, c.image_size // ps).astype(np.int32)
+        pos_ids = self.patch_position_ids(patch_attention_mask, B, gh, gw).astype(np.int32)
         pos_dev = torch.from_numpy(np.ascontiguousarray(pos_ids))
         with torch.cuda.stream(eng.stream):
             pos_dev = pos_dev.to(eng.device)
@@ -104,17 +92,8 @@ class VisionModel:
         ops.linear(pat, w["patch"], w["patch.b"], out32=patch, k_w=K)
         h = ops.f32(T, E)
         ops.embed(patch, None, w["pos"], pos_dev, h, B, P)
-        y, o, mlp = SplitBuf(eng, T, E), SplitBuf(eng, T, E), SplitBuf(eng, T, I)
-        qkv = ops.f32(T, 3 * E)
-        for i in range(c.num_hidden_layers):
-            ops.layer_norm(h, w[f"{i}.ln1.w"], w[f"{i}.ln1.b"], c.layer_norm_eps, out_split=y)
-            ops.linear(y, w[f"{i}.qkv.w"], w[f"{i}.qkv.b"], out32=qkv)
-            ops.attention((qkv, 3 * E, hd), (qkv[:, E:], 3 * E, hd), (qkv[:, 2 * E:], 3 * E, hd), n_heads=nh, n_kv=nh,
-                          hd=hd, Lq=P, S=P, n_seg=B, q_seg=P, k_seg=P, scale=hd ** -0.5, out_split=o)
-            ops.linear(o, w[f"{i}.out.w"], w[f"{i}.out.b"], out32=h, res32=h)
-            ops.layer_norm(h, w[f"{i}.ln2.w"], w[f"{i}.ln2.b"], c.layer_norm_eps, out_split=y)
-            ops.linear(y, w[f"{i}.fc1.w"], w[f"{i}.fc1.b"], out_split=mlp, epi=EPI_GELU_FAST)
-            ops.linear(mlp, w[f"{i}.fc2.w"], w[f"{i}.fc2.b"], out32=h, res32=h)
+        encoder(ops, w, h, c.num_hidden_layers, n_heads=c.num_attention_heads, inter=c.intermediate_size, seg=P,
+                eps=c.layer_norm_eps, epi=self.epi)
         pooled = ops.f32(T, E)
         ops.layer_norm(h, w["post.w"], w["post.b"], 1e-5, out32=pooled)   # nn.LayerNorm default eps (vision.py:184)
         return pooled, None, None

@@ -15,6 +15,7 @@ from ..tower_ops import SplitBuf, TowerOps
 from .config import ModelConfig
 from .language import LanguageModel
 from .vision import VisionModel
+from .weights import random_weights
 
 
 class Connector:
@@ -50,16 +51,7 @@ class Connector:
 
 
 class Model(_Idefics2Model):
-    def __init__(self, config: ModelConfig, device=None):
-        self.config = config
-        self._device = torch.device(device) if device is not None else torch.device("cuda", 0)
-        self._eng = None
-        self._weights = None
-        self.vision_model = VisionModel(config.vision_config, self._engine)
-        self.connector = Connector(config, self._engine)
-        self.language_model = LanguageModel(config.text_config, config, self._engine)
-
-    def init_random(self, seed: int = 0, std: float = 0.02):
-        from .weights import random_weights
-        self.load_weights(random_weights(self.config, seed, std, self._engine().device))
-        return self
+    LanguageModel = LanguageModel
+    VisionModel = VisionModel
+    Connector = Connector
+    random_weights = staticmethod(random_weights)

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from ..idefics2.vision import VisionModel as _SiglipTower
-from ..tower_ops import EPI_GELU_TANH, SplitBuf, TowerOps
+from ..tower_ops import EPI_GELU_TANH
 
 
 def _arange_f32(start: float, stop: float, step: float) -> np.ndarray:
@@ -50,6 +50,8 @@ def position_ids(patch_mask: np.ndarray, side: int, seq: int) -> np.ndarray:
 
 
 class VisionModel(_SiglipTower):
+    epi = EPI_GELU_TANH       # GELU(approx="precise"): the tanh form
+
     def load(self, weights, prefix: str = "vision_model."):
         super().load(weights, prefix)
         pos = self.w["pos"]
@@ -57,47 +59,12 @@ class VisionModel(_SiglipTower):
         with torch.cuda.stream(self._engine().stream):      # one extra all-zero row: the "masked" position
             self.w["pos"] = torch.cat([pos, torch.zeros_like(pos[:1])], 0).contiguous()
 
-    def __call__(self, x: torch.Tensor, patch_attention_mask: Optional[np.ndarray] = None,
-                 output_hidden_states: Optional[bool] = None):
-        """x: NHWC fp32 (n_img, H, W, C) on the device -> (pooler_output fp32 (n_img * P, E), None, None)"""
-        c, eng = self.config, self._engine()
-        ops = TowerOps(eng)
-        B, H, W, C = x.shape
-        ps, E, I = c.patch_size, c.hidden_size, c.intermediate_size
-        gh, gw = H // ps, W // ps
+    def patch_position_ids(self, patch_attention_mask: Optional[np.ndarray], B: int, gh: int, gw: int) -> np.ndarray:
+        """vision.py:95-141: padding patches take the zero row"""
         P = gh * gw
-        T = B * P
-        nh = c.num_attention_heads
-        hd = E // nh
-        K = ps * ps * C
-        w = self.w
         if patch_attention_mask is None:
-            ids = np.tile(np.arange(P, dtype=np.int64), (B, 1))          # vision.py:99-103
-        else:
-            m = np.asarray(patch_attention_mask).astype(bool)
-            ids = position_ids(m, c.image_size // ps, P)
-            ids[~m.reshape(B, -1)[:, :P]] = self.n_pos                   # zero row
-        pos_dev = torch.from_numpy(np.ascontiguousarray(ids.astype(np.int32)))
-        with torch.cuda.stream(eng.stream):
-            pos_dev = pos_dev.to(eng.device)
-        x = x.contiguous()
-        pat = SplitBuf(eng, T, K)
-        ops.patchify(x, ps, pat)
-        patch = ops.f32(T, E)
-        ops.linear(pat, w["patch"], w["patch.b"], out32=patch, k_w=K)
-        h = ops.f32(T, E)
-        ops.embed(patch, None, w["pos"], pos_dev, h, B, P)
-        y, o, mlp = SplitBuf(eng, T, E), SplitBuf(eng, T, E), SplitBuf(eng, T, I)
-        qkv = ops.f32(T, 3 * E)
-        for i in range(c.num_hidden_layers):
-            ops.layer_norm(h, w[f"{i}.ln1.w"], w[f"{i}.ln1.b"], c.layer_norm_eps, out_split=y)
-            ops.linear(y, w[f"{i}.qkv.w"], w[f"{i}.qkv.b"], out32=qkv)
-            ops.attention((qkv, 3 * E, hd), (qkv[:, E:], 3 * E, hd), (qkv[:, 2 * E:], 3 * E, hd), n_heads=nh, n_kv=nh,
-                          hd=hd, Lq=P, S=P, n_seg=B, q_seg=P, k_seg=P, scale=hd ** -0.5, out_split=o)
-            ops.linear(o, w[f"{i}.out.w"], w[f"{i}.out.b"], out32=h, res32=h)
-            ops.layer_norm(h, w[f"{i}.ln2.w"], w[f"{i}.ln2.b"], c.layer_norm_eps, out_split=y)
-            ops.linear(y, w[f"{i}.fc1.w"], w[f"{i}.fc1.b"], out_split=mlp, epi=EPI_GELU_TANH)
-            ops.linear(mlp, w[f"{i}.fc2.w"], w[f"{i}.fc2.b"], out32=h, res32=h)
-        pooled = ops.f32(T, E)
-        ops.layer_norm(h, w["post.w"], w["post.b"], 1e-5, out32=pooled)   # nn.LayerNorm default eps (vision.py:159)
-        return pooled, None, None
+            return np.tile(np.arange(P, dtype=np.int64), (B, 1))          # vision.py:99-103
+        m = np.asarray(patch_attention_mask).astype(bool)
+        ids = position_ids(m, self.config.image_size // self.config.patch_size, P)
+        ids[~m.reshape(B, -1)[:, :P]] = self.n_pos                       # zero row
+        return ids

@@ -5,8 +5,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from ..engine_model import _np
 from ..qwen2_vl.language import LanguageModel as _DecoderLM
-from ..qwen2_vl.language import _np
 
 
 class LanguageModel(_DecoderLM):

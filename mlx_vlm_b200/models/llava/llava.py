@@ -3,121 +3,39 @@
 `_merge_input_ids_with_image_features`, `vision_tower`, `language_model`, `layers`, `sanitize`."""
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict
 
-import numpy as np
 import torch
 
 from ... import _native as N
-from ...engine import Engine
 from ..base import InputEmbeddingsFeatures
-from ..qwen2_vl.language import _np
-from ..qwen2_vl.qwen2_vl import WeightArena, _ids_to_device, weight_manifest
+from ..engine_model import EngineModel, _np, embed_merge, embed_tokens
 from ..tower_ops import EPI_GELU_EXACT, SplitBuf, TowerOps
 from .config import ModelConfig
 from .language import LanguageModel
 from .vision import VisionModel
+from .weights import random_weights
 
 
-def embed_tokens(eng: Engine, ids_host: np.ndarray) -> torch.Tensor:
-    ids_host = np.asarray(ids_host)
-    if ids_host.ndim == 1:
-        ids_host = ids_host[None]
-    B, T = ids_host.shape
-    out = eng.empty((B, T, eng.cfg.hidden))
-    ids = _ids_to_device(eng, ids_host)
-    N.check(eng.lib.b200_embed_merge(ids.data_ptr(), B, T, eng.weights["lm.embed"].data_ptr(), eng.cfg.hidden,
-                                     0, 0, -1, -1, out.data_ptr(), 0, eng.s), "embed")
-    return out
+class Model(EngineModel):
+    LanguageModel = LanguageModel
+    VisionModel = VisionModel
+    random_weights = staticmethod(random_weights)
 
-
-class Model:
     def __init__(self, config: ModelConfig, device=None):
-        self.config = config
-        self._device = torch.device(device) if device is not None else torch.device("cuda", 0)
-        self._eng: Optional[Engine] = None
-        self._weights: Optional[WeightArena] = None
-        self.vision_tower = VisionModel(config.vision_config, self._engine)
-        self.language_model = LanguageModel(config.text_config, config, self._engine)
+        super().__init__(config, device)
+        self.vision_tower = self.VisionModel(config.vision_config, self._engine)
         self.proj: Dict[str, torch.Tensor] = {}
         self.vision_feature_layer = config.vision_feature_layer
         self.vision_feature_select_strategy = config.vision_feature_select_strategy
 
-    # ------------------------------------------------------------- engine (decoder only)
-    def native_config(self) -> N.Qwen2VLConfig:
-        t = self.config.text_config
-        c = N.Qwen2VLConfig()
-        c.hidden, c.n_layers, c.inter = t.hidden_size, t.num_hidden_layers, t.intermediate_size
-        c.n_heads, c.n_kv_heads = t.num_attention_heads, t.num_key_value_heads
-        c.head_dim = t.hidden_size // t.num_attention_heads
-        c.vocab = t.vocab_size
-        c.rms_eps, c.rope_theta = t.rms_norm_eps, t.rope_theta
-        c.mrope_section[0], c.mrope_section[1], c.mrope_section[2] = c.head_dim // 2, 0, 0   # plain RoPE
-        c.tie_embeddings = int(t.tie_word_embeddings)
-        c.external_vision = 1
-        c.v_depth, c.v_embed, c.v_heads, c.v_mlp, c.v_patch_dim, c.v_merge = 0, 8, 1, 8, 8, 1
-        c.v_out, c.v_ln_eps = t.hidden_size, 1e-5
-        return c
-
-    def _engine(self) -> Engine:
-        if self._eng is None:
-            self._eng = Engine(self.native_config(), self._device)
-        return self._eng
-
-    @property
-    def engine(self) -> Engine:
-        return self._engine()
-
-    def _arena(self) -> WeightArena:
-        if self._weights is None:
-            self._weights = WeightArena(weight_manifest(self.native_config()), self._engine().device)
-        return self._weights
-
-    @property
-    def packed_weights(self) -> torch.Tensor:
-        return self._arena().flat
-
-    def _put(self, name, value):
-        v = self._arena().view(name)
-        v.copy_(value.reshape(v.shape).to(device=v.device, dtype=torch.bfloat16))
-        self._engine().set_weight(name, v)
-
-    # ------------------------------------------------------------- weights
-    def sanitize(self, weights):
-        return weights
-
-    def load_weights(self, weights: Dict[str, torch.Tensor], strict: bool = True):
-        """reference-named tensors (vision_tower.* / multi_modal_projector.* / language_model.*)"""
-        eng = self._engine()
-        t = self.config.text_config
-        dev = eng.device
-        hd = t.hidden_size // t.num_attention_heads
-        QKV = (t.num_attention_heads + 2 * t.num_key_value_heads) * hd
+    def _load_vision(self, weights: Dict[str, torch.Tensor]):
+        """reference-named tensors vision_tower.* / multi_modal_projector.*"""
+        dev = self._engine().device
         self.vision_tower.load(self.vision_tower.sanitize({k: v for k, v in weights.items() if k.startswith("vision_tower")}))
         for n in ("linear_1", "linear_2"):
             self.proj[n + ".w"] = weights[f"multi_modal_projector.{n}.weight"].to(device=dev, dtype=torch.bfloat16).contiguous()
             self.proj[n + ".b"] = weights[f"multi_modal_projector.{n}.bias"].to(device=dev, dtype=torch.bfloat16).contiguous()
-        put = self._put
-        put("lm.embed", weights["language_model.model.embed_tokens.weight"])
-        put("lm.norm", weights["language_model.model.norm.weight"])
-        if not t.tie_word_embeddings:
-            put("lm.head", weights["language_model.lm_head.weight"])
-        for i in range(t.num_hidden_layers):
-            p, q = f"language_model.model.layers.{i}.", f"lm.{i}."
-            put(q + "ln1", weights[p + "input_layernorm.weight"])
-            put(q + "ln2", weights[p + "post_attention_layernorm.weight"])
-            put(q + "wqkv", torch.cat([weights[p + f"self_attn.{n}_proj.weight"].to(dev) for n in "qkv"], 0))
-            put(q + "bqkv", torch.zeros(QKV))      # Llama: no q/k/v bias
-            put(q + "wo", weights[p + "self_attn.o_proj.weight"])
-            put(q + "wgu", torch.cat([weights[p + "mlp.gate_proj.weight"].to(dev), weights[p + "mlp.up_proj.weight"].to(dev)], 0))
-            put(q + "wd", weights[p + "mlp.down_proj.weight"])
-        torch.cuda.synchronize(dev)
-
-    def init_random(self, seed: int = 0, std: float = 0.02):
-        """seeded random-init at the configured shapes (benchmarks; no checkpoints offline)"""
-        from .weights import random_weights
-        self.load_weights(random_weights(self.config, seed, std, self._engine().device))
-        return self
 
     # ------------------------------------------------------------- contract
     def encode_image(self, pixel_values: torch.Tensor) -> torch.Tensor:
@@ -167,7 +85,6 @@ class Model:
         ids = _np(input_ids)
         if ids.ndim == 1:
             ids = ids[None]
-        B, T = ids.shape
         tok = self.config.image_token_index
         n_pos = int((ids == tok).sum())
         flat = image_features.reshape(-1, image_features.shape[-1])
@@ -177,27 +94,6 @@ class Model:
         if flat.shape[0] < n_pos:
             raise ValueError(f"shape mismatch: {flat.shape[0]} image feature rows cannot fill {n_pos} <image> "
                              "positions")
-        H = int(flat.shape[-1])
-        out = eng.empty((B, T, H))
-        feats = flat.contiguous()
         if inputs_embeds is None:
-            ids_dev = _ids_to_device(eng, ids)
-            N.check(eng.lib.b200_embed_merge(ids_dev.data_ptr(), B, T, eng.weights["lm.embed"].data_ptr(), H,
-                                             feats.data_ptr(), flat.shape[0], int(tok), -1, out.data_ptr(), 0, eng.s),
-                    "embed_merge")
-            return out
-        sent = B * T
-        ids2 = np.where(ids == tok, sent, np.arange(B * T).reshape(B, T))
-        ids_dev = _ids_to_device(eng, ids2)
-        table = inputs_embeds.reshape(B * T, H).contiguous()
-        N.check(eng.lib.b200_embed_merge(ids_dev.data_ptr(), B, T, table.data_ptr(), H, feats.data_ptr(), flat.shape[0],
-                                         sent, sent, out.data_ptr(), 0, eng.s), "embed_merge")
-        return out
-
-    @property
-    def layers(self):
-        return self.language_model.layers
-
-    def __call__(self, input_ids, pixel_values=None, mask=None, cache=None, **kwargs):
-        feats = self.get_input_embeddings(input_ids, pixel_values, **kwargs)
-        return self.language_model(input_ids, feats.inputs_embeds, mask=mask, cache=cache)
+            return embed_merge(eng, ids, flat, flat.shape[0], tok)
+        return embed_merge(eng, ids, flat, flat.shape[0], inputs_embeds=inputs_embeds, rows=ids == tok)

@@ -8,7 +8,7 @@ from typing import Dict, Optional
 
 import torch
 
-from ..tower_ops import EPI_GELU_FAST, SplitBuf, TowerOps
+from ..tower_ops import EPI_GELU_FAST, SplitBuf, TowerOps, encoder, pack_encoder_layers, sanitize
 from .config import VisionConfig
 
 
@@ -23,17 +23,9 @@ class VisionModel:
         self._engine = engine_getter
         self.w: Dict[str, torch.Tensor] = {}
 
-    # reference vision.py:196-221: PyTorch conv weights [O, C, kH, kW] -> [O, kH, kW, C]
     def sanitize(self, weights):
-        out = {}
-        for k, v in weights.items():
-            if "position_ids" in k:
-                continue
-            if "patch_embedding.weight" in k and v.ndim == 4 and v.shape[1] == self.config.num_channels \
-                    and v.shape[-1] != self.config.num_channels:
-                v = v.permute(0, 2, 3, 1)
-            out[k] = v
-        return out
+        """reference vision.py:196-221"""
+        return sanitize(weights, self.config.num_channels)
 
     def load(self, weights: Dict[str, torch.Tensor]):
         """weights: reference names below `vision_tower.vision_model.` (post-sanitize layouts)"""
@@ -56,15 +48,7 @@ class VisionModel:
             if p + n + ".weight" in weights:
                 put(n + ".w", weights[p + n + ".weight"])
                 put(n + ".b", weights[p + n + ".bias"])
-        for i in range(c.num_hidden_layers):
-            q = p + f"encoder.layers.{i}."
-            put(f"{i}.ln1.w", weights[q + "layer_norm1.weight"]); put(f"{i}.ln1.b", weights[q + "layer_norm1.bias"])
-            put(f"{i}.ln2.w", weights[q + "layer_norm2.weight"]); put(f"{i}.ln2.b", weights[q + "layer_norm2.bias"])
-            put(f"{i}.qkv.w", torch.cat([weights[q + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0))
-            put(f"{i}.qkv.b", torch.cat([weights[q + f"self_attn.{n}_proj.bias"] for n in "qkv"], 0))
-            put(f"{i}.out.w", weights[q + "self_attn.out_proj.weight"]); put(f"{i}.out.b", weights[q + "self_attn.out_proj.bias"])
-            put(f"{i}.fc1.w", weights[q + "mlp.fc1.weight"]); put(f"{i}.fc1.b", weights[q + "mlp.fc1.bias"])
-            put(f"{i}.fc2.w", weights[q + "mlp.fc2.weight"]); put(f"{i}.fc2.b", weights[q + "mlp.fc2.bias"])
+        pack_encoder_layers(weights, p, c.num_hidden_layers, put)
 
     def __call__(self, x: torch.Tensor, output_hidden_states: Optional[bool] = None, feature_layer: int = -2):
         """x: pixel_values NHWC fp32 (B, H, W, C) on the device -> (None, selected state, states) where
@@ -74,12 +58,10 @@ class VisionModel:
         c, eng = self.config, self._engine()
         ops = TowerOps(eng)
         B, H, W, C = x.shape
-        ps, E, I = c.patch_size, c.hidden_size, c.intermediate_size
+        ps, E = c.patch_size, c.hidden_size
         P = (H // ps) * (W // ps)
         L = P + 1
         T = B * L
-        nh = c.num_attention_heads
-        hd = E // nh
         K = ps * ps * C
         w = self.w
         x = x.contiguous()
@@ -93,19 +75,8 @@ class VisionModel:
         ops.layer_norm(emb, w["pre_layrnorm.w"], w["pre_layrnorm.b"], 1e-5, out32=h)   # nn.LayerNorm default eps
         n_states = c.num_hidden_layers + 1
         want = feature_layer % n_states
-        y = SplitBuf(eng, T, E)
-        o = SplitBuf(eng, T, E)
-        mlp = SplitBuf(eng, T, I)
-        qkv = ops.f32(T, 3 * E)
-        for i in range(want):
-            ops.layer_norm(h, w[f"{i}.ln1.w"], w[f"{i}.ln1.b"], c.layer_norm_eps, out_split=y)
-            ops.linear(y, w[f"{i}.qkv.w"], w[f"{i}.qkv.b"], out32=qkv)
-            ops.attention((qkv, 3 * E, hd), (qkv[:, E:], 3 * E, hd), (qkv[:, 2 * E:], 3 * E, hd), n_heads=nh, n_kv=nh,
-                          hd=hd, Lq=L, S=L, n_seg=B, q_seg=L, k_seg=L, scale=hd ** -0.5, out_split=o)
-            ops.linear(o, w[f"{i}.out.w"], w[f"{i}.out.b"], out32=h, res32=h)
-            ops.layer_norm(h, w[f"{i}.ln2.w"], w[f"{i}.ln2.b"], c.layer_norm_eps, out_split=y)
-            ops.linear(y, w[f"{i}.fc1.w"], w[f"{i}.fc1.b"], out_split=mlp, epi=EPI_GELU_FAST)
-            ops.linear(mlp, w[f"{i}.fc2.w"], w[f"{i}.fc2.b"], out32=h, res32=h)
+        encoder(ops, w, h, want, n_heads=c.num_attention_heads, inter=c.intermediate_size, seg=L, eps=c.layer_norm_eps,
+                epi=EPI_GELU_FAST)
         states = _States([None] * n_states)
         states[want] = h
         return None, h, states

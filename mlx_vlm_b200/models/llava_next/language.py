@@ -6,8 +6,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from ..engine_model import _np
 from ..llava.language import LanguageModel as _LlavaLM
-from ..qwen2_vl.language import _np
 
 
 class LanguageModel(_LlavaLM):

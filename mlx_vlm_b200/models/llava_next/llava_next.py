@@ -15,13 +15,11 @@ from typing import Dict, List, Tuple
 import numpy as np
 import torch
 
-from ... import _native as N
 from ..base import InputEmbeddingsFeatures
+from ..engine_model import _np, embed_merge, embed_tokens
 from ..llava.llava import Model as _LlavaModel
-from ..llava.llava import embed_tokens
-from ..qwen2_vl.language import _np
-from ..qwen2_vl.qwen2_vl import _ids_to_device
 from .config import ModelConfig
+from .language import LanguageModel
 
 
 def merge_plan(input_ids, image_token_index: int, n_blocks: int, rows_per_block: int) -> Tuple[List[int], int]:
@@ -46,10 +44,10 @@ def merge_plan(input_ids, image_token_index: int, n_blocks: int, rows_per_block:
 
 
 class Model(_LlavaModel):
+    LanguageModel = LanguageModel
+
     def __init__(self, config: ModelConfig, device=None):
         super().__init__(config, device)
-        from .language import LanguageModel
-        self.language_model = LanguageModel(config.text_config, config, self._engine)
         self.image_newline: torch.Tensor = None   # (hidden,) bf16 on the device, set by load_weights
 
     def load_weights(self, weights: Dict[str, torch.Tensor], strict: bool = True):
@@ -58,8 +56,7 @@ class Model(_LlavaModel):
         torch.cuda.synchronize(self._engine().device)
 
     def init_random(self, seed: int = 0, std: float = 0.02):
-        from ..llava.weights import random_weights
-        W = random_weights(self.config, seed, std, self._engine().device)
+        W = self.random_weights(self.config, seed, std, self._engine().device)
         g = torch.Generator(device=self._engine().device).manual_seed(seed + 1)
         H = self.config.text_config.hidden_size
         W["image_newline"] = (torch.randn(H, generator=g, device=self._engine().device) / H ** 0.5).to(torch.bfloat16)
@@ -92,16 +89,10 @@ class Model(_LlavaModel):
 
     def _merge_input_ids_with_image_features(self, image_features, inputs_embeds, input_ids):
         """llava_next.py:98-121 on the device: host plan (merge_plan) + the shared gather kernel"""
-        eng = self._engine()
+        if inputs_embeds is not None:
+            raise NotImplementedError("llava_next merge: pass inputs_embeds=None (the embedding lookup is fused)")
         n_blocks, P, H = int(image_features.shape[0]), int(image_features.shape[1]), int(image_features.shape[2])
         tok = int(self.config.image_token_index)
         plan, used = merge_plan(input_ids, tok, n_blocks, P)
-        T = len(plan)
-        out = eng.empty((1, T, H))
-        feats = image_features[:max(used, 1)].reshape(-1, H).contiguous()
-        ids_dev = _ids_to_device(eng, np.asarray([plan], dtype=np.int64))
-        if inputs_embeds is not None:
-            raise NotImplementedError("llava_next merge: pass inputs_embeds=None (the embedding lookup is fused)")
-        N.check(eng.lib.b200_embed_merge(ids_dev.data_ptr(), 1, T, eng.weights["lm.embed"].data_ptr(), H, feats.data_ptr(),
-                                         used * P, tok, -1, out.data_ptr(), 0, eng.s), "embed_merge")
-        return out
+        return embed_merge(self._engine(), np.asarray([plan], dtype=np.int64),
+                           image_features[:max(used, 1)].reshape(-1, H), used * P, tok)

@@ -8,66 +8,15 @@ from typing import Dict
 
 import torch
 
-from ... import _native as N
 from ..qwen2_vl.qwen2_vl import Model as _Qwen2VLModel
-from .config import ModelConfig
-from .language import LanguageModel
 from .vision import VisionModel
+from .weights import random_weights
 
 
 class Model(_Qwen2VLModel):
-    def __init__(self, config: ModelConfig, device=None):
-        self.config = config
-        self._device = torch.device(device) if device is not None else torch.device("cuda", 0)
-        self._eng = None
-        self.vision_tower = VisionModel(config.vision_config, self._engine)
-        self.language_model = LanguageModel(config.text_config, config, self._engine)
+    VisionModel = VisionModel
+    random_weights = staticmethod(random_weights)
+    builtin_tower = False
 
-    def native_config(self) -> N.Qwen2VLConfig:
-        t = self.config.text_config
-        c = N.Qwen2VLConfig()
-        c.hidden, c.n_layers, c.inter = t.hidden_size, t.num_hidden_layers, t.intermediate_size
-        c.n_heads, c.n_kv_heads = t.num_attention_heads, t.num_key_value_heads
-        c.head_dim = t.hidden_size // t.num_attention_heads
-        c.vocab = t.vocab_size
-        c.rms_eps, c.rope_theta = t.rms_norm_eps, t.rope_theta
-        sec = t.mrope_section
-        c.mrope_section[0], c.mrope_section[1], c.mrope_section[2] = sec[0], sec[1], sec[2]
-        c.tie_embeddings = int(t.tie_word_embeddings)
-        c.external_vision = 1
-        c.v_depth, c.v_embed, c.v_heads, c.v_mlp, c.v_patch_dim, c.v_merge = 0, 8, 1, 8, 8, 1
-        c.v_out, c.v_ln_eps = t.hidden_size, 1e-6
-        return c
-
-    def load_weights(self, weights: Dict[str, torch.Tensor], strict: bool = True):
-        eng = self._engine()
-        t = self.config.text_config
-        dev = eng.device
-
-        def get(name):
-            if name not in weights:
-                raise KeyError(f"missing weight {name}")
-            return weights[name]
-
+    def _load_vision(self, weights: Dict[str, torch.Tensor]):
         self.vision_tower.load(self.vision_tower.sanitize({k: x for k, x in weights.items() if "vision_tower" in k}))
-        put = self._put
-        put("lm.embed", get("language_model.model.embed_tokens.weight"))
-        put("lm.norm", get("language_model.model.norm.weight"))
-        if not t.tie_word_embeddings:
-            put("lm.head", get("language_model.lm_head.weight"))
-        for i in range(t.num_hidden_layers):
-            p, q = f"language_model.model.layers.{i}.", f"lm.{i}."
-            put(q + "ln1", get(p + "input_layernorm.weight"))
-            put(q + "ln2", get(p + "post_attention_layernorm.weight"))
-            put(q + "wqkv", torch.cat([get(p + f"self_attn.{n}_proj.weight").to(dev) for n in "qkv"], 0))
-            put(q + "bqkv", torch.cat([get(p + f"self_attn.{n}_proj.bias").to(dev) for n in "qkv"], 0))
-            put(q + "wo", get(p + "self_attn.o_proj.weight"))
-            put(q + "wgu", torch.cat([get(p + "mlp.gate_proj.weight").to(dev), get(p + "mlp.up_proj.weight").to(dev)], 0))
-            put(q + "wd", get(p + "mlp.down_proj.weight"))
-        torch.cuda.synchronize(dev)
-
-    def init_random(self, seed: int = 0, std: float = 0.02):
-        """seeded random-init at the configured shapes (benchmarks; no checkpoints offline)"""
-        from .weights import random_weights
-        self.load_weights(random_weights(self.config, seed, std, self._engine().device))
-        return self

@@ -17,15 +17,8 @@ import torch
 from ..base import LanguageModelOutput
 from ..cache import (BatchKVQPool, BatchQuantizedKVCache, BatchRows, KVCache, KVPool, QuantizedKVCache,
                      RowBatchKVCache)
+from ..engine_model import _np, embed_tokens
 from .config import ModelConfig, TextConfig
-
-
-def _np(x, dtype=np.int64):
-    if x is None:
-        return None
-    if isinstance(x, torch.Tensor):
-        return x.detach().cpu().numpy().astype(dtype)
-    return np.asarray(x, dtype=dtype)
 
 
 class LanguageModel:
@@ -251,7 +244,6 @@ class LanguageModel:
             logits = eng.snapshot("logits").view(1, 1, V)
         else:
             if inputs_embeds is None:
-                from .qwen2_vl import embed_tokens
                 inputs_embeds = embed_tokens(eng, ids_host)
             emb = inputs_embeds.reshape(-1, inputs_embeds.shape[-1])
             assert emb.shape[0] == L and emb.dtype == torch.bfloat16 and emb.is_cuda

@@ -1,56 +1,32 @@
 """Qwen2-VL `Model` — the per-model contract of the reference
 (mlx_vlm/models/qwen2_vl/qwen2_vl.py:13-190): `get_input_embeddings`,
 `merge_input_ids_with_image_features`, `vision_tower`, `language_model`, `layers`,
-`sanitize`; plus weight packing for the native engine.
+`sanitize`.  The decoder engine runs its built-in vision tower for this family only: the tower's
+engine fields, arena rows and weight packing are here, the rest is models/engine_model.py.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict
 
-import numpy as np
 import torch
 
 from ... import _native as N
 from ...engine import Engine
 from ..base import InputEmbeddingsFeatures
+from ..engine_model import WeightArena  # noqa: F401  (the arena, importable from here as before)
+from ..engine_model import EngineModel, _np, embed_merge, embed_tokens
+from ..engine_model import weight_manifest as decoder_manifest
 from .config import ModelConfig
-from .language import LanguageModel, _np
+from .language import LanguageModel
 from .vision import VisionModel
 
 
-def _ids_to_device(eng: Engine, ids_host: np.ndarray) -> torch.Tensor:
-    t = torch.from_numpy(np.ascontiguousarray(ids_host, dtype=np.int32))
-    with torch.cuda.stream(eng.stream):
-        return t.to(eng.device)
-
-
-def embed_tokens(eng: Engine, ids_host: np.ndarray) -> torch.Tensor:
-    """nn.Embedding lookup (language.py:183) through the merge kernel with no features."""
-    ids_host = np.asarray(ids_host).reshape(1, -1) if np.asarray(ids_host).ndim == 1 else np.asarray(ids_host)
-    B, T = ids_host.shape
-    H = eng.cfg.hidden
-    out = eng.empty((B, T, H))
-    ids = _ids_to_device(eng, ids_host)
-    N.check(eng.lib.b200_embed_merge(ids.data_ptr(), B, T, eng.weights["lm.embed"].data_ptr(), H,
-                                     0, 0, -1, -1, out.data_ptr(), 0, eng.s), "embed")
-    return out
-
-
-def weight_manifest(c: N.Qwen2VLConfig):
-    """(engine name, shape) of every tensor of the engine layout, in a fixed order (DESIGN.md §3)."""
+def weight_manifest(c: N.Qwen2VLConfig, qk_norm: bool = False):
+    """(engine name, shape) of every tensor of the engine layout, in a fixed order (DESIGN.md §3): the built-in
+    vision tower and merger lead when the engine runs them (external_vision = 0), then the decoder"""
+    if c.external_vision:
+        return decoder_manifest(c, qk_norm)
     E, Em, mg = c.v_embed, c.v_mlp, c.v_merge ** 2 * c.v_embed
-    H, I = c.hidden, c.inter
-    QKV = (c.n_heads + 2 * c.n_kv_heads) * c.head_dim
-    out = []
-    if c.external_vision:   # decoder-only engine (LLaVA / Idefics2): the tower's weights live with the tower
-        out += [("lm.embed", (c.vocab, H)), ("lm.norm", (H,))]
-        if not c.tie_embeddings:
-            out.append(("lm.head", (c.vocab, H)))
-        for i in range(c.n_layers):
-            q = f"lm.{i}."
-            out += [(q + "ln1", (H,)), (q + "ln2", (H,)), (q + "wqkv", (QKV, H)), (q + "bqkv", (QKV,)),
-                    (q + "wo", (H, c.n_heads * c.head_dim)), (q + "wgu", (2 * I, H)), (q + "wd", (H, I))]
-        return out
     out = [("v.patch_embed.w", (E, c.v_patch_dim))]
     for i in range(c.v_depth):
         q = f"v.blk.{i}."
@@ -59,84 +35,35 @@ def weight_manifest(c: N.Qwen2VLConfig):
                 (q + "fc1.w", (Em, E)), (q + "fc1.b", (Em,)), (q + "fc2.w", (E, Em)), (q + "fc2.b", (E,))]
     out += [("v.merger.ln.w", (E,)), ("v.merger.ln.b", (E,)), ("v.merger.fc1.w", (mg, mg)), ("v.merger.fc1.b", (mg,)),
             ("v.merger.fc2.w", (c.v_out, mg)), ("v.merger.fc2.b", (c.v_out,))]
-    out += [("lm.embed", (c.vocab, H)), ("lm.norm", (H,))]
-    if not c.tie_embeddings:
-        out.append(("lm.head", (c.vocab, H)))
-    for i in range(c.n_layers):
-        q = f"lm.{i}."
-        out += [(q + "ln1", (H,)), (q + "ln2", (H,)), (q + "wqkv", (QKV, H)), (q + "bqkv", (QKV,)),
-                (q + "wo", (H, c.n_heads * c.head_dim)), (q + "wgu", (2 * I, H)), (q + "wd", (H, I))]
-    return out
+    return out + decoder_manifest(c, qk_norm)
 
 
-class WeightArena:
-    """ONE device buffer for all weights of a replica (views at 256-byte aligned offsets): the
-    multi-GPU start-up is then a single NCCL broadcast of `flat` (parallel.broadcast_packed)."""
+class Model(EngineModel):
+    LanguageModel = LanguageModel
+    VisionModel = VisionModel
+    qkv_bias = True
+    mrope = True
+    forward_kwargs = True
+    builtin_tower = True      # Qwen2.5-VL and Qwen3-VL run a decoder-only engine: their towers are their own
 
-    def __init__(self, manifest, device):
-        self.offsets = {}
-        off = 0
-        for name, shape in manifest:
-            n = int(np.prod(shape))
-            self.offsets[name] = (off, shape)
-            off += (n + 127) // 128 * 128
-        self.flat = torch.empty(off, dtype=torch.bfloat16, device=device)
-
-    def view(self, name: str) -> torch.Tensor:
-        off, shape = self.offsets[name]
-        return self.flat[off:off + int(np.prod(shape))].view(*shape)
-
-
-class Model:
     def __init__(self, config: ModelConfig, device=None):
-        self.config = config
-        self._device = torch.device(device) if device is not None else torch.device("cuda", 0)
-        self._eng: Optional[Engine] = None
-        self.vision_tower = VisionModel(config.vision_config, self._engine)
-        self.language_model = LanguageModel(config.text_config, config, self._engine)
+        super().__init__(config, device)
+        self.vision_tower = self.VisionModel(config.vision_config, self._engine) if self.VisionModel else None
 
     # ------------------------------------------------------------- engine
     def native_config(self) -> N.Qwen2VLConfig:
-        t, v = self.config.text_config, self.config.vision_config
-        c = N.Qwen2VLConfig()
-        c.hidden, c.n_layers, c.inter = t.hidden_size, t.num_hidden_layers, t.intermediate_size
-        c.n_heads, c.n_kv_heads = t.num_attention_heads, t.num_key_value_heads
-        c.head_dim = t.hidden_size // t.num_attention_heads
-        c.vocab = t.vocab_size
-        c.rms_eps, c.rope_theta = t.rms_norm_eps, t.rope_theta
-        sec = t.mrope_section
-        c.mrope_section[0], c.mrope_section[1], c.mrope_section[2] = sec[0], sec[1], sec[2]
-        c.tie_embeddings = int(t.tie_word_embeddings)
-        c.v_depth, c.v_embed, c.v_heads = v.depth, v.embed_dim, v.num_heads
-        c.v_mlp = int(v.embed_dim * v.mlp_ratio)
-        c.v_patch_dim = v.in_channels * v.temporal_patch_size * v.patch_size * v.patch_size
-        c.v_merge, c.v_out, c.v_ln_eps = v.spatial_merge_size, v.hidden_size, v.layer_norm_eps
+        c = super().native_config()
+        if self.builtin_tower:
+            v = self.config.vision_config
+            c.external_vision = 0
+            c.v_depth, c.v_embed, c.v_heads = v.depth, v.embed_dim, v.num_heads
+            c.v_mlp = int(v.embed_dim * v.mlp_ratio)
+            c.v_patch_dim = v.in_channels * v.temporal_patch_size * v.patch_size * v.patch_size
+            c.v_merge, c.v_out, c.v_ln_eps = v.spatial_merge_size, v.hidden_size, v.layer_norm_eps
         return c
 
-    def _engine(self) -> Engine:
-        if self._eng is None:
-            self._eng = Engine(self.native_config(), self._device)
-        return self._eng
-
-    def _arena(self) -> WeightArena:
-        if getattr(self, "_weights", None) is None:
-            self._weights = WeightArena(weight_manifest(self.native_config()), self._engine().device)
-        return self._weights
-
-    @property
-    def packed_weights(self) -> torch.Tensor:
-        """the flat device buffer every engine weight is a view of"""
-        return self._arena().flat
-
-    def _put(self, name: str, value: torch.Tensor):
-        """copy `value` into the arena view of `name` (bf16) and register it with the engine"""
-        v = self._arena().view(name)
-        v.copy_(value.reshape(v.shape).to(device=v.device, dtype=torch.bfloat16))
-        self._engine().set_weight(name, v)
-
-    @property
-    def engine(self) -> Engine:
-        return self._engine()
+    def _manifest(self):
+        return weight_manifest(self.native_config(), self.qk_norm)
 
     # ------------------------------------------------------------ weights
     def sanitize(self, weights):
@@ -154,25 +81,18 @@ class Model:
             renamed[name] = value
         return renamed
 
-    def load_weights(self, weights: Dict[str, torch.Tensor], strict: bool = True):
-        """Pack reference-named tensors into the engine layout (bf16, device):
-        q/k/v rows fused into wqkv, gate/up rows into wgu (DESIGN.md §layout)."""
-        eng = self._engine()
-        t, v = self.config.text_config, self.config.vision_config
-        dev = eng.device
-
-        def dv(x):
-            return x.to(device=dev, dtype=torch.bfloat16).contiguous()
+    def _load_vision(self, weights: Dict[str, torch.Tensor]):
+        """the built-in tower's and the merger's tensors, packed into the engine layout"""
+        v = self.config.vision_config
 
         def get(name):
-            if name not in weights:
+            if name not in w:
                 raise KeyError(f"missing weight {name}")
-            return weights[name]
+            return w[name]
 
         w = self.vision_tower.sanitize({k: x for k, x in weights.items() if "vision_tower" in k})
-        E = v.embed_dim
         put = self._put
-        put("v.patch_embed.w", w["vision_tower.patch_embed.proj.weight"].reshape(E, -1))
+        put("v.patch_embed.w", get("vision_tower.patch_embed.proj.weight").reshape(v.embed_dim, -1))
         for i in range(v.depth):
             p, q = f"vision_tower.blocks.{i}.", f"v.blk.{i}."
             for a, b in (("norm1.weight", "ln1.w"), ("norm1.bias", "ln1.b"), ("norm2.weight", "ln2.w"),
@@ -184,48 +104,25 @@ class Model:
         for a, b in (("ln_q.weight", "ln.w"), ("ln_q.bias", "ln.b"), ("mlp.0.weight", "fc1.w"),
                      ("mlp.0.bias", "fc1.b"), ("mlp.2.weight", "fc2.w"), ("mlp.2.bias", "fc2.b")):
             put("v.merger." + b, get("vision_tower.merger." + a))
-        put("lm.embed", get("language_model.model.embed_tokens.weight"))
-        put("lm.norm", get("language_model.model.norm.weight"))
-        if not t.tie_word_embeddings:
-            put("lm.head", get("language_model.lm_head.weight"))
-        for i in range(t.num_hidden_layers):
-            p, q = f"language_model.model.layers.{i}.", f"lm.{i}."
-            put(q + "ln1", get(p + "input_layernorm.weight"))
-            put(q + "ln2", get(p + "post_attention_layernorm.weight"))
-            put(q + "wqkv", torch.cat([get(p + f"self_attn.{n}_proj.weight").to(dev) for n in "qkv"], 0))
-            put(q + "bqkv", torch.cat([get(p + f"self_attn.{n}_proj.bias").to(dev) for n in "qkv"], 0))
-            put(q + "wo", get(p + "self_attn.o_proj.weight"))
-            put(q + "wgu", torch.cat([get(p + "mlp.gate_proj.weight").to(dev), get(p + "mlp.up_proj.weight").to(dev)], 0))
-            put(q + "wd", get(p + "mlp.down_proj.weight"))
-        torch.cuda.synchronize(dev)
 
     def init_random(self, seed: int = 0, std: float = 0.02):
-        """Seeded random-init at the configured shapes, generated on the device
-        (benchmark weights; SURVEY §8d: N(0, 0.02), norm weights 1, norm biases 0)."""
+        """Seeded random-init at the configured shapes, generated on the device in arena order
+        (benchmark weights; SURVEY §8d: N(0, 0.02), norm weights 1, norm biases 0).  A family without the
+        built-in tower loads its reference-named `random_weights` instead."""
+        if not self.builtin_tower:
+            return super().init_random(seed, std)
         eng = self._engine()
-        t, v = self.config.text_config, self.config.vision_config
         g = torch.Generator(device=eng.device).manual_seed(seed)
-
-        def rnd(*shape):
-            return (torch.randn(shape, generator=g, device=eng.device, dtype=torch.float32) * std
-                    ).to(torch.bfloat16)
-
-        def ones(n):
-            return torch.ones(n, device=eng.device, dtype=torch.bfloat16)
-
-        def zeros(n):
-            return torch.zeros(n, device=eng.device, dtype=torch.bfloat16)
-
-        c = self.native_config()
         arena = self._arena()
-        for name, shape in weight_manifest(c):
+        for name, shape in self._manifest():
             v = arena.view(name)
             if name.endswith(("ln1.w", "ln2.w", "ln.w", ".ln1", ".ln2", "lm.norm")):
                 v.fill_(1.0)              # norm weights 1
             elif name.endswith(("ln1.b", "ln2.b", "ln.b")):
                 v.zero_()                 # norm biases 0
             else:
-                v.copy_(rnd(*shape))
+                v.copy_((torch.randn(shape, generator=g, device=eng.device, dtype=torch.float32) * std
+                         ).to(torch.bfloat16))
             eng.set_weight(name, v)
         torch.cuda.synchronize(eng.device)
         return self
@@ -286,31 +183,6 @@ class Model:
         if eng is None:
             raise N.B200Error("merge_input_ids_with_image_features needs the model's engine "
                               "(call it through Model.get_input_embeddings or pass _engine=)")
-        H = int(image_features.shape[-1])
-        out = eng.empty((B, T, H))
-        feats = image_features.contiguous()
-        if inputs_embeds is None:
-            ids_dev = _ids_to_device(eng, ids)
-            N.check(eng.lib.b200_embed_merge(
-                ids_dev.data_ptr(), B, T, eng.weights["lm.embed"].data_ptr(), H, feats.data_ptr(),
-                n_feats, int(image_token_id), int(video_token_id), out.data_ptr(), 0, eng.s),
-                "embed_merge")
-            return out
-        # pre-computed embeddings: use them as the lookup table (row index = b*T + t)
-        sent = B * T
-        ids2 = np.where(mask, sent, np.arange(B * T).reshape(B, T))
-        ids_dev = _ids_to_device(eng, ids2)
-        table = inputs_embeds.reshape(B * T, H).contiguous()
-        N.check(eng.lib.b200_embed_merge(ids_dev.data_ptr(), B, T, table.data_ptr(), H,
-                                         feats.data_ptr(), n_feats, sent, sent, out.data_ptr(), 0,
-                                         eng.s), "embed_merge")
-        return out
-
-    @property
-    def layers(self):
-        return self.language_model.layers
-
-    def __call__(self, input_ids, pixel_values=None, mask=None, cache=None, **kwargs):
-        feats = self.get_input_embeddings(input_ids, pixel_values, **kwargs)
-        kwargs = {"pixel_values": pixel_values, **kwargs}
-        return self.language_model(input_ids, feats.inputs_embeds, mask=mask, cache=cache, **kwargs)
+        if inputs_embeds is None:       # the fused lookup: either token id takes a feature row
+            return embed_merge(eng, ids, image_features, n_feats, image_token_id, video_token_id)
+        return embed_merge(eng, ids, image_features, n_feats, inputs_embeds=inputs_embeds, rows=mask)

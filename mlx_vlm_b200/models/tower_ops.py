@@ -128,3 +128,52 @@ class TowerOps:
         E = patch.shape[1]
         N.check(self.lib.b200_tower_embed(patch.data_ptr(), N.ptr(cls), pos.data_ptr(), N.ptr(pos_ids), emb.data_ptr(),
                                           B, P, E, pos.shape[0], self.eng.s), "tower_embed")
+
+
+# ---------------------------------------------------------------- the CLIP / SigLIP encoder of LLaVA and Idefics
+def sanitize(weights, num_channels: int):
+    """reference clip / siglip `sanitize`: `position_ids` buffers are dropped and a PyTorch patch conv
+    [O, C, kH, kW] becomes channels-last [O, kH, kW, C]"""
+    out = {}
+    for k, v in weights.items():
+        if "position_ids" in k:
+            continue
+        if "patch_embedding.weight" in k and v.ndim == 4 and v.shape[1] == num_channels and v.shape[-1] != num_channels:
+            v = v.permute(0, 2, 3, 1)
+        out[k] = v
+    return out
+
+
+def pack_encoder_layers(weights, prefix: str, n_layers: int, put):
+    """`{prefix}encoder.layers.{i}.*` -> the tower weights `{i}.*` (q/k/v rows and biases fused) through `put`"""
+    for i in range(n_layers):
+        q = prefix + f"encoder.layers.{i}."
+        put(f"{i}.ln1.w", weights[q + "layer_norm1.weight"]); put(f"{i}.ln1.b", weights[q + "layer_norm1.bias"])
+        put(f"{i}.ln2.w", weights[q + "layer_norm2.weight"]); put(f"{i}.ln2.b", weights[q + "layer_norm2.bias"])
+        put(f"{i}.qkv.w", torch.cat([weights[q + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0))
+        put(f"{i}.qkv.b", torch.cat([weights[q + f"self_attn.{n}_proj.bias"] for n in "qkv"], 0))
+        put(f"{i}.out.w", weights[q + "self_attn.out_proj.weight"]); put(f"{i}.out.b", weights[q + "self_attn.out_proj.bias"])
+        put(f"{i}.fc1.w", weights[q + "mlp.fc1.weight"]); put(f"{i}.fc1.b", weights[q + "mlp.fc1.bias"])
+        put(f"{i}.fc2.w", weights[q + "mlp.fc2.weight"]); put(f"{i}.fc2.b", weights[q + "mlp.fc2.bias"])
+
+
+def encoder(ops: TowerOps, w, h: torch.Tensor, n_layers: int, *, n_heads: int, inter: int, seg: int, eps: float,
+            epi: int):
+    """encoder layers 0 .. n_layers - 1, in place on the fp32 residual stream h (T, E) of T / seg images of seg tokens
+    each: LN -> qkv -> attention inside each image -> out + residual -> LN -> fc1 with the activation epilogue `epi`
+    -> fc2 + residual"""
+    eng = ops.eng
+    T, E = h.shape
+    hd = E // n_heads
+    y, o, mlp = SplitBuf(eng, T, E), SplitBuf(eng, T, E), SplitBuf(eng, T, inter)
+    qkv = ops.f32(T, 3 * E)
+    for i in range(n_layers):
+        ops.layer_norm(h, w[f"{i}.ln1.w"], w[f"{i}.ln1.b"], eps, out_split=y)
+        ops.linear(y, w[f"{i}.qkv.w"], w[f"{i}.qkv.b"], out32=qkv)
+        ops.attention((qkv, 3 * E, hd), (qkv[:, E:], 3 * E, hd), (qkv[:, 2 * E:], 3 * E, hd), n_heads=n_heads,
+                      n_kv=n_heads, hd=hd, Lq=seg, S=seg, n_seg=T // seg, q_seg=seg, k_seg=seg, scale=hd ** -0.5,
+                      out_split=o)
+        ops.linear(o, w[f"{i}.out.w"], w[f"{i}.out.b"], out32=h, res32=h)
+        ops.layer_norm(h, w[f"{i}.ln2.w"], w[f"{i}.ln2.b"], eps, out_split=y)
+        ops.linear(y, w[f"{i}.fc1.w"], w[f"{i}.fc1.b"], out_split=mlp, epi=epi)
+        ops.linear(mlp, w[f"{i}.fc2.w"], w[f"{i}.fc2.b"], out32=h, res32=h)
