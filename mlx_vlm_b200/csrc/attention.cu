@@ -154,11 +154,8 @@ int attention(const void* q, long q_ts, long q_hs, const void* k, long k_ts, lon
   B200_REQUIRE(!causal || S >= Lq, "attention: causal needs S >= Lq");
   const size_t smem = (size_t)ATT_QT * hd * 4 + (size_t)ATT_QT * S * 2;
   B200_REQUIRE(smem <= 220 * 1024, "attention: S=%d too long for the two-pass kernel", S);
-  static size_t max_set = 48 * 1024;
-  if (smem > max_set) {
-    B200_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)(220 * 1024)));
-    max_set = 220 * 1024;
+  if (smem > 48 * 1024) {
+    if (int rc = kernel_opt_in((const void*)attention_kernel, 220 * 1024, false)) return rc;
   }
   AttnParams p;
   p.q = (const bf16*)q; p.k = (const bf16*)k; p.v = (const bf16*)v; p.out = (bf16*)out;

@@ -39,55 +39,11 @@ struct FaBars {
   uint64_t q_full, k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
-__device__ __forceinline__ uint32_t f_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void f_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(f_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void f_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(f_u32(bar)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void f_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(f_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void f_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  const uint32_t addr = f_u32(bar);
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void f_tma_3d(void* dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1,
-                                         int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(f_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(c2), "r"(f_u32(bar))
-      : "memory");
-}
 // 2^x on the SFU (one MUFU instruction, rel. error 2^-22: far below the bf16 rounding of p that follows)
 __device__ __forceinline__ float f_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// row max / sum over the 4 threads of a quad (they hold the same accumulator rows)
-__device__ __forceinline__ float f_quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float f_quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 __global__ void __launch_bounds__(FA_THREADS, 1)
@@ -116,40 +72,40 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int kbq = (p.hdp + 63) >> 6;         // 64-column blocks of the head dimension
   const int vblk = p.hdp * 128;              // bytes of one 64-key block of a V^T tile
 
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_launch_dependents();
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmQ)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmK)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmV)) : "memory");
-    f_init(&bars.q_full, 1);
+    mbar_init(&bars.q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      f_init(&bars.k_full[i], 1);
-      f_init(&bars.k_empty[i], 8);   // one arrival per consumer warp
-      f_init(&bars.v_full[i], 1);
-      f_init(&bars.v_empty[i], 8);
+      mbar_init(&bars.k_full[i], 1);
+      mbar_init(&bars.k_empty[i], 8);   // one arrival per consumer warp
+      mbar_init(&bars.v_full[i], 1);
+      mbar_init(&bars.v_empty[i], 8);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
   }
   __syncthreads();
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pdl_wait();
 
   if (wg == 0) {
     if (threadIdx.x == 0) {  // ===== TMA producer =====
-      f_expect_tx(&bars.q_full, (uint32_t)kbq * FA_BLK);
-      for (int c = 0; c < kbq; ++c) f_tma_3d(Qs + c * FA_BLK, &tmQ, &bars.q_full, c * 64, h, p.q0 + row0);
+      mbar_expect_tx(&bars.q_full, (uint32_t)kbq * FA_BLK);
+      for (int c = 0; c < kbq; ++c) tma_3d(Qs + c * FA_BLK, &tmQ, &bars.q_full, c * 64, h, p.q0 + row0);
       for (int i = 0; i < 2 * n_tiles; ++i) {
         const int j = i % n_tiles, s = i & 1;
-        f_wait(&bars.k_empty[s], ((i >> 1) & 1) ^ 1);
-        f_expect_tx(&bars.k_full[s], (uint32_t)kbq * FA_BLK);
+        mbar_wait(&bars.k_empty[s], ((i >> 1) & 1) ^ 1);
+        mbar_expect_tx(&bars.k_full[s], (uint32_t)kbq * FA_BLK);
         for (int c = 0; c < kbq; ++c)
-          f_tma_3d(Ks + s * 2 * FA_BLK + c * FA_BLK, &tmK, &bars.k_full[s], c * 64, kvh, p.k0 + j * FA_TK);
+          tma_3d(Ks + s * 2 * FA_BLK + c * FA_BLK, &tmK, &bars.k_full[s], c * 64, kvh, p.k0 + j * FA_TK);
         if (i >= n_tiles) {
           const int sv = j & 1;
-          f_wait(&bars.v_empty[sv], ((j >> 1) & 1) ^ 1);
-          f_expect_tx(&bars.v_full[sv], 2u * (uint32_t)vblk);
+          mbar_wait(&bars.v_empty[sv], ((j >> 1) & 1) ^ 1);
+          mbar_expect_tx(&bars.v_full[sv], 2u * (uint32_t)vblk);
           for (int c = 0; c < 2; ++c)
-            f_tma_3d(Vs + sv * 2 * FA_BLK + c * vblk, &tmV, &bars.v_full[sv], p.k0 + j * FA_TK + c * 64, 0, kvh);
+            tma_3d(Vs + sv * 2 * FA_BLK + c * vblk, &tmV, &bars.v_full[sv], p.k0 + j * FA_TK + c * 64, 0, kvh);
         }
       }
     }
@@ -168,13 +124,13 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   const int col0 = 2 * (lane & 3);
   constexpr float LOG2E = 1.4426950408889634f;
-  const uint32_t q_a = wg_smem(Qs) + c * 64 * 128;
+  const uint32_t q_a = smem_u32(Qs) + c * 64 * 128;
   const int ksteps = p.hdp >> 4;
   float sacc[64];
   // S = Qs . K^T of the tile in ring slot s (M64 x N128 per warpgroup), then the slot is released
   auto scores = [&](int s, uint32_t par) {
-    f_wait(&bars.k_full[s], par);
-    const uint32_t k_a = wg_smem(Ks + s * 2 * FA_BLK);
+    mbar_wait(&bars.k_full[s], par);
+    const uint32_t k_a = smem_u32(Ks + s * 2 * FA_BLK);
     wg_fence_acc(sacc);
     wg_arrive();
     for (int ks = 0; ks < ksteps; ++ks) {
@@ -185,9 +141,9 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     wg_wait<0>();
     wg_fence_acc(sacc);
     __syncwarp();
-    if (lane == 0) f_arrive(&bars.k_empty[s]);
+    if (lane == 0) mbar_arrive(&bars.k_empty[s]);
   };
-  f_wait(&bars.q_full, 0);
+  mbar_wait(&bars.q_full, 0);
   // The softmax is the instruction-bound part: the inner loops are kept to a few instructions per element
   // (bf16 rounding, one FMA into the exponent, ex2 on the SFU, multiplication by 1/l).
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
@@ -207,7 +163,7 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           cm = fmaxf(cm, v);
         }
       }
-      cm = f_quad_max(cm);
+      cm = quad_max(cm);
       if (cm > -INFINITY) {
         const float mn = fmaxf(m[hr], cm);
         const float nb = -mn * LOG2E;
@@ -222,7 +178,7 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   float inv_l[2], nbm[2];
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
-    inv_l[hr] = 1.0f / f_quad_sum(l[hr]);
+    inv_l[hr] = 1.0f / quad_sum(l[hr]);
     nbm[hr] = -m[hr] * LOG2E;
   }
   float oacc[8][8];
@@ -251,8 +207,8 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       }
     }
     const int sv = j & 1;
-    f_wait(&bars.v_full[sv], (j >> 1) & 1);
-    const uint32_t v_a = wg_smem(Vs + sv * 2 * FA_BLK);
+    mbar_wait(&bars.v_full[sv], (j >> 1) & 1);
+    const uint32_t v_a = smem_u32(Vs + sv * 2 * FA_BLK);
 #pragma unroll
     for (int ch = 0; ch < 8; ++ch) wg_fence_acc(oacc[ch]);
     wg_arrive();
@@ -268,7 +224,7 @@ attention_fa_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 #pragma unroll
     for (int ch = 0; ch < 8; ++ch) wg_fence_acc(oacc[ch]);
     __syncwarp();
-    if (lane == 0) f_arrive(&bars.v_empty[sv]);
+    if (lane == 0) mbar_arrive(&bars.v_empty[sv]);
   }
   // ---- epilogue: O -> bf16 -> global, two columns per store ----
 #pragma unroll
@@ -327,29 +283,14 @@ int attention_fa(const void* q, long q_ts, long q_hs, const void* k, long k_ts, 
   if ((rc = fa_tmap3(q, hd, n_heads, q_hs, q_tot, q_ts, 64, 1, FA_TQ, &tq))) return rc;
   if ((rc = fa_tmap3(k, hd, n_kv, k_hs, k_tot, k_ts, 64, 1, FA_TK, &tk))) return rc;
   if ((rc = fa_tmap3(vt, k_tot, hd, vt_ds, n_kv, vt_hs, 64, hdp, 1, &tv))) return rc;
-  static unsigned long long set_mask = 0ull;
-  int dev = 0;
-  B200_CUDA(cudaGetDevice(&dev));
   const size_t smem = 10 * FA_BLK + 1024;
-  if (!(set_mask >> (dev & 63) & 1ull)) {
-    B200_CUDA(cudaFuncSetAttribute(attention_fa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    set_mask |= 1ull << (dev & 63);
-  }
+  if ((rc = kernel_opt_in((const void*)attention_fa_kernel, (int)smem, false))) return rc;
   FaParams p;
   p.out = (bf16*)out; p.o_ts = o_ts; p.n_heads = n_heads; p.n_kv = n_kv; p.hd = hd; p.hdp = hdp;
   p.Lq = Lq; p.S = S; p.causal = causal; p.q0 = q0; p.k0 = k0;
   p.segs = (const int4*)segs;
-  cudaLaunchConfig_t lc = {};
-  lc.gridDim = dim3(cdiv(Lq, FA_TQ), n_heads, segs ? n_seg : 1);
-  lc.blockDim = dim3(FA_THREADS);
-  lc.dynamicSmemBytes = smem;
-  lc.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = at;
-  lc.numAttrs = 1;
-  B200_CUDA(cudaLaunchKernelEx(&lc, attention_fa_kernel, tq, tk, tv, p));
+  B200_CUDA(launch(attention_fa_kernel, dim3(cdiv(Lq, FA_TQ), n_heads, segs ? n_seg : 1), dim3(FA_THREADS), smem, st,
+                   PDL_LAUNCH, tq, tk, tv, p));
   return B200_OK;
 }
 

@@ -34,18 +34,6 @@ struct AttnTcParams {
   float scale_bf;
 };
 
-__device__ __forceinline__ void a_fence_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ float a_quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
-__device__ __forceinline__ float a_quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-
 // byte offset of element (row r, column c) of a [128 x 128] bf16 operand stored as two
 // 64-column blocks, each 128 rows x 128 B with the 128-byte swizzle
 __device__ __forceinline__ uint32_t sw_off(int r, int c) {
@@ -153,7 +141,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const Attn
   const int vis_tile = p.causal ? min(S, S - p.Lq + q_last + 1) : S;
   const int n_tiles = (vis_tile + TK - 1) / TK;
 
-  const uint32_t q_a = wg_smem(Qs) + wg * 64 * 128, k_a = wg_smem(Ks), v_a = wg_smem(Vt);
+  const uint32_t q_a = smem_u32(Qs) + wg * 64 * 128, k_a = smem_u32(Ks), v_a = smem_u32(Vt);
   const int ksteps = hd >> 4;  // 16 dims per MMA
   float sacc[64];
   auto scores = [&]() {
@@ -174,7 +162,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const Attn
   for (int jt = 0; jt < n_tiles; ++jt) {
     if (jt > 0) __syncthreads();  // every warpgroup's MMAs have read the previous K tile
     stage_rows<false>(Ks, kb, p.k_ts, jt * TK, S, hd, 0.f);
-    a_fence_async();
+    fence_proxy_async();
     __syncthreads();
     scores();
     const int jbase = jt * TK + col0;
@@ -191,7 +179,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const Attn
           cm = fmaxf(cm, v);
         }
       }
-      cm = a_quad_max(cm);
+      cm = quad_max(cm);
       if (cm > -INFINITY) {
         const float mn = fmaxf(m[hr], cm);
         float add = 0.f;
@@ -204,7 +192,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const Attn
     }
   }
 #pragma unroll
-  for (int hr = 0; hr < 2; ++hr) l[hr] = a_quad_sum(l[hr]);
+  for (int hr = 0; hr < 2; ++hr) l[hr] = quad_sum(l[hr]);
 
   // ---------------- pass 2: p = bf16(exp(s - m) / l), O += P . V ----------------
   float oacc[8][8];
@@ -217,7 +205,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attention_tc_kernel(const Attn
     __syncthreads();  // the previous tile's MMAs have read Ks / Vt
     stage_rows<false>(Ks, kb, p.k_ts, jt * TK, S, hd, 0.f);
     stage_vt(Vt, vb, p.v_ts, jt * TK, S, hd);
-    a_fence_async();
+    fence_proxy_async();
     __syncthreads();
     scores();
     const int jbase = jt * TK + col0;
@@ -280,12 +268,8 @@ bool attention_tc_supported(const void* q, long q_ts, long q_hs, const void* k, 
 int attention_tc(const void* q, long q_ts, long q_hs, const void* k, long k_ts, long k_hs,
                  const void* v, long v_ts, long v_hs, void* out, long o_ts, int n_heads, int n_kv,
                  int hd, int Lq, int S, int causal, float scale, cudaStream_t st) {
-  static unsigned long long set_mask = 0ull;
   const size_t smem = 6 * KBLK + 1024;
-  if (first_use_on_device(&set_mask)) {
-    B200_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)smem));
-  }
+  if (int rc = kernel_opt_in((const void*)attention_tc_kernel, (int)smem, false)) return rc;
   AttnTcParams p;
   p.q = (const bf16*)q; p.k = (const bf16*)k; p.v = (const bf16*)v; p.out = (bf16*)out;
   p.q_ts = q_ts; p.q_hs = q_hs; p.k_ts = k_ts; p.k_hs = k_hs; p.v_ts = v_ts; p.v_hs = v_hs;

@@ -133,40 +133,162 @@ __device__ __forceinline__ float gelu_exact_bf(float x) {
   return rbf(d * 0.5f);
 }
 
-inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
-
-// per-DEVICE one-time setup (cudaFuncSetAttribute is per device): true the first time the current device asks
-inline bool first_use_on_device(unsigned long long* mask) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return true;
-  const unsigned long long bit = 1ull << (dev & 63);
-  if (*mask & bit) return false;
-  *mask |= bit;
-  return true;
+// sum over a block of NWARPS warps through red[NWARPS]; every thread gets the total
+template <int NWARPS>
+__device__ __forceinline__ float block_sum(float v, float* red) {
+  v = warp_sum(v);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float t = 0.f;
+#pragma unroll
+  for (int w = 0; w < NWARPS; ++w) t += red[w];
+  return t;
+}
+// the same for a warp count known at run time only
+__device__ __forceinline__ float block_sum(float v, float* red, int nwarps) {
+  v = warp_sum(v);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float t = 0.f;
+  for (int w = 0; w < nwarps; ++w) t += red[w];
+  return t;
 }
 
+// float -> u32 whose unsigned order is the float order (the high half of a packed argmax key)
+__device__ __forceinline__ uint32_t orderable(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// ---- Hopper asynchronous copies: mbarrier, 1-D bulk copy, proxy fence ------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
+               "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ uint32_t mbar_try_wait(uint32_t addr, uint32_t parity) {
+  uint32_t done;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(done)
+      : "r"(addr), "r"(parity)
+      : "memory");
+  return done;
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  const uint32_t addr = smem_u32(bar);
+  uint32_t done;
+  do {
+    done = mbar_try_wait(addr, parity);
+  } while (!done);
+}
+// bounded wait (k_mega): a scheduling bug must not hang the GPU (sets *err = 2 and falls through)
+__device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity, int* err) {
+  uint32_t done;
+  const uint32_t addr = smem_u32(bar);
+  unsigned spins = 0;
+  do {
+    done = mbar_try_wait(addr, parity);
+    if (!done && ++spins > (1u << 20)) {
+      *err = 2;
+      break;
+    }
+  } while (!done);
+}
+// 1-D bulk copy global -> shared through the TMA engine, completing on `bar`, with an L2 cache policy
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar,
+                                         uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+__device__ __forceinline__ uint64_t policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// shared-memory writes of the generic proxy (ordinary stores, mbarrier init) become visible to the async proxy
+// (TMA, wgmma operands)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
+
+// 1-D grid for `work` items of `block` threads each, capped at 16 CTAs per SM of the H100 (grid-stride kernels)
+inline int grid_for(long work, int block) {
+  long g = (work + block - 1) / block;
+  if (g > 132L * 16) g = 132L * 16;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+
+// Function attributes are per (kernel, device).  Raises the kernel's dynamic shared-memory limit to max_dyn_smem
+// (when > 0) and asks for the maximum shared-memory carve-out (when max_carveout) on the current device; a value
+// already set for this kernel on this device is not set again, so callers may ask before every launch.
+int kernel_opt_in(const void* kern, int max_dyn_smem, bool max_carveout);
+
 // ---- programmatic dependent launch -------------------------------------------------
+__device__ __forceinline__ void pdl_launch_dependents() {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // Every kernel of the prefill / vision / batched-decode sequences starts with pdl_prologue():
 // it lets the NEXT kernel of the stream begin (its barrier set-up and the prefetch of its
 // weights overlap this kernel) and then waits until everything the PREVIOUS kernels wrote is visible.
 __device__ __forceinline__ void pdl_prologue() {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pdl_launch_dependents();
+  pdl_wait();
 }
+
+// ---- launches with attributes ----------------------------------------------------------------
+struct LaunchOpts {
+  bool pdl;          // programmatic stream serialization: the kernel may start before the previous one ends
+  int cluster_x;     // > 0: thread-block clusters of cluster_x x 1 x 1 CTAs
+  bool cooperative;  // every CTA resident at once (or the launch fails)
+};
+constexpr LaunchOpts PDL_LAUNCH = {true, 0, false};
+
 #ifdef __CUDACC__
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
-                              Args... args) {
+inline cudaError_t launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+                          LaunchOpts opts, Args... args) {
+  cudaLaunchAttribute at[3];
+  unsigned n = 0;
+  if (opts.pdl) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (opts.cluster_x > 0) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n++].val.clusterDim = {(unsigned)opts.cluster_x, 1, 1};
+  }
+  if (opts.cooperative) {
+    at[n].id = cudaLaunchAttributeCooperative;
+    at[n++].val.cooperative = 1;
+  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 #endif

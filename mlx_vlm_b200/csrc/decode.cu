@@ -35,54 +35,8 @@ namespace b200 {
 // ---------------------------------------------------------------------------
 // helpers
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void pdl_launch_dependents() {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 __device__ __forceinline__ uint4 ldg16(const void* p) {
   return *reinterpret_cast<const uint4*>(p);
-}
-__device__ __forceinline__ uint32_t s_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mb_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mb_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s_u32(bar)),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mb_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mb_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  const uint32_t addr = s_u32(bar);
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-// 1-D bulk copy global -> shared through the TMA engine, evict-first in L2
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar,
-                                         uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1], %2, [%3], %4;" ::"r"(s_u32(dst)),
-      "l"(src), "r"(bytes), "r"(s_u32(bar)), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ uint64_t policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
 }
 
 // ---------------------------------------------------------------------------
@@ -150,11 +104,11 @@ __global__ void __launch_bounds__(STREAM_THREADS, 2) k_stream(const StreamP p) {
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.n_stages; ++s) {
-      mb_init(&full_bar[s], 1);
-      mb_init(&empty_bar[s], 8);
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
   }
   __syncthreads();
   const int my_tiles = (p.tiles > (int)blockIdx.x)
@@ -169,11 +123,11 @@ __global__ void __launch_bounds__(STREAM_THREADS, 2) k_stream(const StreamP p) {
         const int t = blockIdx.x + it * gridDim.x;
         const int s = it % p.n_stages;
         const uint32_t ph = (it / p.n_stages) & 1;
-        mb_wait(&empty_bar[s], ph ^ 1);
+        mbar_wait(&empty_bar[s], ph ^ 1);
         int rows = p.R;
         if (MODE != SM_QKV) rows = min(p.R, p.N - t * p.R);
         const uint32_t bytes = (uint32_t)rows * rows_unit;
-        mb_expect_tx(&full_bar[s], bytes * T::NRW);
+        mbar_expect_tx(&full_bar[s], bytes * T::NRW);
         uint8_t* dst = sm + (long)s * p.stage_bytes;
         bulk_g2s(dst, tile_src<MODE>(p, t, 0), bytes, &full_bar[s], pol);
         if (T::PAIR) bulk_g2s(dst + (long)p.R * rows_unit, tile_src<MODE>(p, t, 1), bytes,
@@ -248,7 +202,7 @@ __global__ void __launch_bounds__(STREAM_THREADS, 2) k_stream(const StreamP p) {
     const uint32_t ph = (it / p.n_stages) & 1;
     int rows = p.R;
     if (MODE != SM_QKV) rows = min(p.R, p.N - t * p.R);
-    mb_wait(&full_bar[s], ph);
+    mbar_wait(&full_bar[s], ph);
     const uint8_t* base = sm + (long)s * p.stage_bytes + (long)rloc * rows_unit;
     float acc[T::NRW];
     {
@@ -296,7 +250,7 @@ __global__ void __launch_bounds__(STREAM_THREADS, 2) k_stream(const StreamP p) {
 #pragma unroll
     for (int m = 0; m < T::NRW; ++m) acc[m] = warp_sum(acc[m]);
     __syncwarp();
-    if (lane == 0) mb_arrive(&empty_bar[s]);  // this warp is done reading the stage
+    if (lane == 0) mbar_arrive(&empty_bar[s]);  // this warp is done reading the stage
     if (p.S > 1) {  // split-K: combine the slices of a row through shared memory
       if (lane == 0) {
 #pragma unroll
@@ -716,11 +670,6 @@ __global__ void __launch_bounds__(256) k_attn(const DecodeDims d, const bf16* __
 // k_sample: logprobs = bf16(logits - bf16(logsumexp)), greedy argmax with the
 // lowest index on ties (packed 64-bit atomicMax), last CTA finalises the step.
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t orderable(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 __global__ void __launch_bounds__(256) k_sample(const DecodeDims d,
                                                 const bf16* __restrict__ logits,
                                                 const float2* __restrict__ partials, int n_part,
@@ -836,33 +785,8 @@ static bool g_pdl = false;  // off by default; programmatic dependent launch for
 void decode_set_sm_count(int n) { g_sm_count = n > 0 ? n : 132; }
 void decode_set_pdl(bool on) { g_pdl = on; }
 
-template <typename... KArgs, typename... Args>
-static int launch_ex(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
-                     int cluster_x, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (g_pdl) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  if (cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster_x;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
-  B200_CUDA(cudaLaunchKernelEx(&cfg, kern, KArgs(args)...));
-  return B200_OK;
-}
+// launch attributes of the step's kernels: PDL when decode_set_pdl() turned it on, a cluster when cluster_x > 1
+static LaunchOpts step_opts(int cluster_x = 1) { return {g_pdl, cluster_x > 1 ? cluster_x : 0, false}; }
 
 // tile geometry: R row(-pair)s per tile (R*S == 8 consumer warps), stage <= ~50 KB
 static int stream_geometry(StreamP& p, bool pair, int units /*rows or pairs available*/) {
@@ -887,27 +811,21 @@ static int launch_stream(const StreamP& p, int max_ctas, cudaStream_t s) {
   const int chx = cdiv(cdiv(nvec, p.S), 32);
   const int grid = p.tiles < max_ctas ? p.tiles : max_ctas;
   const size_t smem = (size_t)p.n_stages * p.stage_bytes;
-  if (chx <= 2) return launch_ex(k_stream<MODE, 2>, dim3(grid), dim3(STREAM_THREADS), smem, s, 1, p);
-  if (chx <= 6) return launch_ex(k_stream<MODE, 6>, dim3(grid), dim3(STREAM_THREADS), smem, s, 1, p);
-  if (chx <= 10) return launch_ex(k_stream<MODE, 10>, dim3(grid), dim3(STREAM_THREADS), smem, s, 1, p);
-  set_error("decode: K=%d needs %d activation chunks per lane (max 10)", p.K, chx);
-  return B200_ERR_INVALID;
+  B200_REQUIRE(chx <= 10, "decode: K=%d needs %d activation chunks per lane (max 10)", p.K, chx);
+  B200_CUDA(launch(chx <= 2 ? k_stream<MODE, 2> : chx <= 6 ? k_stream<MODE, 6> : k_stream<MODE, 10>, dim3(grid),
+                   dim3(STREAM_THREADS), smem, s, step_opts(), p));
+  return B200_OK;
 }
 
 // every kernel of the decode step asks for the SAME (maximum) shared-memory carve-out:
 // a carve-out change between kernels needs an idle SM and would forbid the
 // co-residency of consecutive kernels that PDL relies on.
-template <typename F>
-static int set_carveout(F kern, int dyn_smem) {
-  if (dyn_smem > 0)
-    B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem));
-  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared));
+template <int MODE>
+static int stream_opt_in() {
+  int rc;
+  for (const void* k : {(const void*)k_stream<MODE, 2>, (const void*)k_stream<MODE, 6>, (const void*)k_stream<MODE, 10>})
+    if ((rc = kernel_opt_in(k, STREAM_SMEM_BUDGET, true))) return rc;
   return B200_OK;
-}
-template <int MODE, int CHX>
-static int set_stream_attr() {
-  return set_carveout(k_stream<MODE, CHX>, STREAM_SMEM_BUDGET);
 }
 
 static int attn_hsplit(const DecodeDims& d, int gmax) {
@@ -929,18 +847,12 @@ size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap) {
 
 int decode_prepare() {
   int rc;
-  if ((rc = set_stream_attr<SM_QKV, 2>()) || (rc = set_stream_attr<SM_QKV, 6>()) ||
-      (rc = set_stream_attr<SM_QKV, 10>()) || (rc = set_stream_attr<SM_ORES, 2>()) ||
-      (rc = set_stream_attr<SM_ORES, 6>()) || (rc = set_stream_attr<SM_ORES, 10>()) ||
-      (rc = set_stream_attr<SM_GATEUP, 2>()) || (rc = set_stream_attr<SM_GATEUP, 6>()) ||
-      (rc = set_stream_attr<SM_GATEUP, 10>()) || (rc = set_stream_attr<SM_DRES, 2>()) ||
-      (rc = set_stream_attr<SM_DRES, 6>()) || (rc = set_stream_attr<SM_DRES, 10>()) ||
-      (rc = set_stream_attr<SM_HEAD, 2>()) || (rc = set_stream_attr<SM_HEAD, 6>()) ||
-      (rc = set_stream_attr<SM_HEAD, 10>()))
+  if ((rc = stream_opt_in<SM_QKV>()) || (rc = stream_opt_in<SM_ORES>()) || (rc = stream_opt_in<SM_GATEUP>()) ||
+      (rc = stream_opt_in<SM_DRES>()) || (rc = stream_opt_in<SM_HEAD>()))
     return rc;
-  if ((rc = set_carveout(k_sample, 0)) || (rc = set_carveout(k_set_state, 0)) ||
-      (rc = set_carveout(k_qk_norm_rope<4>, 0)) || (rc = set_carveout(k_qk_norm_rope<2>, 0)))
-    return rc;
+  for (const void* k : {(const void*)k_sample, (const void*)k_set_state, (const void*)k_qk_norm_rope<4>,
+                        (const void*)k_qk_norm_rope<2>})
+    if ((rc = kernel_opt_in(k, 0, true))) return rc;
   return B200_OK;
 }
 
@@ -949,12 +861,13 @@ int attn_prepare(const DecodeDims& d, int cluster) {
   if (d.cap <= ATT1_MAX_CAP) {
     const size_t smem = attn1_smem(d);
     B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
-    if ((rc = set_carveout(k_attn1<128>, (int)smem)) || (rc = set_carveout(k_attn1<64>, (int)smem)))
+    if ((rc = kernel_opt_in((const void*)k_attn1<128>, (int)smem, true)) ||
+        (rc = kernel_opt_in((const void*)k_attn1<64>, (int)smem, true)))
       return rc;
   } else {
     const size_t smem = attn_smem_bytes(d, cdiv(d.cap, cluster));
     B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
-    if ((rc = set_carveout(k_attn, (int)smem))) return rc;
+    if ((rc = kernel_opt_in((const void*)k_attn, (int)smem, true))) return rc;
   }
   return B200_OK;
 }
@@ -975,8 +888,9 @@ int launch_qkv(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* qbuf,
   if ((rc = launch_stream<SM_QKV>(p, g_sm_count, s)) || !qn) return rc;
   B200_REQUIRE(kn && (d.hd == 64 || d.hd == 128), "decode q/k norm: head_dim=%d (64 | 128)", d.hd);
   const dim3 grid(cdiv(d.n_heads + d.n_kv, 8));
-  if (d.hd == 128) return launch_ex(k_qk_norm_rope<4>, grid, dim3(256), 0, s, 1, d, qbuf, kc, st, inv_freq, qn, kn);
-  return launch_ex(k_qk_norm_rope<2>, grid, dim3(256), 0, s, 1, d, qbuf, kc, st, inv_freq, qn, kn);
+  B200_CUDA(launch(d.hd == 128 ? k_qk_norm_rope<4> : k_qk_norm_rope<2>, grid, dim3(256), 0, s, step_opts(), d, qbuf,
+                   kc, st, inv_freq, qn, kn));
+  return B200_OK;
 }
 
 int launch_attn(const DecodeDims& d, const bf16* qbuf, const bf16* kc, const bf16* vc, bf16* out,
@@ -984,17 +898,16 @@ int launch_attn(const DecodeDims& d, const bf16* qbuf, const bf16* kc, const bf1
   B200_REQUIRE(d.hd == 64 || d.hd == 128, "decode attention: head_dim=%d (64|128)", d.hd);
   if (d.cap <= ATT1_MAX_CAP) {
     const int hs = attn_hsplit(d, ATT1_G);
-    if (d.hd == 128)
-      return launch_ex(k_attn1<128>, dim3(d.n_kv * hs), dim3(256), attn1_smem(d), s, 1, d, qbuf, kc,
-                       vc, out, st, hs);
-    return launch_ex(k_attn1<64>, dim3(d.n_kv * hs), dim3(256), attn1_smem(d), s, 1, d, qbuf, kc, vc,
-                     out, st, hs);
+    B200_CUDA(launch(d.hd == 128 ? k_attn1<128> : k_attn1<64>, dim3(d.n_kv * hs), dim3(256), attn1_smem(d), s,
+                     step_opts(), d, qbuf, kc, vc, out, st, hs));
+    return B200_OK;
   }
   const int hs = attn_hsplit(d, ATT_MAXG);
   B200_REQUIRE(cluster <= ATT_MAXCL, "decode attention: cluster %d > %d", cluster, ATT_MAXCL);
   const int chunk_cap = cdiv(d.cap, cluster);
-  return launch_ex(k_attn, dim3(cluster, d.n_kv * hs, 1), dim3(256), attn_smem_bytes(d, chunk_cap),
-                   s, cluster, d, qbuf, kc, vc, out, st, chunk_cap, hs);
+  B200_CUDA(launch(k_attn, dim3(cluster, d.n_kv * hs, 1), dim3(256), attn_smem_bytes(d, chunk_cap), s,
+                   step_opts(cluster), d, qbuf, kc, vc, out, st, chunk_cap, hs));
+  return B200_OK;
 }
 
 int launch_res(const bf16* W, const bf16* x, bf16* h, int N, int K, cudaStream_t s) {
@@ -1041,8 +954,9 @@ int launch_head(const DecodeDims& d, const bf16* norm_w, const bf16* E, const bf
 int launch_sample(const DecodeDims& d, const bf16* logits, const float2* partials, bf16* logprobs,
                   const bf16* E, bf16* h, DecState* st, int* token_log, int log_cap,
                   const int* force_tokens, int advance, cudaStream_t s) {
-  return launch_ex(k_sample, dim3(g_sm_count), dim3(256), 0, s, 1, d, logits, partials,
-                   head_ctas(d), logprobs, E, h, st, token_log, log_cap, force_tokens, advance);
+  B200_CUDA(launch(k_sample, dim3(g_sm_count), dim3(256), 0, s, step_opts(), d, logits, partials, head_ctas(d),
+                   logprobs, E, h, st, token_log, log_cap, force_tokens, advance));
+  return B200_OK;
 }
 
 int launch_set_state(DecState* st, int tok, int ctx, int pos, int use_force, int set_tok,

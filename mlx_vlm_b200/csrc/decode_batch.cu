@@ -31,20 +31,6 @@ namespace {
 
 constexpr int BD_AG_MAX = 4;  // q heads per attention CTA: 4, 2 or 1 — the smallest that keeps the grid within one wave
 
-__device__ __forceinline__ void bd_pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void bd_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-__device__ __forceinline__ float bd_block_sum(float v, float* red, int nwarps) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-  for (int w = 0; w < nwarps; ++w) t += red[w];
-  return t;
-}
-
 // h[b] = embed[tok[b]];  xn[b] = RMSNorm(h[b]) * w   (the first norm of the next step)
 __device__ __forceinline__ void bd_embed_norm_row(const bf16* __restrict__ embed, int tok, int H,
                                                   const bf16* __restrict__ lnw, float eps, bf16* h,
@@ -59,7 +45,7 @@ __device__ __forceinline__ void bd_embed_norm_row(const bf16* __restrict__ embed
 #pragma unroll
     for (int j = 0; j < 8; ++j) ss = fmaf(f[j], f[j], ss);
   }
-  const float tot = bd_block_sum(ss, red, blockDim.x >> 5);
+  const float tot = block_sum(ss, red, blockDim.x >> 5);
   const float rs = 1.0f / sqrtf(tot / (float)H + eps);
   for (int c = threadIdx.x; c < nv; c += blockDim.x) {
     float f[8], w[8];
@@ -158,7 +144,7 @@ __device__ __forceinline__ void bd_q8_val(const uint8_t* codes, const bf16* sc, 
 
 template <int HD, int AG, bool Q8>
 __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
-  bd_pdl_launch();
+  pdl_launch_dependents();
   extern __shared__ __align__(16) uint8_t bd_sm[];
   constexpr int NCH = HD / 8, half = HD / 2;
   constexpr int SEG = HD / 8;   // dims per lane in the P.V phase (lane = key sub-index x dim segment)
@@ -188,7 +174,7 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
   const bf16* kqb = Q8 ? p.q8b + plane0 / p.gs : nullptr;
   const bf16* vqs = Q8 ? kqs + p.v_off / p.gs : nullptr;
   const bf16* vqb = Q8 ? kqb + p.v_off / p.gs : nullptr;
-  bd_pdl_wait();
+  pdl_wait();
   const int ctx = p.ctx[row], pos = p.pos[row];
   const int nkeys = ctx + 1;
   // Every dependent global round trip costs ~1 us here, so the requests are issued as early as their
@@ -477,11 +463,6 @@ __global__ void __launch_bounds__(256) bd_attn_kernel(const BdAttnP p) {
 }
 
 // ---- sampler + state update + next embedding, one CTA per row ------------------------------------
-__device__ __forceinline__ uint32_t bd_orderable(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 struct BdSampleP {
   const bf16* logits;  // [B][ldv]
   bf16* logprobs;      // [B][ldv] or nullptr
@@ -498,7 +479,7 @@ struct BdSampleP {
 };
 
 __global__ void __launch_bounds__(1024) bd_sample_kernel(const BdSampleP p) {
-  bd_pdl_launch();
+  pdl_launch_dependents();
   __shared__ float red[32];
   __shared__ float2 stat[32];
   __shared__ unsigned long long keys[32];
@@ -506,7 +487,7 @@ __global__ void __launch_bounds__(1024) bd_sample_kernel(const BdSampleP p) {
   __shared__ int s_tok;
   const int b = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  bd_pdl_wait();
+  pdl_wait();
   // rows are ldv = round8(V) apart; the tail [V, ldv) holds -inf (preset once, never written)
   const bf16* lg = p.logits + (long)b * p.ldv;
   const int nv = p.ldv >> 3;
@@ -549,7 +530,7 @@ __global__ void __launch_bounds__(1024) bd_sample_kernel(const BdSampleP p) {
     for (int j = 0; j < 8; ++j) {
       o[j] = rbf(f[j] - lse);
       const unsigned long long key =
-          ((unsigned long long)bd_orderable(o[j]) << 32) | (0xFFFFFFFFu - (uint32_t)(c * 8 + j));
+          ((unsigned long long)orderable(o[j]) << 32) | (0xFFFFFFFFu - (uint32_t)(c * 8 + j));
       best = key > best ? key : best;
     }
     if (p.logprobs) {
@@ -604,7 +585,7 @@ struct BdProcsP {
 __global__ void __launch_bounds__(1024) bd_procs_kernel(const BdProcsP p) {
   __shared__ int win[BD_HIST_MAX];
   const int b = blockIdx.x, t = threadIdx.x;
-  bd_pdl_wait();
+  pdl_wait();
   const int* par = p.pr.params + b * BD_PROC_PARAMS;
   const int flags = par[0];
   if (flags == 0) return;
@@ -679,9 +660,9 @@ __global__ void __launch_bounds__(256) bd_topk_part_kernel(const bf16* __restric
   __shared__ unsigned long long red[8];
   const int s = blockIdx.x, b = blockIdx.y, S = gridDim.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  bd_pdl_wait();
+  pdl_wait();
   const int base = s * BD_TOPK_SLICE, n = min(BD_TOPK_SLICE, V - base);
-  for (int i = threadIdx.x; i < n; i += 256) key[i] = bd_orderable(bf2f(lp[(long)b * ldv + base + i]));
+  for (int i = threadIdx.x; i < n; i += 256) key[i] = orderable(bf2f(lp[(long)b * ldv + base + i]));
   __syncthreads();
   unsigned long long prev = ~0ull;
   for (int r = 0; r < k; ++r) {
@@ -711,7 +692,7 @@ __global__ void __launch_bounds__(256) bd_topk_merge_kernel(const unsigned long 
                                                             int* __restrict__ ids_log, float* __restrict__ lp_log) {
   __shared__ unsigned long long c[BD_TOPK_CAND_MAX];
   const int b = blockIdx.x, n = S * k;
-  bd_pdl_wait();
+  pdl_wait();
   for (int i = threadIdx.x; i < n; i += 256) c[i] = cand[(long)b * n + i];
   __syncthreads();
   const long at = ((long)(n_out ? (n_out[b] - 1) % log_cap : 0) * max_b + b) * BD_TOPK_MAX;   // no log: [B][20]
@@ -803,22 +784,6 @@ static int bd_alloc(BatchDecoder* d, const BdModel& m, int max_b) {
   return B200_OK;
 }
 
-template <typename... KArgs, typename... Args>
-static int bd_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  B200_CUDA(cudaLaunchKernelEx(&cfg, kern, KArgs(args)...));
-  return B200_OK;
-}
-
 static size_t bd_attn_smem(const DecodeDims& d, int ag) {
   return ((size_t)(ag + 2) * d.hd + (size_t)ag * d.cap + (size_t)8 * ag * d.hd) * 4;
 }
@@ -834,11 +799,9 @@ static int bd_attn_heads_per_cta(const DecodeDims& d, int B, int sm_count) {
 
 template <int HD, bool Q8>
 static int bd_attn_launch(int ag, dim3 grid, size_t smem, cudaStream_t s, const BdAttnP& ap) {
-  switch (ag) {
-    case 1: return bd_launch(bd_attn_kernel<HD, 1, Q8>, grid, dim3(256), smem, s, ap);
-    case 2: return bd_launch(bd_attn_kernel<HD, 2, Q8>, grid, dim3(256), smem, s, ap);
-    default: return bd_launch(bd_attn_kernel<HD, 4, Q8>, grid, dim3(256), smem, s, ap);
-  }
+  B200_CUDA(launch(ag == 1 ? bd_attn_kernel<HD, 1, Q8> : ag == 2 ? bd_attn_kernel<HD, 2, Q8> : bd_attn_kernel<HD, 4, Q8>,
+                   grid, dim3(256), smem, s, PDL_LAUNCH, ap));
+  return B200_OK;
 }
 
 static int bd_attn_dispatch(const DecodeDims& d, int ag, dim3 grid, cudaStream_t s, const BdAttnP& ap, bool q8) {
@@ -848,15 +811,14 @@ static int bd_attn_dispatch(const DecodeDims& d, int ag, dim3 grid, cudaStream_t
 }
 
 static int bd_set_smem_attrs() {
-  static unsigned long long attr_mask = 0ull;
-  if (!first_use_on_device(&attr_mask)) return B200_OK;
   const void* ks[] = {(const void*)bd_attn_kernel<128, 1, false>, (const void*)bd_attn_kernel<128, 2, false>,
                       (const void*)bd_attn_kernel<128, 4, false>, (const void*)bd_attn_kernel<64, 1, false>,
                       (const void*)bd_attn_kernel<64, 2, false>,  (const void*)bd_attn_kernel<64, 4, false>,
                       (const void*)bd_attn_kernel<128, 1, true>,  (const void*)bd_attn_kernel<128, 2, true>,
                       (const void*)bd_attn_kernel<128, 4, true>,  (const void*)bd_attn_kernel<64, 1, true>,
                       (const void*)bd_attn_kernel<64, 2, true>,   (const void*)bd_attn_kernel<64, 4, true>};
-  for (const void* k : ks) B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  for (const void* k : ks)
+    if (int rc = kernel_opt_in(k, 200 * 1024, false)) return rc;
   return B200_OK;
 }
 
@@ -912,7 +874,7 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
   if (d->procs.params) {
     BdProcsP pp;
     pp.logits = d->logits; pp.ldv = d->ldv; pp.V = dd.vocab; pp.tok = d->tok; pp.active = d->active; pp.pr = d->procs;
-    if ((rc = bd_launch(bd_procs_kernel, dim3(B), dim3(1024), 0, s, pp))) return rc;
+    B200_CUDA(launch(bd_procs_kernel, dim3(B), dim3(1024), 0, s, PDL_LAUNCH, pp));
     *launches += 1;
   }
   BdSampleP sp;
@@ -920,16 +882,14 @@ static int bd_enqueue_step(BatchDecoder* d, const BdModel& m, cudaStream_t s, lo
   sp.tok = d->tok; sp.ctx = d->ctx; sp.pos = d->pos; sp.n_out = d->n_out; sp.active = d->active;
   sp.token_log = d->token_log; sp.lp_log = d->lp_log; sp.log_cap = d->log_cap; sp.max_b = d->max_b;
   sp.embed = m.embed; sp.ln0 = m.layers[0].ln1; sp.eps = dd.eps; sp.h = d->h; sp.xn = d->xn;
-  if ((rc = bd_launch(bd_sample_kernel, dim3(B), dim3(1024), 0, s, sp))) return rc;
+  B200_CUDA(launch(bd_sample_kernel, dim3(B), dim3(1024), 0, s, PDL_LAUNCH, sp));
   *launches += 2;
   if (d->procs.top_k > 0) {  // over the logprob rows bd_sample wrote (want_logprobs is forced on)
     const int S = (dd.vocab + BD_TOPK_SLICE - 1) / BD_TOPK_SLICE, k = d->procs.top_k;
-    if ((rc = bd_launch(bd_topk_part_kernel, dim3(S, B), dim3(256), 0, s, (const bf16*)d->logprobs, d->ldv, dd.vocab,
-                        k, d->topk_cand)))
-      return rc;
-    if ((rc = bd_launch(bd_topk_merge_kernel, dim3(B), dim3(256), 0, s, (const unsigned long long*)d->topk_cand, S, k,
-                        (const int*)d->n_out, d->log_cap, d->max_b, d->topk_ids, d->topk_lp)))
-      return rc;
+    B200_CUDA(launch(bd_topk_part_kernel, dim3(S, B), dim3(256), 0, s, PDL_LAUNCH, (const bf16*)d->logprobs, d->ldv, dd.vocab,
+                        k, d->topk_cand));
+    B200_CUDA(launch(bd_topk_merge_kernel, dim3(B), dim3(256), 0, s, PDL_LAUNCH, (const unsigned long long*)d->topk_cand, S, k,
+                        (const int*)d->n_out, d->log_cap, d->max_b, d->topk_ids, d->topk_lp));
     *launches += 2;
   }
   return B200_OK;
@@ -1066,25 +1026,24 @@ int batch_procs_apply(bf16* logits, const bf16* logprobs, int B, int V, int ldv,
                       const BdProcs& pr, int* top_ids, float* top_lp, cudaStream_t s) {
   B200_REQUIRE(B >= 1 && B <= 16 && V > 0 && ldv >= V, "batch procs apply: bad arguments");
   B200_REQUIRE(pr.top_k >= 0 && pr.top_k <= BD_TOPK_MAX, "batch procs apply: top_k %d", pr.top_k);
-  int rc;
   if (pr.params) {
     B200_REQUIRE(logits && tok && active && pr.penalties && pr.hist && pr.hist_len && pr.hist_cap >= 1 &&
                  pr.hist_cap <= BD_HIST_MAX, "batch procs apply: bad processor arguments");
     BdProcsP pp;
     pp.logits = logits; pp.ldv = ldv; pp.V = V; pp.tok = tok; pp.active = active; pp.pr = pr;
-    if ((rc = bd_launch(bd_procs_kernel, dim3(B), dim3(1024), 0, s, pp))) return rc;
+    B200_CUDA(launch(bd_procs_kernel, dim3(B), dim3(1024), 0, s, PDL_LAUNCH, pp));
   }
   if (pr.top_k > 0) {
     const int S = (V + BD_TOPK_SLICE - 1) / BD_TOPK_SLICE;
     B200_REQUIRE(logprobs && top_ids && top_lp && S * pr.top_k <= BD_TOPK_CAND_MAX, "batch procs apply: bad top-k arguments");
     unsigned long long* cand = nullptr;
     B200_CUDA(cudaMallocAsync(&cand, (size_t)B * S * pr.top_k * 8, s));
-    rc = bd_launch(bd_topk_part_kernel, dim3(S, B), dim3(256), 0, s, logprobs, ldv, V, pr.top_k, cand);
-    if (!rc)
-      rc = bd_launch(bd_topk_merge_kernel, dim3(B), dim3(256), 0, s, (const unsigned long long*)cand, S, pr.top_k,
-                     (const int*)nullptr, 1, B, top_ids, top_lp);
+    cudaError_t e = launch(bd_topk_part_kernel, dim3(S, B), dim3(256), 0, s, PDL_LAUNCH, logprobs, ldv, V, pr.top_k, cand);
+    if (e == cudaSuccess)
+      e = launch(bd_topk_merge_kernel, dim3(B), dim3(256), 0, s, PDL_LAUNCH, (const unsigned long long*)cand, S, pr.top_k,
+                 (const int*)nullptr, 1, B, top_ids, top_lp);
     B200_CUDA(cudaFreeAsync(cand, s));
-    if (rc) return rc;
+    B200_CUDA(e);
   }
   return B200_OK;
 }

@@ -42,12 +42,12 @@ __device__ __forceinline__ void produce_phase(const MegaPhase& g, const bf16* W,
   int tn = 0;
   for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
     const int s = rg.slot();
-    mb_wait(&sh->empty_bar[s], rg.parity() ^ 1u, &sh->err);
+    mbar_wait_bounded(&sh->empty_bar[s], rg.parity() ^ 1u, &sh->err);
     if (tdbg && tn < 30) tdbg[tn++] = gtimer();
     int rows = g.R;
     if (MODE != PH_QKV) rows = min(g.R, g.N - t * g.R);
     const uint32_t bytes = (uint32_t)rows * rows_unit;
-    mb_expect_tx(&sh->full_bar[s], bytes * T::NRW);
+    mbar_expect_tx(&sh->full_bar[s], bytes * T::NRW);
     uint8_t* dst = ring + (long)s * MEGA_STAGE;
     bulk_g2s(dst, mega_tile_src<MODE>(g, W, W2, hd, t, 0), bytes, &sh->full_bar[s], pol);
     if (T::PAIR)
@@ -253,7 +253,7 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
     const int s = rg.slot();
     int rows = g.R;
     if (MODE != PH_QKV) rows = min(g.R, g.N - t * g.R);
-    mb_wait(&sh->full_bar[s], rg.parity(), &sh->err);
+    mbar_wait_bounded(&sh->full_bar[s], rg.parity(), &sh->err);
     if (tdbg && threadIdx.x == 0 && tn < 30) tdbg[tn++] = gtimer();
     rg.advance();
     const uint8_t* base = ring + (long)s * MEGA_STAGE + (long)rloc * rows_unit;
@@ -299,7 +299,7 @@ __device__ __forceinline__ void consume_phase(const MegaP& p, const MegaPhase& g
 #pragma unroll
     for (int m = 0; m < T::NRW; ++m) acc[m] = warp_sum(acc[m]);
     __syncwarp();
-    if (lane == 0) mb_arrive(&sh->empty_bar[s]);
+    if (lane == 0) mbar_arrive(&sh->empty_bar[s]);
     if (tdbg && threadIdx.x == 0 && tn < 30) tdbg[tn++] = gtimer();
     if (g.S > 1) {
       if (lane == 0) {
@@ -353,14 +353,14 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) k_mega(const MegaP p) {
   if (p.st->error) return;  // a previous step gave up: do not spin again
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.n_stages; ++s) {
-      mb_init(&sh.full_bar[s], 1);
-      mb_init(&sh.empty_bar[s], 8);
+      mbar_init(&sh.full_bar[s], 1);
+      mbar_init(&sh.empty_bar[s], 8);
     }
     sh.err = 0;
     sh.bar_base = p.st->bar_base;
     sh.att_base = p.st->att_base;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
   }
   __syncthreads();
   Ring rg;
@@ -503,32 +503,12 @@ static int mega_chx(const MegaPhase& g) { return cdiv(cdiv(g.K >> 3, g.S), 32); 
 
 template <int CHH, int CHI>
 static int launch_k_mega(const MegaP& p, int grid, size_t smem, cudaStream_t s) {
-  // the function attributes are per device (a second engine on another GPU of the same process
-  // must opt in again)
-  static unsigned long long set_mask = 0ull;
-  int dev = 0;
-  B200_CUDA(cudaGetDevice(&dev));
-  if (!(set_mask >> (dev & 63) & 1ull)) {
-    B200_CUDA(cudaFuncSetAttribute(k_mega<CHH, CHI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   227 * 1024 - 2048));
-    B200_CUDA(cudaFuncSetAttribute(k_mega<CHH, CHI>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                   cudaSharedmemCarveoutMaxShared));
-    set_mask |= 1ull << (dev & 63);
-  }
+  int rc;
+  if ((rc = kernel_opt_in((const void*)k_mega<CHH, CHI>, 227 * 1024 - 2048, true))) return rc;
   // COOPERATIVE launch: the software grid barrier needs every CTA resident at once; the driver
   // refuses the launch (instead of letting it deadlock) if the grid cannot be co-resident, and
   // never schedules it partially next to another kernel.
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(MEGA_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeCooperative;
-  at[0].val.cooperative = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  B200_CUDA(cudaLaunchKernelEx(&cfg, k_mega<CHH, CHI>, p));
+  B200_CUDA(launch(k_mega<CHH, CHI>, dim3(grid), dim3(MEGA_THREADS), smem, s, LaunchOpts{false, 0, true}, p));
   return B200_OK;
 }
 

@@ -4,6 +4,9 @@
 // workspace and the KV pool (torch-allocated device memory).
 #include <stdarg.h>
 
+#include <array>
+#include <map>
+#include <mutex>
 #include <optional>
 #include <string>
 #include <unordered_map>
@@ -25,6 +28,24 @@ void set_error(const char* fmt, ...) {
 int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
   set_error("CUDA error %d (%s) at %s:%d in %s", (int)e, cudaGetErrorString(e), file, line, what);
   return B200_ERR_CUDA;
+}
+
+int kernel_opt_in(const void* kern, int max_dyn_smem, bool max_carveout) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, std::array<int, 2>> set;  // (kernel, device) -> values set, 0 = none
+  int dev = 0;
+  B200_CUDA(cudaGetDevice(&dev));
+  const cudaFuncAttribute attr[2] = {cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     cudaFuncAttributePreferredSharedMemoryCarveout};
+  const int want[2] = {max_dyn_smem, max_carveout ? (int)cudaSharedmemCarveoutMaxShared : 0};
+  std::lock_guard<std::mutex> g(mu);
+  std::array<int, 2>& have = set[{kern, dev}];
+  for (int i = 0; i < 2; ++i) {
+    if (want[i] <= 0 || have[i] == want[i]) continue;
+    B200_CUDA(cudaFuncSetAttribute(kern, attr[i], want[i]));
+    have[i] = want[i];
+  }
+  return B200_OK;
 }
 
 struct VBlk {
@@ -159,8 +180,6 @@ struct b200_engine {
   int last_steps = 0;
   bool timing_valid = false;
   int attn_cluster = 8;
-  bool decode_prepared = false;  // decode_prepare() has run for this engine
-  int attn_prepared_cap = -1, attn_prepared_cluster = -1;  // attn_prepare() has run for this capacity and cluster
   // megakernel
   int use_mega = 1;  // 0: one kernel per phase, 1: k_mega
   bool mega_fits = true;  // false: this shape / cache capacity does not fit the persistent kernel
@@ -1103,10 +1122,7 @@ int b200_engine_prefill(b200_engine* e, const void* embeds, const int* pos3, int
   const bf16* h = (const bf16*)(e->ws + lm_ws(c, T).h);
   // last row through the fused head + sampler; arms the decode state
   const DecodeDims d = e->dims();
-  if (!e->decode_prepared) {
-    if ((rc = decode_prepare())) return rc;
-    e->decode_prepared = true;
-  }
+  if ((rc = decode_prepare())) return rc;
   e->ctx_host = ctx0 + T;
   e->pos_host = ctx0 + T + rope_delta;
   if ((rc = launch_set_state(e->st, 0, e->ctx_host, e->pos_host, 0, 0, e->embed, e->h, c.hidden, s)))
@@ -1167,10 +1183,7 @@ int b200_engine_prefill_batch(b200_engine* e, const void* embeds, const int* pos
   B200_CUDA(cudaEventRecord(e->loc_ev, s));   // the table (and its staging copy) may be rewritten after this point
   if (rc) return rc;
   const DecodeDims d = e->dims();
-  if (!e->decode_prepared) {
-    if ((rc = decode_prepare())) return rc;
-    e->decode_prepared = true;
-  }
+  if ((rc = decode_prepare())) return rc;
   for (int g = 0; g < n_seq; ++g) {   // first token of every sequence: fused head + sampler on its last row
     if ((rc = launch_set_state(e->st, 0, segs[g].T, segs[g].T, 0, 0, e->embed, e->h, c.hidden, s))) return rc;
     if ((rc = launch_head(d, e->norm, e->head, h + (long)(segs[g].off + segs[g].T - 1) * H, e->logits, e->partials, s)))
@@ -1219,10 +1232,7 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   if ((rc = launch_set_state(e->st, 0, e->ctx_host, e->pos_host, force_tokens_host ? 1 : 0, 0,
                              e->embed, e->h, e->cfg.hidden, s)))
     return rc;
-  if (!e->decode_prepared) {
-    if ((rc = decode_prepare())) return rc;
-    e->decode_prepared = true;
-  }
+  if ((rc = decode_prepare())) return rc;
   if (e->use_mega && e->mega_fits && !e->mega_ready) {
     if ((rc = mega_prepare(e, s))) {
       // a geometry the persistent kernel cannot hold (very long cache: the attention scratch
@@ -1237,11 +1247,8 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
     // cache that k_mega holds is not refused for being too long for k_attn
     if (e->kvb.kind == KvKind::q8) {
       if ((rc = kvq_decode_prepare(e->dims(), e->attn_cluster))) return rc;
-    } else if (!e->active_mega() &&
-               (e->attn_prepared_cap != e->kvb.cap || e->attn_prepared_cluster != e->attn_cluster)) {
+    } else if (!e->active_mega()) {
       if ((rc = attn_prepare(e->dims(), e->attn_cluster))) return rc;
-      e->attn_prepared_cap = e->kvb.cap;
-      e->attn_prepared_cluster = e->attn_cluster;
     }
   }
   if (e->use_graph && !e->gexec) {

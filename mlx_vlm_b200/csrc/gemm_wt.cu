@@ -67,43 +67,6 @@ struct WtParams {
   int n_pad;
 };
 
-__device__ __forceinline__ uint32_t w_smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void w_mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(w_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void w_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(w_smem_u32(bar)),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void w_mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(w_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void w_mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  const uint32_t addr = w_smem_u32(bar);
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void w_tma_2d(void* dst, const CUtensorMap* tmap, uint64_t* bar, int c0,
-                                         int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3}], [%4];" ::"r"(w_smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(w_smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void w_pdl_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void w_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void w_ebar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // the 2 consumer warpgroups
 
 // accumulator -> bf16 staging element: + bias, one rounding, activation
@@ -176,25 +139,25 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
   const int stage_bytes = p.KS * (WT_WBLK + xblk);
   const int NS = p.n_stages;
 
-  w_pdl_launch();  // the next kernel may start its prologue / weight prefetch as SM resources free up
+  pdl_launch_dependents();  // the next kernel may start its prologue / weight prefetch as SM resources free up
 
   auto issue_w = [&](int it, int s) {
     uint8_t* sW = ring + (long)s * stage_bytes;
     const int cnt = min(p.KS, kb1 - kb0 - it * p.KS);
     if (p.flags & 2u) {  // debug: no loads at all, the MMAs run on whatever the ring holds
-      w_mbar_arrive(&full_bar[s]);
+      mbar_arrive(&full_bar[s]);
       return;
     }
-    w_mbar_expect_tx(&full_bar[s], (uint32_t)cnt * (WT_WBLK + xblk));
+    mbar_expect_tx(&full_bar[s], (uint32_t)cnt * (WT_WBLK + xblk));
     for (int j = 0; j < cnt; ++j) {
       int kbw = kb0 + it * p.KS + j;
       if (p.kb_w > 0) kbw %= p.kb_w;
       const int kc = kbw * WT_BK;
       if (swiglu) {
-        w_tma_2d(sW + j * WT_WBLK, &tmW, &full_bar[s], kc, n0);
-        w_tma_2d(sW + j * WT_WBLK + 64 * 128, &tmW, &full_bar[s], kc, p.inter + n0);
+        tma_2d(sW + j * WT_WBLK, &tmW, &full_bar[s], kc, n0);
+        tma_2d(sW + j * WT_WBLK + 64 * 128, &tmW, &full_bar[s], kc, p.inter + n0);
       } else {
-        w_tma_2d(sW + j * WT_WBLK, &tmW, &full_bar[s], kc, n0);
+        tma_2d(sW + j * WT_WBLK, &tmW, &full_bar[s], kc, n0);
       }
     }
   };
@@ -203,7 +166,7 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     uint8_t* sX = ring + (long)s * stage_bytes + p.KS * WT_WBLK;
     const int cnt = min(p.KS, kb1 - kb0 - it * p.KS);
     for (int j = 0; j < cnt; ++j)
-      w_tma_2d(sX + j * xblk, &tmX, &full_bar[s], (kb0 + it * p.KS + j) * WT_BK, t0);
+      tma_2d(sX + j * xblk, &tmX, &full_bar[s], (kb0 + it * p.KS + j) * WT_BK, t0);
   };
 
   const int pre = n_it < NS ? n_it : NS;
@@ -211,23 +174,23 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmX)) : "memory");
     for (int s = 0; s < NS; ++s) {
-      w_mbar_init(&full_bar[s], 1);
-      w_mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
     // weights never depend on the previous kernel: request them before waiting for it
     for (int it = 0; it < pre; ++it) issue_w(it, it);
   }
   __syncthreads();
-  w_pdl_wait();  // everything the previous kernels wrote (X, residual) is visible from here on
+  pdl_wait();  // everything the previous kernels wrote (X, residual) is visible from here on
 
   if (wg == 0) {
     if (threadIdx.x == 0) {  // ===== TMA producer =====
       for (int it = 0; it < pre; ++it) issue_x(it, it);
       for (int it = pre; it < n_it; ++it) {
         const int s = it % NS;
-        w_mbar_wait(&empty_bar[s], ((it / NS) & 1) ^ 1);
+        mbar_wait(&empty_bar[s], ((it / NS) & 1) ^ 1);
         issue_w(it, s);
         issue_x(it, s);
       }
@@ -246,10 +209,10 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
     for (int i = 0; i < 8; ++i) acc[ch][i] = 0.f;
   for (int it = 0; it < n_it; ++it) {
     const int s = it % NS;
-    w_mbar_wait(&full_bar[s], (it / NS) & 1);
+    mbar_wait(&full_bar[s], (it / NS) & 1);
     if (!(p.flags & 1u)) {
-      const uint32_t w_a = wg_smem(ring + (long)s * stage_bytes) + c * 64 * 128;
-      const uint32_t x_a = wg_smem(ring + (long)s * stage_bytes + p.KS * WT_WBLK);
+      const uint32_t w_a = smem_u32(ring + (long)s * stage_bytes) + c * 64 * 128;
+      const uint32_t x_a = smem_u32(ring + (long)s * stage_bytes + p.KS * WT_WBLK);
       const int cnt = min(p.KS, kb1 - kb0 - it * p.KS);
 #pragma unroll
       for (int ch = 0; ch < WT_MAX_CH; ++ch) wg_fence_acc(acc[ch]);
@@ -269,7 +232,7 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
       for (int ch = 0; ch < WT_MAX_CH; ++ch) wg_fence_acc(acc[ch]);
     }
     __syncwarp();
-    if (lane == 0) w_mbar_arrive(&empty_bar[s]);  // this warp's MMAs have read the ring slot
+    if (lane == 0) mbar_arrive(&empty_bar[s]);  // this warp's MMAs have read the ring slot
   }
 
   // ===== epilogue (the 256 consumer threads) =====
@@ -422,19 +385,6 @@ gemm_wt_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
 // decode step: there the kernel is a chain of L2 round trips, and 1024 threads issue every load of a row at once
 constexpr int FIN_N_MAX = 8192;  // N <= FIN_THREADS * 4 * FIN_MAXV in both shapes
 
-template <int FIN_THREADS>
-__device__ __forceinline__ float fin_block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-#pragma unroll
-  for (int w = 0; w < FIN_THREADS / 32; ++w) t += red[w];
-  return t;
-}
-
 template <int FIN_THREADS, int FIN_MAXV>
 __global__ void __launch_bounds__(FIN_THREADS)
 finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ bias,
@@ -442,8 +392,8 @@ finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ 
                    int norm_kind, const bf16* __restrict__ nw, const bf16* __restrict__ nb, float eps,
                    bf16* __restrict__ xn, long ldx, int T, int N) {
   __shared__ float red[FIN_THREADS / 32];
-  w_pdl_launch();
-  w_pdl_wait();
+  pdl_launch_dependents();
+  pdl_wait();
   const int t = blockIdx.x;
   const int nv = N >> 2;
   float4 h[FIN_MAXV];
@@ -486,7 +436,7 @@ finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ 
   }
   if (norm_kind == B200_NORM_NONE) return;
   if (norm_kind == B200_NORM_RMS) {
-    const float tot = fin_block_sum<FIN_THREADS>(s2, red);
+    const float tot = block_sum<FIN_THREADS / 32>(s2, red);
     const float rs = 1.0f / sqrtf(tot / (float)N + eps);
 #pragma unroll
     for (int u = 0; u < FIN_MAXV; ++u) {
@@ -503,7 +453,7 @@ finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ 
     return;
   }
   // LayerNorm: fp32 mean / variance (two passes over the registers), cast, * w, + b
-  const float mu = fin_block_sum<FIN_THREADS>(s1, red) / (float)N;
+  const float mu = block_sum<FIN_THREADS / 32>(s1, red) / (float)N;
   float v = 0.f;
 #pragma unroll
   for (int u = 0; u < FIN_MAXV; ++u) {
@@ -514,7 +464,7 @@ finish_rows_kernel(const float* __restrict__ P, int S, const bf16* __restrict__ 
       v += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
     }
   }
-  const float var = fin_block_sum<FIN_THREADS>(v, red) / (float)N;
+  const float var = block_sum<FIN_THREADS / 32>(v, red) / (float)N;
   const float rstd = 1.0f / sqrtf(var + eps);
 #pragma unroll
   for (int u = 0; u < FIN_MAXV; ++u) {
@@ -744,34 +694,13 @@ int gemm_wt(const void* X, long ldx, const void* W, const void* bias, const void
   int rc = wt_tmap(W, (long)(ext && ext->ldw > 0 ? ext->ldw : k_w), N, k_w, mode == B200_WT_SWIGLU ? 64 : WT_ROWS, &tw);
   if (rc) return rc;
   if ((rc = wt_tmap(X, ldx, T, K, cfg.TN, &tx))) return rc;
-  static unsigned long long set_mask = 0ull;
-  int dev = 0;
-  B200_CUDA(cudaGetDevice(&dev));
-  if (!(set_mask >> (dev & 63) & 1ull)) {
-    for (auto* k : {gemm_wt_kernel<false, 8>, gemm_wt_kernel<false, 16>, gemm_wt_kernel<true, 8>,
-                    gemm_wt_kernel<true, 16>}) {
-      B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 1024));
-      B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    }
-    set_mask |= 1ull << (dev & 63);
-  }
   const int row_blocks = mode == B200_WT_SWIGLU ? cdiv(inter, 64) : cdiv(N, WT_ROWS);
-  cudaLaunchConfig_t lc = {};
-  lc.gridDim = dim3(row_blocks, cdiv(T, cfg.TN), splits);
-  lc.blockDim = dim3(WT_THREADS);
-  lc.dynamicSmemBytes = smem;
-  lc.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = at;
-  lc.numAttrs = 1;
   const bool tower = mode == B200_WT_F32 || mode == B200_WT_SPLIT, wide = cfg.TN > 128;
-  if (tower) {
-    B200_CUDA(cudaLaunchKernelEx(&lc, wide ? gemm_wt_kernel<true, 16> : gemm_wt_kernel<true, 8>, tw, tx, p));
-  } else {
-    B200_CUDA(cudaLaunchKernelEx(&lc, wide ? gemm_wt_kernel<false, 16> : gemm_wt_kernel<false, 8>, tw, tx, p));
-  }
+  auto* kern = !tower ? (!wide ? gemm_wt_kernel<false, 8> : gemm_wt_kernel<false, 16>)
+                      : (!wide ? gemm_wt_kernel<true, 8> : gemm_wt_kernel<true, 16>);
+  if ((rc = kernel_opt_in((const void*)kern, 227 * 1024 - 1024, true))) return rc;
+  B200_CUDA(launch(kern, dim3(row_blocks, cdiv(T, cfg.TN), splits), dim3(WT_THREADS), smem, st, PDL_LAUNCH, tw, tx,
+                   p));
   return B200_OK;
 }
 
@@ -1008,25 +937,10 @@ int finish_rows(const float* P, int S, const void* bias, const void* resid, long
   B200_REQUIRE(norm_kind == B200_NORM_NONE || (xn && (norm_kind != B200_NORM_RMS || nw)),
                "finish_rows: norm output / weight missing");
   B200_REQUIRE((ldr % 4) == 0 && (ldh % 4) == 0 && (ldx % 4) == 0, "finish_rows: strides must be multiples of 4");
-  cudaLaunchConfig_t lc = {};
-  lc.gridDim = dim3(T);
   const bool few_rows = T <= 32;
-  lc.blockDim = dim3(few_rows ? 1024 : 256);
-  lc.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = at;
-  lc.numAttrs = 1;
-  if (few_rows) {
-    B200_CUDA(cudaLaunchKernelEx(&lc, finish_rows_kernel<1024, 2>, P, S, (const bf16*)bias, (const bf16*)resid, ldr,
-                                 (bf16*)h_out, ldh, norm_kind, (const bf16*)nw, (const bf16*)nb, eps,
-                                 (bf16*)xn, ldx, T, N));
-  } else {
-    B200_CUDA(cudaLaunchKernelEx(&lc, finish_rows_kernel<256, 8>, P, S, (const bf16*)bias, (const bf16*)resid, ldr,
-                                 (bf16*)h_out, ldh, norm_kind, (const bf16*)nw, (const bf16*)nb, eps,
-                                 (bf16*)xn, ldx, T, N));
-  }
+  B200_CUDA(launch(few_rows ? finish_rows_kernel<1024, 2> : finish_rows_kernel<256, 8>, dim3(T),
+                   dim3(few_rows ? 1024 : 256), 0, st, PDL_LAUNCH, P, S, (const bf16*)bias, (const bf16*)resid, ldr,
+                   (bf16*)h_out, ldh, norm_kind, (const bf16*)nw, (const bf16*)nb, eps, (bf16*)xn, ldx, T, N));
   return B200_OK;
 }
 

@@ -278,10 +278,7 @@ static int attn_q8_hsplit(const DecodeDims& d) {
 int kvq_decode_prepare(const DecodeDims& d, int cluster) {
   const size_t smem = attn_q8_smem(d, cdiv(d.cap, cluster));
   B200_REQUIRE(smem <= 220 * 1024, "8-bit decode attention: cache capacity %d too large", d.cap);
-  B200_CUDA(cudaFuncSetAttribute(k_attn_q8, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  B200_CUDA(cudaFuncSetAttribute(k_attn_q8, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared));
-  return B200_OK;
+  return kernel_opt_in((const void*)k_attn_q8, (int)smem, true);
 }
 
 int launch_attn_q8(const DecodeDims& d, const bf16* qbuf, const KvqPlanes& kc8, const KvqPlanes& vc8,
@@ -294,19 +291,8 @@ int launch_attn_q8(const DecodeDims& d, const bf16* qbuf, const KvqPlanes& kc8, 
   B200_REQUIRE(cluster >= 1 && cluster <= AQ_MAXCL, "8-bit decode attention: cluster %d", cluster);
   const int hs = attn_q8_hsplit(d);
   const int chunk_cap = cdiv(d.cap, cluster);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(cluster, d.n_kv * hs, 1);
-  cfg.blockDim = dim3(256);
-  cfg.dynamicSmemBytes = attn_q8_smem(d, chunk_cap);
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  B200_CUDA(cudaLaunchKernelEx(&cfg, k_attn_q8, d, qbuf, kc8, vc8, stage_k, stage_v, out, st, chunk_cap, hs));
+  B200_CUDA(launch(k_attn_q8, dim3(cluster, d.n_kv * hs, 1), dim3(256), attn_q8_smem(d, chunk_cap), s,
+                   LaunchOpts{false, cluster, false}, d, qbuf, kc8, vc8, stage_k, stage_v, out, st, chunk_cap, hs));
   return B200_OK;
 }
 

@@ -1,5 +1,5 @@
-// Device pieces of the persistent decode kernel k_mega (decode_mega.cu): mbarrier / bulk-copy
-// wrappers, the software grid barrier, the distributed attention phase and the sampler.
+// Device pieces of the persistent decode kernel k_mega (decode_mega.cu): the software grid barrier,
+// the distributed attention phase and the sampler.
 #pragma once
 #include "common.cuh"
 #include "decode.cuh"
@@ -8,52 +8,6 @@ namespace b200 {
 
 namespace {
 
-__device__ __forceinline__ uint32_t s_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mb_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mb_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s_u32(bar)),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mb_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(bar)) : "memory");
-}
-// bounded wait: a scheduling bug must not hang the GPU (sets *err and falls through)
-__device__ __forceinline__ void mb_wait(uint64_t* bar, uint32_t parity, int* err) {
-  uint32_t done;
-  const uint32_t addr = s_u32(bar);
-  unsigned spins = 0;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (!done && ++spins > (1u << 20)) {
-      *err = 2;
-      break;
-    }
-  } while (!done);
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar,
-                                         uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1], %2, [%3], %4;" ::"r"(s_u32(dst)),
-      "l"(src), "r"(bytes), "r"(s_u32(bar)), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ uint64_t policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
 // activations written by other CTAs in an earlier phase: read through L2
 __device__ __forceinline__ uint4 ldcg16(const void* p) {
   return __ldcg(reinterpret_cast<const uint4*>(p));
@@ -431,11 +385,6 @@ __device__ __forceinline__ void attn_phase(const MegaP& p, const bf16* kc, const
 #undef ATT_STAMP
 }
 
-__device__ __forceinline__ uint32_t orderable_u(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 // software grid barrier among the consumer threads of all CTAs
 __device__ __forceinline__ void grid_barrier(const MegaP& p, MegaShared* sh, unsigned& idx) {
   cbar();
@@ -491,7 +440,7 @@ __device__ __forceinline__ void mega_sample_finalize(const MegaP& p, MegaShared&
       for (int j = 0; j < 8; ++j) {
         o[j] = rbf(f[j] - lse);
         const unsigned long long key =
-            ((unsigned long long)orderable_u(o[j]) << 32) | (0xFFFFFFFFu - (uint32_t)(c * 8 + j));
+            ((unsigned long long)orderable(o[j]) << 32) | (0xFFFFFFFFu - (uint32_t)(c * 8 + j));
         best = key > best ? key : best;
       }
       uint4 ov;

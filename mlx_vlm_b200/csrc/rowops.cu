@@ -348,10 +348,10 @@ int qk_norm(void* qkv, int T, int n_heads, int n_kv, int hd, const void* qn, con
   const long warps = (long)T * (n_heads + n_kv);
   const dim3 grid(cdiv(warps, 8));
   if (hd == 128)
-    B200_CUDA(launch_pdl(qk_norm_kernel<4>, grid, dim3(256), 0, st, (bf16*)qkv, T, n_heads, n_kv, (const bf16*)qn,
+    B200_CUDA(launch(qk_norm_kernel<4>, grid, dim3(256), 0, st, PDL_LAUNCH, (bf16*)qkv, T, n_heads, n_kv, (const bf16*)qn,
                          (const bf16*)kn, eps));
   else
-    B200_CUDA(launch_pdl(qk_norm_kernel<2>, grid, dim3(256), 0, st, (bf16*)qkv, T, n_heads, n_kv, (const bf16*)qn,
+    B200_CUDA(launch(qk_norm_kernel<2>, grid, dim3(256), 0, st, PDL_LAUNCH, (bf16*)qkv, T, n_heads, n_kv, (const bf16*)qn,
                          (const bf16*)kn, eps));
   return B200_OK;
 }
@@ -451,25 +451,18 @@ __global__ void __launch_bounds__(512) embed_merge_kernel(const int* __restrict_
 }
 
 // ---------------------------------------------------------------------------
-static inline int grid_for(long work, int block) {
-  long g = (work + block - 1) / block;
-  if (g > 132L * 16) g = 132L * 16;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 int cast_f32_bf16(const float* src, void* dst, long n, cudaStream_t st) {
   B200_REQUIRE(n >= 0, "cast: n<0");
   if (n == 0) return B200_OK;
   B200_REQUIRE(((uintptr_t)src & 15) == 0 && ((uintptr_t)dst & 7) == 0, "cast: misaligned");
-  B200_CUDA(launch_pdl(cast_f32_bf16_kernel, dim3(grid_for((n + 3) / 4, 256)), dim3(256), 0, st, src, (bf16*)dst, n));
+  B200_CUDA(launch(cast_f32_bf16_kernel, dim3(grid_for((n + 3) / 4, 256)), dim3(256), 0, st, PDL_LAUNCH, src, (bf16*)dst, n));
   return B200_OK;
 }
 
 int layer_norm(const void* x, const void* w, const void* b, void* y, int rows, int dim, float eps,
                cudaStream_t st) {
   B200_REQUIRE(rows > 0 && dim > 0 && (dim % 8) == 0, "layer_norm: rows=%d dim=%d", rows, dim);
-  B200_CUDA(launch_pdl(layer_norm_kernel, dim3(cdiv(rows, 8)), dim3(256), 0, st, (const bf16*)x, (const bf16*)w,
+  B200_CUDA(launch(layer_norm_kernel, dim3(cdiv(rows, 8)), dim3(256), 0, st, PDL_LAUNCH, (const bf16*)x, (const bf16*)w,
                        (const bf16*)b, (bf16*)y, rows, dim, eps));
   return B200_OK;
 }
@@ -477,7 +470,7 @@ int layer_norm(const void* x, const void* w, const void* b, void* y, int rows, i
 int rms_norm(const void* x, const void* w, void* y, int rows, int dim, float eps,
              cudaStream_t st) {
   B200_REQUIRE(rows > 0 && dim > 0 && (dim % 8) == 0 && w, "rms_norm: rows=%d dim=%d", rows, dim);
-  B200_CUDA(launch_pdl(rms_norm_kernel, dim3(cdiv(rows, 8)), dim3(256), 0, st, (const bf16*)x, (const bf16*)w,
+  B200_CUDA(launch(rms_norm_kernel, dim3(cdiv(rows, 8)), dim3(256), 0, st, PDL_LAUNCH, (const bf16*)x, (const bf16*)w,
                        (bf16*)y, rows, dim, eps));
   return B200_OK;
 }
@@ -505,13 +498,13 @@ int mrope_kv_write(void* qkv, const int* pos3, const float* inv_freq, const int*
     if (groups > slots) groups = slots;
     if (groups < 1) groups = 1;
     const int per = (slots + groups - 1) / groups;
-    B200_CUDA(launch_pdl(mrope_kv_write_tiled_kernel, dim3(tiles, (slots + per - 1) / per), dim3(256), 0, st, (bf16*)qkv,
+    B200_CUDA(launch(mrope_kv_write_tiled_kernel, dim3(tiles, (slots + per - 1) / per), dim3(256), 0, st, PDL_LAUNCH, (bf16*)qkv,
                          pos3, inv_freq, axis_sel, (bf16*)kc, (bf16*)vc, T, ctx0, cap, n_heads, n_kv, hd, q_scale, (bf16*)vt,
                          t_ld, ref, layer, (bf16*)kws, (const int2*)tok_loc, row_stride, per));
     return B200_OK;
   }
   const long total = (long)T * (n_heads + 2 * n_kv) * (hd / 2);
-  B200_CUDA(launch_pdl(mrope_kv_write_kernel, dim3(grid_for(total, 256)), dim3(256), 0, st, (bf16*)qkv, pos3, inv_freq,
+  B200_CUDA(launch(mrope_kv_write_kernel, dim3(grid_for(total, 256)), dim3(256), 0, st, PDL_LAUNCH, (bf16*)qkv, pos3, inv_freq,
                        axis_sel, (bf16*)kc, (bf16*)vc, T, ctx0, cap, n_heads, n_kv, hd, q_scale, (bf16*)vt, t_ld, ref,
                        layer, (bf16*)kws, (const int2*)tok_loc, row_stride));
   return B200_OK;
@@ -628,7 +621,7 @@ __global__ void vision_qkv_post_kernel(bf16* __restrict__ qkv, const int* __rest
 int vision_rope_table(const int* pos_hw, const float* inv_freq, int n_tok, int hd, void* cs, cudaStream_t st) {
   B200_REQUIRE(n_tok > 0 && (hd % 4) == 0 && cs, "vision_rope_table: bad shape");
   const int total = n_tok * (hd / 2);
-  B200_CUDA(launch_pdl(vision_rope_table_kernel, dim3(cdiv(total, 256)), dim3(256), 0, st, pos_hw, inv_freq, n_tok, hd / 2,
+  B200_CUDA(launch(vision_rope_table_kernel, dim3(cdiv(total, 256)), dim3(256), 0, st, PDL_LAUNCH, pos_hw, inv_freq, n_tok, hd / 2,
                        (float2*)cs));
   return B200_OK;
 }
@@ -638,7 +631,7 @@ int vision_qkv_post(void* qkv, const int* pos_hw, const float* inv_freq, int n_t
   B200_REQUIRE(n_tok > 0 && n_heads > 0 && (hd % 8) == 0 && hd <= 128 && (t_ld % 8) == 0 && t_ld >= n_tok,
                "vision_qkv_post: bad shape (hd=%d t_ld=%d)", hd, t_ld);
   const float scale_bf = __bfloat162float(__float2bfloat16_rn(scale));
-  B200_CUDA(launch_pdl(vision_qkv_post_kernel, dim3(cdiv(n_tok, 32), n_heads), dim3(256), 0, st, (bf16*)qkv, pos_hw,
+  B200_CUDA(launch(vision_qkv_post_kernel, dim3(cdiv(n_tok, 32), n_heads), dim3(256), 0, st, PDL_LAUNCH, (bf16*)qkv, pos_hw,
                        inv_freq, n_tok, n_heads, hd, scale_bf, (bf16*)vt, t_ld, (const float2*)cs));
   return B200_OK;
 }
@@ -657,8 +650,7 @@ int embed_merge(const int* ids, int B, int T, const void* table, int hidden, con
   B200_REQUIRE(B > 0 && T > 0 && (hidden % 8) == 0, "embed_merge: bad shape");
   B200_REQUIRE((long)T * 4 <= 200 * 1024, "embed_merge: T=%d too long", T);
   if ((size_t)T * 4 > 48 * 1024) {
-    B200_CUDA(cudaFuncSetAttribute(embed_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   T * 4));
+    if (int rc = kernel_opt_in((const void*)embed_merge_kernel, T * 4, false)) return rc;
   }
   int per_row = (T + 7) / 8;  // >= 8 positions per CTA
   const int cap_ctas = (2 * 132 + B - 1) / B;

@@ -30,18 +30,6 @@ __device__ __forceinline__ void split_store2(bf16* dst, int n_pad, float a, floa
   *reinterpret_cast<uint32_t*>(dst + n_pad) = pack2(a - h0, b - h1);
 }
 
-__device__ __forceinline__ float t_block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) t += red[w];
-  return t;
-}
-
 // LayerNorm in fp32 (nn.LayerNorm on an fp32 array: fp32 statistics, fp32 affine); output as fp32
 // and / or as the split operand of the next GEMM.  One CTA per row, N % 4 == 0, N <= 8192.
 __global__ void __launch_bounds__(256) f32_layer_norm_kernel(const float* __restrict__ x, long ldx,
@@ -64,7 +52,7 @@ __global__ void __launch_bounds__(256) f32_layer_norm_kernel(const float* __rest
       s1 += (h[u].x + h[u].y) + (h[u].z + h[u].w);
     }
   }
-  const float mu = t_block_sum(s1, red) / (float)N;
+  const float mu = block_sum<8>(s1, red) / (float)N;
   float v = 0.f;
 #pragma unroll
   for (int u = 0; u < 8; ++u) {
@@ -74,7 +62,7 @@ __global__ void __launch_bounds__(256) f32_layer_norm_kernel(const float* __rest
       v += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
     }
   }
-  const float rstd = rsqrtf(t_block_sum(v, red) / (float)N + eps);
+  const float rstd = rsqrtf(block_sum<8>(v, red) / (float)N + eps);
 #pragma unroll
   for (int u = 0; u < 8; ++u) {
     const int c = threadIdx.x + 256 * u;
@@ -114,7 +102,7 @@ __global__ void __launch_bounds__(256) f32_rms_norm_kernel(const float* __restri
       s2 += (h[u].x * h[u].x + h[u].y * h[u].y) + (h[u].z * h[u].z + h[u].w * h[u].w);
     }
   }
-  const float rs = rsqrtf(t_block_sum(s2, red) / (float)N + eps);
+  const float rs = rsqrtf(block_sum<8>(s2, red) / (float)N + eps);
 #pragma unroll
   for (int u = 0; u < 8; ++u) {
     const int c = threadIdx.x + 256 * u;
@@ -455,20 +443,10 @@ __global__ void __launch_bounds__(AF_THREADS) attention_f32_kernel(const AttnF32
 
 template <int HDP>
 static int attn_f32_launch(const AttnF32P& p, dim3 grid, cudaStream_t st) {
-  static unsigned long long attr_mask = 0ull;
-  if (first_use_on_device(&attr_mask)) {
-    B200_CUDA(cudaFuncSetAttribute(attention_f32_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)attn_f32_smem<HDP>()));
-  }
+  if (int rc = kernel_opt_in((const void*)attention_f32_kernel<HDP>, (int)attn_f32_smem<HDP>(), false)) return rc;
   attention_f32_kernel<HDP><<<grid, AF_THREADS, attn_f32_smem<HDP>(), st>>>(p);
   B200_CHECK_LAUNCH();
   return B200_OK;
-}
-
-static inline int t_grid(long work, int block) {
-  long g = (work + block - 1) / block;
-  if (g > 132L * 16) g = 132L * 16;
-  return (int)(g < 1 ? 1 : g);
 }
 
 }  // namespace
@@ -496,7 +474,7 @@ int f32_rms_norm(const float* x, long ldx, const void* w, float eps, float* out3
 
 int f32_swiglu_split(const float* gu, long ldg, void* out, long ld_split, int n_pad, int T, int I, cudaStream_t st) {
   B200_REQUIRE(gu && out && T > 0 && I > 0 && (I % 4) == 0 && (ldg % 4) == 0 && (ld_split % 4) == 0, "f32_swiglu: bad shape");
-  f32_swiglu_split_kernel<<<t_grid((long)T * (I / 4), 256), 256, 0, st>>>(gu, ldg, (bf16*)out, ld_split, n_pad, T, I);
+  f32_swiglu_split_kernel<<<grid_for((long)T * (I / 4), 256), 256, 0, st>>>(gu, ldg, (bf16*)out, ld_split, n_pad, T, I);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -504,7 +482,7 @@ int f32_swiglu_split(const float* gu, long ldg, void* out, long ld_split, int n_
 int f32_split(const float* x, long ldx, void* out, long ld_split, int n_pad, int T, int N, cudaStream_t st) {
   B200_REQUIRE(x && out && T > 0 && N > 0 && (N % 4) == 0 && (ldx % 4) == 0 && (ld_split % 4) == 0 && (n_pad % 4) == 0,
                "f32_split: bad shape");
-  f32_split_kernel<<<t_grid((long)T * (N / 4), 256), 256, 0, st>>>(x, ldx, (bf16*)out, ld_split, n_pad, T, N);
+  f32_split_kernel<<<grid_for((long)T * (N / 4), 256), 256, 0, st>>>(x, ldx, (bf16*)out, ld_split, n_pad, T, N);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -514,7 +492,7 @@ int pixel_shuffle_split(const float* x, int n_img, int side, int E, int s, int r
   B200_REQUIRE(x && out && n_img > 0 && s > 0 && side > 0 && side % s == 0 && (E % 4) == 0 && n_pad >= E * s * s &&
                    (ld_split % 4) == 0 && (n_pad % 4) == 0, "pixel_shuffle_split: bad shape");
   const long total = (long)n_img * (side / s) * (side / s) * s * s * (E / 4);
-  pixel_shuffle_split_kernel<<<t_grid(total, 256), 256, 0, st>>>(x, n_img, side, E, s, round_in, (bf16*)out, ld_split,
+  pixel_shuffle_split_kernel<<<grid_for(total, 256), 256, 0, st>>>(x, n_img, side, E, s, round_in, (bf16*)out, ld_split,
                                                                  n_pad);
   B200_CHECK_LAUNCH();
   return B200_OK;
@@ -524,7 +502,7 @@ int clip_patchify(const float* pix, int B, int H, int W, int C, int ps, void* ou
   B200_REQUIRE(pix && out && B > 0 && H % ps == 0 && W % ps == 0 && Kp >= ps * ps * C && (Kp % 8) == 0,
                "clip_patchify: bad shape");
   const long total = (long)B * (H / ps) * (W / ps) * Kp;
-  clip_patchify_kernel<<<t_grid(total, 256), 256, 0, st>>>(pix, B, H, W, C, ps, (bf16*)out, Kp);
+  clip_patchify_kernel<<<grid_for(total, 256), 256, 0, st>>>(pix, B, H, W, C, ps, (bf16*)out, Kp);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -533,7 +511,7 @@ int tower_embed(const float* patch, const void* cls, const void* pos, const int*
                 int E, int n_pos, cudaStream_t st) {
   B200_REQUIRE(patch && pos && emb && B > 0 && P > 0 && (E % 4) == 0, "tower_embed: bad shape");
   const long total = (long)B * (P + (cls ? 1 : 0)) * (E / 4);
-  tower_embed_kernel<<<t_grid(total, 256), 256, 0, st>>>(patch, (const bf16*)cls, (const bf16*)pos, pos_ids, emb, B, P,
+  tower_embed_kernel<<<grid_for(total, 256), 256, 0, st>>>(patch, (const bf16*)cls, (const bf16*)pos, pos_ids, emb, B, P,
                                                          E, n_pos);
   B200_CHECK_LAUNCH();
   return B200_OK;
@@ -543,7 +521,7 @@ int f32_vision_rope(float* qkv, long ld, const int* pos_hw, const float* inv_fre
                     cudaStream_t st) {
   B200_REQUIRE(qkv && pos_hw && inv_freq && T > 0 && n_heads > 0 && (hd % 4) == 0 && ld >= 3L * n_heads * hd,
                "f32_vision_rope: bad shape");
-  f32_vision_rope_kernel<<<t_grid((long)T * n_heads * hd, 256), 256, 0, st>>>(qkv, ld, pos_hw, inv_freq, T, n_heads, hd);
+  f32_vision_rope_kernel<<<grid_for((long)T * n_heads * hd, 256), 256, 0, st>>>(qkv, ld, pos_hw, inv_freq, T, n_heads, hd);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -552,7 +530,7 @@ int f32_gather_rows(const float* in, long ld_in, const int* idx, int n_idx, int 
                     cudaStream_t st) {
   B200_REQUIRE(in && idx && out && n_idx > 0 && unit > 0 && n > 0 && (n % 4) == 0 && (ld_in % 4) == 0 && (ld_out % 4) == 0,
                "f32_gather_rows: bad shape");
-  f32_gather_rows_kernel<<<t_grid((long)n_idx * unit * (n / 4), 256), 256, 0, st>>>(in, ld_in, idx, n_idx, unit, n, out,
+  f32_gather_rows_kernel<<<grid_for((long)n_idx * unit * (n / 4), 256), 256, 0, st>>>(in, ld_in, idx, n_idx, unit, n, out,
                                                                                    ld_out);
   B200_CHECK_LAUNCH();
   return B200_OK;

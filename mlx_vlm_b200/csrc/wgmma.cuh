@@ -9,6 +9,8 @@
 #include <cuda.h>
 #include <stdint.h>
 
+#include "common.cuh"
+
 namespace b200 {
 
 // Host: the TMA descriptor of a bf16 tensor of rank 2 or 3 that fills such operands: dims[0] is the contiguous
@@ -23,9 +25,32 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
          ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ uint32_t wg_smem(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+// TMA tile copies global -> shared through such a descriptor, completing on `bar`; c0 is the contiguous coordinate
+__device__ __forceinline__ void tma_2d(void* dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%2, %3}], [%4];" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+      : "memory");
 }
+__device__ __forceinline__ void tma_3d(void* dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
+      : "memory");
+}
+
+// row max / sum over the 4 threads of a quad (they hold the same accumulator rows)
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
 // before the first wgmma that reads registers written by ordinary instructions
 __device__ __forceinline__ void wg_arrive() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -86,6 +86,32 @@ def test_attention(lib, Lq, S_, nh, nkv, hd, causal):
     cmp_bf16(out.view(Lq, nh, hd), want[0].transpose(0, 1), f"attention Lq={Lq} S={S_} hd={hd}")
 
 
+def test_attention_two_pass_on_two_devices(lib):
+    """b200_attention's two-pass kernel (head_dim 72: not a multiple of 16, so the tensor-core kernel declines) with
+    S = 2048, i.e. 16 * 72 * 4 + 16 * 2048 * 2 = 70 KB of shared memory, on device 0 and then on device 1 of one
+    process: the kernel's shared-memory limit is a per-device attribute, raised on each device it runs on"""
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two GPUs")
+    from mlx_vlm_b200 import _native as Nn
+    from oracle import mlx_semantics as S
+    Lq, S_, nh, nkv, hd = 8, 2048, 4, 2, 72
+    r = R()
+    q = rnd(1, nh, Lq, hd, seed=40)
+    k = rnd(1, nkv, S_, hd, seed=41)
+    v = rnd(1, nkv, S_, hd, seed=42)
+    want = S.sdpa(r, q, k, v, hd ** -0.5, False)[0].transpose(0, 1)
+    for dev in (0, 1):
+        with torch.cuda.device(dev):
+            dq = to_dev(q[0].transpose(0, 1))
+            dk, dv = to_dev(k[0]), to_dev(v[0])
+            out = torch.zeros(Lq, nh * hd, dtype=torch.bfloat16, device="cuda")
+            Nn.check(lib.b200_attention(dq.data_ptr(), nh * hd, hd, dk.data_ptr(), hd, S_ * hd, dv.data_ptr(), hd,
+                                        S_ * hd, out.data_ptr(), nh * hd, nh, nkv, hd, Lq, S_, 0, float(hd ** -0.5),
+                                        0), f"attention on device {dev}")
+            torch.cuda.synchronize()
+        cmp_bf16(out.view(Lq, nh, hd), want, f"two-pass attention on device {dev}")
+
+
 def test_vision_rope(lib):
     from mlx_vlm_b200 import _native as Nn
     from oracle import qwen2vl as O
