@@ -130,6 +130,16 @@ int b200_attention(const void* q, long q_tok_stride, long q_head_stride,
 int b200_attention_fa(const void* q, long q_ts, long q_hs, const void* k, long k_ts, long k_hs,
                       const void* vt, long vt_hs, long vt_ds, void* out, long o_ts, int n_heads,
                       int n_kv, int hd, int Lq, int S, int causal, void* stream);
+/* b200_attention_fa on a part of larger tensors (the vision tower's frames, the batched prefill's sequences):
+ * q holds q_tot tokens and k / vt hold k_tot keys; queries [q0, q0+Lq) attend to keys [k0, k0+S), out row t at
+ * out + t*o_ts.  segs (device, 16-byte aligned, or NULL): n_seg rows of int4 (q0, Lq, k0, S), one segment per
+ * grid slice, which then replace the scalar q0 / Lq / k0 / S (Lq = the longest segment sizes the grid).  The key
+ * tile of a segment may read keys past its S up to k_tot: their scores are masked, but their V^T columns must be
+ * finite (a NaN times a zero probability is NaN). */
+int b200_attention_fa_seg(const void* q, long q_ts, long q_hs, const void* k, long k_ts, long k_hs,
+                          const void* vt, long vt_hs, long vt_ds, void* out, long o_ts, int n_heads,
+                          int n_kv, int hd, int Lq, int S, int causal, int q0, int q_tot, int k0, int k_tot,
+                          const void* segs, int n_seg, void* stream);
 /* vision tower after the qkv GEMM: 2-D rotary on q,k in place (vision.py:35-50), q pre-scaled
  * by bf16(scale), V^T written to vt[head][dim][t_ld] (t_ld % 8 == 0, >= n_tok) */
 int b200_vision_qkv_post(void* qkv, const int* pos_hw, const float* inv_freq, int n_tok, int n_heads,

@@ -50,6 +50,7 @@ SIGNATURES = {
     "b200_attention": (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _I, _I, _I, _I, _I, _I,
                             _F, _P]),
     "b200_attention_fa": (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_attention_fa_seg": (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L] + [_I] * 10 + [_P, _I, _P]),
     "b200_vision_qkv_post": (_I, [_P, _P, _P, _I, _I, _I, _F, _P, _I, _P]),
     "b200_swiglu": (_I, [_P, _P, _I, _I, _P]),
     "b200_embed_merge": (_I, [_P, _I, _I, _P, _I, _P, _I, _I, _I, _P, _P, _P]),

@@ -302,3 +302,11 @@ extern "C" int b200_attention_fa(const void* q, long q_ts, long q_hs, const void
   return b200::attention_fa(q, q_ts, q_hs, k, k_ts, k_hs, vt, vt_hs, vt_ds, out, o_ts, n_heads, n_kv, hd, Lq, S,
                             causal, (cudaStream_t)stream, 0, Lq, 0, S, nullptr, 0);
 }
+
+extern "C" int b200_attention_fa_seg(const void* q, long q_ts, long q_hs, const void* k, long k_ts, long k_hs,
+                                     const void* vt, long vt_hs, long vt_ds, void* out, long o_ts, int n_heads,
+                                     int n_kv, int hd, int Lq, int S, int causal, int q0, int q_tot, int k0, int k_tot,
+                                     const void* segs, int n_seg, void* stream) {
+  return b200::attention_fa(q, q_ts, q_hs, k, k_ts, k_hs, vt, vt_hs, vt_ds, out, o_ts, n_heads, n_kv, hd, Lq, S,
+                            causal, (cudaStream_t)stream, q0, q_tot, k0, k_tot, segs, n_seg);
+}

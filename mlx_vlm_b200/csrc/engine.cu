@@ -417,7 +417,11 @@ static LmWs lm_ws(const b200_qwen2vl_config& c, long T) {
   o.att = w.take(T * QH * 2);
   // T x 2 x inter bf16 that no kernel addresses.  Without it the batched prefill of
   // test_qwen3_vl_gpu::test_lock_step_rows_equal_single_requests[tiny] samples a wrong first token (the same
-  // bytes placed after `kws` also pass): kept until that dependency is found.
+  // bytes placed after `kws` also pass): kept until that dependency is found.  No kernel of a one-layer prefill
+  // touches these bytes: with the workspace filled with NaN before each call, single prefills (fresh prompt, later
+  // chunk, a 3600-token prompt) and batched prefills (Qwen2-VL-2B / 7B and Qwen3-VL head geometries) leave them NaN,
+  // and no NaN reaches their outputs (tests/test_prefill_attention_gpu.py checks both).  Without the pad that test
+  // still samples token 0, for a sequence of its second batched prefill (two layers, head_dim 64).
   w.take(T * 2L * c.inter * 2);
   o.act = w.take(T * c.inter * 2);   // SwiGLU output
   o.pos = w.take(3L * T * 4);        // position ids (graph input)

@@ -838,11 +838,16 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
       cand.push_back(model);
     }
     // ---- time them (the tuning launches never add a residual: the output stays idempotent) ----
-    // An fp32 output that is also its own residual (h += W.x in place) must not be overwritten by the
-    // measurement: those launches write a scratch buffer from the stream-ordered allocator instead.
+    // An output that is also its own residual (h += W.x in place, bf16 or fp32) must not be overwritten by the
+    // measurement: whenever a residual is given, those launches write a scratch buffer from the stream-ordered
+    // allocator instead of the caller's output.
     WtExt ext_copy;
     const WtExt* ext_t = nullptr;
     float* scratch32 = nullptr;
+    void* C_t = C;
+    if (residual && C) {
+      B200_CUDA(cudaMallocAsync(&C_t, (size_t)T * (size_t)ldc * sizeof(bf16), st));
+    }
     if (ext) {
       ext_copy = *ext;
       if (mode == B200_WT_F32 && ext->res32 && ext->C32) {
@@ -868,7 +873,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
         break;
       }
       for (int r = 0; r < REP && rc == B200_OK; ++r)
-        rc = gemm_wt(X, ldx, W, bias, nullptr, 0, C, ldc, partial, T, N, K, epilogue, mode, inter, cand[i], 0, st, ext_t);
+        rc = gemm_wt(X, ldx, W, bias, nullptr, 0, C_t, ldc, partial, T, N, K, epilogue, mode, inter, cand[i], 0, st, ext_t);
       cudaError_t ce = cudaStreamEndCapture(st, &graph);
       if (rc != B200_OK || ce != cudaSuccess || !graph) {
         if (graph) cudaGraphDestroy(graph);
@@ -895,6 +900,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     if (scratch32) cudaFreeAsync(scratch32, st);
+    if (C_t != C) cudaFreeAsync(C_t, st);
     if (rc) {
       set_error("gemm_wt: configuration measurement failed (T=%d N=%d K=%d mode=%d)", T, N, K, mode);
       return rc;

@@ -30,6 +30,7 @@ def _cfg(c):
     (576, 1280, 1176, 0, False, False, None),           # patch embed (K tail 1176 = 18*64+24)
     (700, 1000, 520, 1, True, True, (256, 1, 2, 1)),    # large token tile, ragged N, gelu + residual
     (272, 1536, 8960, 0, False, True, None),            # LM down + residual, no bias
+    (3600, 3584, 1024, 0, False, "inplace", None),      # 7B o_proj / down of a long chunk: h = h + x.W^T in place
 ])
 def test_gemm_wt_bf16(lib, T, N, K, epi, bias, res, cfg):
     from mlx_vlm_b200 import _native as Nn
@@ -53,6 +54,8 @@ def test_gemm_wt_bf16(lib, T, N, K, epi, bias, res, cfg):
     if res:
         dr = torch.zeros(T, ldn, dtype=torch.bfloat16, device="cuda")
         dr[:, :N] = to_dev(resid)
+        if res == "inplace":   # the output is its own residual, as in the engine's long-chunk residual add
+            Cc = dr
     Nn.check(lib.b200_gemm_wt(dX.data_ptr(), K, dW.data_ptr(), Nn.ptr(db), Nn.ptr(dr), ldn, Cc.data_ptr(), ldn, 0,
                               T, N, K, epi, BF16, 0, _cfg(cfg), 0, 0), "gemm_wt")
     torch.cuda.synchronize()
