@@ -19,7 +19,7 @@
 //            HEAD   final RMSNorm + tied-embedding GEMV + logsumexp partials
 //   * k_attn1: single-CTA GQA attention per (kv head, q-head group), lane-per-key
 //     scores (no shuffles), for contexts up to ATT1_MAX_CAP keys; k_attn (cluster
-//     of CTAs, DSMEM push) beyond that.
+//     of CTAs, DSMEM push) beyond that, and at every context over an 8-bit pool.
 //   * k_sample: logprobs (bf16), greedy argmax (lowest index on ties), token log,
 //     state advance, next-token embedding.
 // Rounding points follow oracle/qwen2vl.py::lm_layers_forward.
@@ -515,20 +515,33 @@ __global__ void __launch_bounds__(256) k_attn1(const DecodeDims d, const bf16* _
 }
 
 // ---------------------------------------------------------------------------
-// k_attn: long contexts — a cluster of CL CTAs per (kv head, q-head group); rank r
-// owns keys [r*chunk, (r+1)*chunk).  Softmax statistics and partial outputs are
-// PUSHED to the peers' shared memory (st.shared::cluster): two cluster barriers.
+// k_attn: a cluster of CL CTAs per (kv head, q-head group); rank r owns keys
+// [r*chunk, (r+1)*chunk).  Softmax statistics and partial outputs are PUSHED to
+// the peers' shared memory (st.shared::cluster): two cluster barriers.
+//   Q8 = false: kc / vc are the layer's bf16 K / V planes (long contexts: k_attn1
+//               serves the short ones).
+//   Q8 = true:  k8 / v8 are the layer's 8-bit planes (format kvq.cuh), dequantized
+//               on load, and kc / vc the bf16 staging planes where the QKV kernel
+//               left the new row.  That row is quantized first, one CTA stores it,
+//               and the current token attends to its own key and value in their
+//               quantized form (QuantizedKVCache.update_and_fetch quantizes before
+//               it returns).
 // ---------------------------------------------------------------------------
+// The dynamic shared memory of every kernel in this file is one symbol, `sm`, and nvcc gives it the alignment of its
+// last declaration outside a template.  This one keeps it at 16 bytes, the layout the file's kernels are built with;
+// without it k_stream's __align__(128) would take over and move the shared memory of k_sample and k_stream<SM_HEAD>.
+extern __shared__ __align__(16) uint8_t sm[];
+
+template <bool Q8>
 __global__ void __launch_bounds__(256) k_attn(const DecodeDims d, const bf16* __restrict__ qbuf,
                                               const bf16* __restrict__ kc,
                                               const bf16* __restrict__ vc, bf16* __restrict__ out,
                                               const DecState* __restrict__ st, int chunk_cap,
-                                              int hsplit) {
+                                              int hsplit, const KvqPlanes k8, const KvqPlanes v8) {
   pdl_launch_dependents();
   cg::cluster_group cluster = cg::this_cluster();
   const int CL = (int)cluster.num_blocks();
   const int rank = (int)cluster.block_rank();
-  extern __shared__ __align__(16) uint8_t sm[];
   const int Gall = d.n_heads / d.n_kv;
   const int G = Gall / hsplit;  // q heads of this CTA
   const int hd = d.hd;
@@ -537,13 +550,66 @@ __global__ void __launch_bounds__(256) k_attn(const DecodeDims d, const bf16* __
   float* stats = sc + (long)ATT_MAXG * chunk_cap;      // [CL][G][2]   (filled by the peers)
   float* part = stats + ATT_MAXCL * ATT_MAXG * 2;      // [CL][G*hd]   (rank 0 only is read)
   float* red = part + (long)ATT_MAXCL * ATT_MAXG * hd; // [8][G*hd]
+  float* newrow = red + (long)8 * ATT_MAXG * hd;       // Q8: [2][hd], the new K and V row, dequantized
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kvh = blockIdx.y / hsplit;
   const int h0 = kvh * Gall + (blockIdx.y % hsplit) * G;  // first q head of this CTA
-  const bf16* kb = kc + (long)kvh * d.cap * hd;
-  const bf16* vb = vc + (long)kvh * d.cap * hd;
+  const long row0 = (long)kvh * d.cap;                    // position 0 of this kv head
+  const bf16* kb = kc + row0 * hd;
+  const bf16* vb = vc + row0 * hd;
+  const int ng = Q8 ? hd / k8.gs : 0;  // groups per row
   pdl_wait();
-  const int nkeys = st->ctx + 1;
+  const int ctx = st->ctx;
+  const int nkeys = ctx + 1;
+  if constexpr (Q8) {
+    // the new row: warp w < 2 * ng quantizes group w % ng of K (w < ng) or V; one CTA stores it
+    if (warp < 2 * ng) {
+      const int side = warp / ng, g = warp % ng, E = k8.gs >> 5;
+      const bf16* s = (side ? vb : kb) + (long)ctx * hd + g * k8.gs + lane * E;
+      float w[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) if (e < E) w[e] = bf2f(s[e]);
+      uint32_t code[4];
+      float scale, bias;
+      kvq_quantize_group(w, E, code, &scale, &bias);
+      const float sb = rbf(scale), bb = rbf(bias);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) if (e < E)
+          newrow[side * hd + g * k8.gs + lane * E + e] = kvq_dequant(code[e], sb, bb);
+      if (rank == 0 && (blockIdx.y % hsplit) == 0) {
+        const KvqPlanes P = side ? v8 : k8;
+        uint8_t* c = P.codes + (row0 + ctx) * hd + g * k8.gs + lane * E;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) if (e < E) c[e] = (uint8_t)code[e];
+        if (lane == 0) {
+          P.scales[(row0 + ctx) * ng + g] = f2bf(scale);
+          P.biases[(row0 + ctx) * ng + g] = f2bf(bias);
+        }
+      }
+    }
+    __syncthreads();
+  }
+  // the lane's EPL elements of K (side 0) or V (side 1) at position pos
+  auto load_row = [&](int side, int pos, float* f) {
+    if constexpr (Q8) {
+      if (pos == ctx) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) f[e] = (e < EPL) ? newrow[side * hd + lane * EPL + e] : 0.f;
+      } else {
+        kvq_load_row(side ? v8 : k8, row0 + pos, ng, lane, EPL, f);
+      }
+    } else {
+      const bf16* r = (side ? vb : kb) + (long)pos * hd + lane * EPL;
+      f[0] = f[1] = f[2] = f[3] = 0.f;
+      if (EPL == 4) {
+        unpack4(*reinterpret_cast<const uint2*>(r), f);
+      } else {
+        const uint32_t w = *reinterpret_cast<const uint32_t*>(r);
+        f[0] = __uint_as_float(w << 16);
+        f[1] = __uint_as_float(w & 0xffff0000u);
+      }
+    }
+  };
   const int chunk = (nkeys + CL - 1) / CL;
   const int k0 = min(nkeys, rank * chunk), k1 = min(nkeys, k0 + chunk);
   const int nloc = k1 - k0;
@@ -560,15 +626,8 @@ __global__ void __launch_bounds__(256) k_attn(const DecodeDims d, const bf16* __
   }
   // ---- scores (rounded to bf16) ----
   for (int j = warp; j < nloc; j += 8) {
-    const bf16* kr = kb + (long)(k0 + j) * hd + lane * EPL;
-    float kf[4] = {0.f, 0.f, 0.f, 0.f};
-    if (EPL == 4) {
-      unpack4(*reinterpret_cast<const uint2*>(kr), kf);
-    } else {
-      const uint32_t w = *reinterpret_cast<const uint32_t*>(kr);
-      kf[0] = __uint_as_float(w << 16);
-      kf[1] = __uint_as_float(w & 0xffff0000u);
-    }
+    float kf[4];
+    load_row(0, k0 + j, kf);
     float s[ATT_MAXG];
 #pragma unroll
     for (int g = 0; g < ATT_MAXG; ++g)
@@ -624,15 +683,8 @@ __global__ void __launch_bounds__(256) k_attn(const DecodeDims d, const bf16* __
 #pragma unroll
     for (int e = 0; e < 4; ++e) acc[g][e] = 0.f;
   for (int j = warp; j < nloc; j += 8) {
-    const bf16* vr = vb + (long)(k0 + j) * hd + lane * EPL;
-    float vf[4] = {0.f, 0.f, 0.f, 0.f};
-    if (EPL == 4) {
-      unpack4(*reinterpret_cast<const uint2*>(vr), vf);
-    } else {
-      const uint32_t w = *reinterpret_cast<const uint32_t*>(vr);
-      vf[0] = __uint_as_float(w << 16);
-      vf[1] = __uint_as_float(w & 0xffff0000u);
-    }
+    float vf[4];
+    load_row(1, k0 + j, vf);
 #pragma unroll
     for (int g = 0; g < ATT_MAXG; ++g) {
       if (g < G) {
@@ -840,9 +892,10 @@ constexpr int ATT1_MAX_CAP = 4096;
 static size_t attn1_smem(const DecodeDims& d) {
   return ((size_t)ATT1_G * d.hd + (size_t)ATT1_G * d.cap + (size_t)8 * ATT1_G * d.hd) * 4;
 }
-size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap) {
+// k_attn: scores, statistics, partial outputs, the warps' sums and, 8-bit only, the new row
+static size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap, bool q8) {
   return ((size_t)ATT_MAXG * chunk_cap + (size_t)ATT_MAXCL * ATT_MAXG * 2 +
-          (size_t)ATT_MAXCL * ATT_MAXG * d.hd + (size_t)8 * ATT_MAXG * d.hd) * 4;
+          (size_t)ATT_MAXCL * ATT_MAXG * d.hd + (size_t)8 * ATT_MAXG * d.hd + (q8 ? 2 * (size_t)d.hd : 0)) * 4;
 }
 
 int decode_prepare() {
@@ -856,20 +909,19 @@ int decode_prepare() {
   return B200_OK;
 }
 
-int attn_prepare(const DecodeDims& d, int cluster) {
-  int rc;
-  if (d.cap <= ATT1_MAX_CAP) {
+int attn_prepare(const DecodeDims& d, int cluster, bool q8) {
+  if (!q8 && d.cap <= ATT1_MAX_CAP) {
     const size_t smem = attn1_smem(d);
     B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
+    int rc;
     if ((rc = kernel_opt_in((const void*)k_attn1<128>, (int)smem, true)) ||
         (rc = kernel_opt_in((const void*)k_attn1<64>, (int)smem, true)))
       return rc;
-  } else {
-    const size_t smem = attn_smem_bytes(d, cdiv(d.cap, cluster));
-    B200_REQUIRE(smem <= 220 * 1024, "decode attention: cache capacity %d too large", d.cap);
-    if ((rc = kernel_opt_in((const void*)k_attn, (int)smem, true))) return rc;
+    return B200_OK;
   }
-  return B200_OK;
+  const size_t smem = attn_smem_bytes(d, cdiv(d.cap, cluster), q8);
+  B200_REQUIRE(smem <= 220 * 1024, "%sdecode attention: cache capacity %d too large", q8 ? "8-bit " : "", d.cap);
+  return kernel_opt_in(q8 ? (const void*)k_attn<true> : (const void*)k_attn<false>, (int)smem, true);
 }
 
 int launch_qkv(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* qbuf, bf16* kc,
@@ -893,20 +945,27 @@ int launch_qkv(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* qbuf,
   return B200_OK;
 }
 
-int launch_attn(const DecodeDims& d, const bf16* qbuf, const bf16* kc, const bf16* vc, bf16* out,
-                const DecState* st, int cluster, cudaStream_t s) {
+int launch_attn(const DecodeDims& d, const bf16* qbuf, const AttnKv& kv, bf16* out, const DecState* st, int cluster,
+                cudaStream_t s) {
   B200_REQUIRE(d.hd == 64 || d.hd == 128, "decode attention: head_dim=%d (64|128)", d.hd);
-  if (d.cap <= ATT1_MAX_CAP) {
+  const bool q8 = kv.k8.codes != nullptr;
+  if (!q8 && d.cap <= ATT1_MAX_CAP) {
     const int hs = attn_hsplit(d, ATT1_G);
     B200_CUDA(launch(d.hd == 128 ? k_attn1<128> : k_attn1<64>, dim3(d.n_kv * hs), dim3(256), attn1_smem(d), s,
-                     step_opts(), d, qbuf, kc, vc, out, st, hs));
+                     step_opts(), d, qbuf, kv.k, kv.v, out, st, hs));
     return B200_OK;
   }
+  B200_REQUIRE(cluster >= 1 && cluster <= ATT_MAXCL, "decode attention: cluster %d (1..%d)", cluster, ATT_MAXCL);
   const int hs = attn_hsplit(d, ATT_MAXG);
-  B200_REQUIRE(cluster <= ATT_MAXCL, "decode attention: cluster %d > %d", cluster, ATT_MAXCL);
   const int chunk_cap = cdiv(d.cap, cluster);
-  B200_CUDA(launch(k_attn, dim3(cluster, d.n_kv * hs, 1), dim3(256), attn_smem_bytes(d, chunk_cap), s,
-                   step_opts(cluster), d, qbuf, kc, vc, out, st, chunk_cap, hs));
+  if (q8) {
+    const int gs = kv.k8.gs;
+    B200_REQUIRE(gs == 32 || gs == 64 || gs == 128, "8-bit decode attention: group size %d", gs);
+    B200_REQUIRE(d.hd % gs == 0, "8-bit decode attention: group size %d does not divide head_dim %d", gs, d.hd);
+  }
+  B200_CUDA(launch(q8 ? k_attn<true> : k_attn<false>, dim3(cluster, d.n_kv * hs, 1), dim3(256),
+                   attn_smem_bytes(d, chunk_cap, q8), s, step_opts(cluster), d, qbuf, kv.k, kv.v, out, st, chunk_cap,
+                   hs, kv.k8, kv.v8));
   return B200_OK;
 }
 

@@ -1,6 +1,7 @@
 // Shared declarations of the decode-step kernels (decode.cu) and the engine.
 #pragma once
 #include "common.cuh"
+#include "kvq.cuh"
 
 namespace b200 {
 
@@ -137,18 +138,26 @@ void decode_set_sm_count(int n);
 void decode_set_pdl(bool on);
 // kernel attributes of the decode step that do not depend on the cache (once per engine)
 int decode_prepare();
-// the per-phase bf16 attention (k_attn1 up to 4096 positions, else k_attn on clusters of `cluster` CTAs): refuses a
-// capacity its shared memory cannot hold; run before the steps it serves
-int attn_prepare(const DecodeDims& d, int cluster);
+// the per-phase attention: bf16 pool, k_attn1 up to 4096 positions, else k_attn on clusters of `cluster` CTAs; 8-bit
+// pool (q8), k_attn at every capacity.  Refuses a capacity its shared memory cannot hold; run before the steps it serves
+int attn_prepare(const DecodeDims& d, int cluster, bool q8);
 int head_grid();
-size_t attn_smem_bytes(const DecodeDims& d, int chunk_cap);
 // qn / kn (Qwen3-VL q_norm / k_norm weights, both or neither): the QKV kernel leaves q / k unrotated and a second
 // kernel (k_qk_norm_rope) normalises and rotates the q heads and the new K row
 int launch_qkv(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* qbuf, bf16* kc,
                bf16* vc, const DecState* st, const float* inv_freq, cudaStream_t s, const bf16* qn = nullptr,
                const bf16* kn = nullptr);
-int launch_attn(const DecodeDims& d, const bf16* qbuf, const bf16* kc, const bf16* vc, bf16* out,
-                const DecState* st, int cluster, cudaStream_t s);
+// The K / V rows of one layer (bound row, kv head stride cap positions) the per-phase attention reads.
+//   bf16 pool:  k / v are its planes and k8.codes is null.
+//   8-bit pool: k8 / v8 are its planes, and k / v the bf16 staging planes where the QKV kernel left the new row at
+//               position ctx.  The attention quantizes that row, appends it to k8 / v8 and attends over positions
+//               0..ctx, the new one in its quantized form.
+struct AttnKv {
+  const bf16 *k, *v;
+  KvqPlanes k8, v8;
+};
+int launch_attn(const DecodeDims& d, const bf16* qbuf, const AttnKv& kv, bf16* out, const DecState* st, int cluster,
+                cudaStream_t s);
 int launch_res(const bf16* W, const bf16* x, bf16* h, int N, int K, cudaStream_t s);
 int launch_gateup(const DecodeDims& d, const LayerW& lw, const bf16* h, bf16* act, cudaStream_t s);
 int launch_head(const DecodeDims& d, const bf16* norm_w, const bf16* E, const bf16* h,

@@ -342,36 +342,27 @@ static int enqueue_step(b200_engine* e, cudaStream_t s) {
   const auto& c = e->cfg;
   int rc;
   if (e->active_mega()) return mega_launch(e->mp, e->sm_count, s);
-  if (e->kvb.kind == KvKind::q8) {
-    const KvBinding& b = e->kvb;
-    bf16* sk = e->q8_stage;
-    bf16* sv = sk + (long)c.n_kv_heads * b.cap * c.head_dim;
-    for (int l = 0; l < c.n_layers; ++l) {
-      const LayerW& lw = e->layers[l];
-      if ((rc = launch_qkv(d, lw, e->h, e->qbuf, sk, sv, e->st, e->lm_inv_freq, s, e->qk_norm ? e->qn[l] : nullptr,
-                           e->qk_norm ? e->kn[l] : nullptr)))
-        return rc;
-      if ((rc = launch_attn_q8(d, e->qbuf, e->q8_plane(b.q8, l, 0, e->kv_row, b.rows, b.cap),
-                               e->q8_plane(b.q8, l, 1, e->kv_row, b.rows, b.cap), sk, sv, e->attn, e->st,
-                               e->attn_cluster, s)))
-        return rc;
-      if ((rc = launch_res(lw.wo, e->attn, e->h, c.hidden, c.n_heads * c.head_dim, s))) return rc;
-      if ((rc = launch_gateup(d, lw, e->h, e->act, s))) return rc;
-      if ((rc = launch_res(lw.wd, e->act, e->h, c.hidden, c.inter, s))) return rc;
-    }
-  } else {
+  // the 8-bit kind: the QKV kernel leaves the new K / V row in the staging planes, and the attention appends it to the
+  // 8-bit pool
+  const KvBinding& b = e->kvb;
+  const bool q8 = b.kind == KvKind::q8;
+  const long stage_v = (long)c.n_kv_heads * b.cap * c.head_dim;  // the V staging plane follows the K one
   for (int l = 0; l < c.n_layers; ++l) {
     const LayerW& lw = e->layers[l];
-    bf16* kc = e->kptr(l, e->kv_row);
-    bf16* vc = e->vptr(l, e->kv_row);
+    bf16* kc = q8 ? e->q8_stage : e->kptr(l, e->kv_row);
+    bf16* vc = q8 ? e->q8_stage + stage_v : e->vptr(l, e->kv_row);
     if ((rc = launch_qkv(d, lw, e->h, e->qbuf, kc, vc, e->st, e->lm_inv_freq, s, e->qk_norm ? e->qn[l] : nullptr,
                          e->qk_norm ? e->kn[l] : nullptr)))
       return rc;
-    if ((rc = launch_attn(d, e->qbuf, kc, vc, e->attn, e->st, e->attn_cluster, s))) return rc;
+    AttnKv kv{kc, vc};
+    if (q8) {
+      kv.k8 = e->q8_plane(b.q8, l, 0, e->kv_row, b.rows, b.cap);
+      kv.v8 = e->q8_plane(b.q8, l, 1, e->kv_row, b.rows, b.cap);
+    }
+    if ((rc = launch_attn(d, e->qbuf, kv, e->attn, e->st, e->attn_cluster, s))) return rc;
     if ((rc = launch_res(lw.wo, e->attn, e->h, c.hidden, c.n_heads * c.head_dim, s))) return rc;
     if ((rc = launch_gateup(d, lw, e->h, e->act, s))) return rc;
     if ((rc = launch_res(lw.wd, e->act, e->h, c.hidden, c.inter, s))) return rc;
-  }
   }
   if ((rc = launch_head(d, e->norm, e->head, e->h, e->logits, e->partials, s))) return rc;
   if ((rc = launch_sample(d, e->logits, e->partials, e->logprobs, e->embed, e->h, e->st,
@@ -1249,11 +1240,7 @@ int b200_engine_decode(b200_engine* e, int n_steps, const int* force_tokens_host
   if (!(e->use_graph && e->gexec)) {
     // the per-phase attention kernel: its capacity limit and shared memory apply to the steps it serves only, so a
     // cache that k_mega holds is not refused for being too long for k_attn
-    if (e->kvb.kind == KvKind::q8) {
-      if ((rc = kvq_decode_prepare(e->dims(), e->attn_cluster))) return rc;
-    } else if (!e->active_mega()) {
-      if ((rc = attn_prepare(e->dims(), e->attn_cluster))) return rc;
-    }
+    if (!e->active_mega() && (rc = attn_prepare(e->dims(), e->attn_cluster, e->kvb.kind == KvKind::q8))) return rc;
   }
   if (e->use_graph && !e->gexec) {
     // capture one step on the engine's own stream (capture does not execute)

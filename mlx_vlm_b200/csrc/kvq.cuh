@@ -1,4 +1,4 @@
-// The 8-bit KV cache format: the one place that knows how K/V rows are quantized and laid out.
+// The 8-bit KV cache format: the one place that knows how K/V rows are quantized, laid out and read back.
 //
 // Layout of an 8-bit pool of `planes` (layer, k/v, row, kv head) planes, `cap` positions each:
 //   codes   uint8 [planes][cap][hd]          one byte per element; read as uint32 words, element 4i+j
@@ -21,7 +21,6 @@
 // Divisions are IEEE (__fdiv_rn) and rint is round-half-even; the build uses no fast-math.
 #pragma once
 #include "common.cuh"
-#include "decode.cuh"
 
 namespace b200 {
 
@@ -68,17 +67,20 @@ __device__ __forceinline__ float kvq_dequant(uint32_t code, float scale, float b
   return rbf(fmaf(scale, (float)code, bias));
 }
 
-// decode attention over an 8-bit pool (kvq.cu).  kc8 / vc8: K / V planes of the bound row of this layer
-// (kv head stride cap * hd codes, cap * hd / gs scales); stage_k / stage_v: bf16 planes [n_kv][cap][hd] where
-// the QKV kernel left the new row at position ctx.  Quantizes the new row, appends it to the pool and attends
-// over positions 0..ctx, the new one in its quantized form.
-int kvq_decode_prepare(const DecodeDims& d, int cluster);
+// EPL (2 or 4) dequantized elements of position `pos` of one kv head plane, dims [lane*EPL, lane*EPL+EPL)
+__device__ __forceinline__ void kvq_load_row(const KvqPlanes& P, long row, int ng, int lane, int EPL, float* f) {
+  const uint8_t* c = P.codes + row * (long)(ng * P.gs) + lane * EPL;
+  const uint32_t code = (EPL == 4) ? *reinterpret_cast<const uint32_t*>(c)
+                                   : (uint32_t)*reinterpret_cast<const uint16_t*>(c);
+  const long si = row * ng + (lane * EPL) / P.gs;
+  const float sc = bf2f(P.scales[si]), bi = bf2f(P.biases[si]);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) f[e] = (e < EPL) ? kvq_dequant((code >> (8 * e)) & 0xffu, sc, bi) : 0.f;
+}
+
 // quantize positions [pos0, pos0 + n) of `planes` bf16 planes (capacity cap) into dst (capacity dst_cap); writeback:
 // replace those bf16 rows by their dequantized values
 int kvq_quantize_rows(bf16* src, int cap, const KvqPlanes& dst, int dst_cap, long planes, int pos0, int n, int hd,
                       bool writeback, cudaStream_t s);
-int launch_attn_q8(const DecodeDims& d, const bf16* qbuf, const KvqPlanes& kc8, const KvqPlanes& vc8,
-                   const bf16* stage_k, const bf16* stage_v, bf16* out, const DecState* st, int cluster,
-                   cudaStream_t s);
 
 }  // namespace b200

@@ -57,7 +57,7 @@ def attn1_smem(hd, cap):                      # decode.cu attn1_smem
     return (ATT1_G * hd + ATT1_G * cap + 8 * ATT1_G * hd) * 4
 
 
-def attn_smem(hd, cap, cl):                   # decode.cu attn_smem_bytes(d, cdiv(cap, cluster))
+def attn_smem(hd, cap, cl):                   # decode.cu attn_smem_bytes(d, cdiv(cap, cluster), false)
     return (ATT_MAXG * cdiv(cap, cl) + ATT_MAXCL * ATT_MAXG * 2 + ATT_MAXCL * ATT_MAXG * hd + 8 * ATT_MAXG * hd) * 4
 
 

@@ -117,20 +117,23 @@ def _check_pool(model, c, pool, ref, n):
 @pytest.mark.parametrize("hd,gs", [(64, 32), (64, 64), (128, 32), (128, 64), (128, 128)])
 # past 4096 positions: trailing ranks of 8 with few keys, one rank holding 4600, two ranks of 4500
 @pytest.mark.parametrize("ctx,cluster", [(5, 1), (300, 8), (1000, 4), (4500, 8), (4600, 1), (9000, 2)])
-def test_decode_attention_kernel(hd, gs, ctx, cluster):
-    """k_attn_q8 on its own: the new row (staging plane, position ctx) is appended bit-exact to what the reference
-    quantize gives, the rows before it are untouched, and the output is sdpa over the dequantized K/V (the new
-    row included) within relative L2 1e-3."""
+# q heads per kv head: 6 (two CTAs of 3), 7 (one CTA), 1, 8 (two CTAs of 4)
+@pytest.mark.parametrize("n_heads,n_kv", [(12, 2), (28, 4), (16, 16), (8, 1)])
+def test_decode_attention_kernel(hd, gs, ctx, cluster, n_heads, n_kv):
+    """The 8-bit k_attn on its own: the new row (staging plane, position ctx) is appended bit-exact to what the
+    reference quantize gives, the rows before it are untouched, and the output is sdpa over the dequantized K/V (the
+    new row included) within relative L2 1e-3.  The pool's scales and biases at ctx and past it hold NaN before the
+    call, so a read of the pool there poisons the output."""
     from mlx_vlm_b200 import _native as N
     from oracle import mlx_semantics as S
     from _util import cmp_bf16
-    n_heads, n_kv, cap = 12, 2, ((ctx + 256) // 256) * 256
+    cap = ((ctx + 256) // 256) * 256
     ng = hd // gs
     rng = np.random.default_rng(ctx + hd + gs)
     bf = lambda a: torch.from_numpy(np.asarray(a, dtype=np.float32)).to(torch.bfloat16)
     kv = bf(rng.standard_normal((2, n_kv, cap, hd)) * 0.8)
-    codes, scales, biases = (np.zeros((2, n_kv, cap, hd), np.uint8) + 7, np.zeros((2, n_kv, cap, ng), np.float32),
-                             np.zeros((2, n_kv, cap, ng), np.float32))
+    codes, scales, biases = (np.zeros((2, n_kv, cap, hd), np.uint8) + 7, np.full((2, n_kv, cap, ng), np.nan, np.float32),
+                             np.full((2, n_kv, cap, ng), np.nan, np.float32))
     c_, s_, b_ = K.quantize(kv.float().numpy()[:, :, :ctx], gs)
     codes[:, :, :ctx], scales[:, :, :ctx], biases[:, :, :ctx] = c_, s_, b_
     stage = torch.zeros(2, n_kv, cap, hd, dtype=torch.bfloat16)
@@ -150,10 +153,11 @@ def test_decode_attention_kernel(hd, gs, ctx, cluster):
     gc, gsc, gb = dc.cpu().numpy(), ds.float().cpu().numpy(), db.float().cpu().numpy()
     assert np.array_equal(gc[:, :, ctx], nc) and np.array_equal(gsc[:, :, ctx], ns) and np.array_equal(gb[:, :, ctx], nb)
     assert np.array_equal(gc[:, :, :ctx], codes[:, :, :ctx]) and np.array_equal(gc[:, :, ctx + 1:], codes[:, :, ctx + 1:])
+    assert np.isnan(gsc[:, :, ctx + 1:]).all() and np.isnan(gb[:, :, ctx + 1:]).all()
     deq = torch.from_numpy(K.dequantize(gc[:, :, :ctx + 1], gsc[:, :, :ctx + 1], gb[:, :, :ctx + 1], gs))
     R = S.Rounder("bf16")
     want = S.sdpa(R, q.float()[None, :, None, :], deq[0][None], deq[1][None], hd ** -0.5, causal=False)
-    cmp_bf16(out, want[0, :, 0], f"k_attn_q8 hd={hd} gs={gs} ctx={ctx} cluster={cluster}", rel_l2=1e-3)
+    cmp_bf16(out, want[0, :, 0], f"8-bit k_attn heads={n_heads}/{n_kv} hd={hd} gs={gs} ctx={ctx} cluster={cluster}", rel_l2=1e-3)
 
 
 @pytest.mark.parametrize("kind,gs,step,before", [("tiny", 64, 5, 7), ("wide2", 128, 16, 20)])

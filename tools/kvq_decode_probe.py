@@ -1,5 +1,5 @@
 """Decode step time of Qwen2-VL-2B (synthetic weights) with a bf16 KV cache (k_mega, and the per-phase kernels)
-and with the 8-bit cache (per-phase kernels + k_attn_q8), alternating the arms at the same context.  Prints one
+and with the 8-bit cache (per-phase kernels, the 8-bit k_attn), alternating the arms at the same context.  Prints one
 JSON line.
 
     python tools/kvq_decode_probe.py [ctx ...]
