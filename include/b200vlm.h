@@ -304,7 +304,8 @@ int b200_engine_set_graph(b200_engine* e, int enabled);
  * grid barrier); a geometry it cannot hold runs the per-phase kernels.  Any other value is
  * B200_ERR_INVALID and leaves the mode unchanged. */
 int b200_engine_set_mega(b200_engine* e, int enabled);
-/* debugging / test aid: device pointer and size of an internal buffer.  names: "h", "act". */
+/* debugging / test aid: device pointer and size of an internal buffer.  names: "h", "act", "q" (the last decode
+ * step's rotated q heads). */
 int b200_engine_debug_buffer(b200_engine* e, const char* name, void** ptr, long* bytes);
 /* synchronous: reads the device-side error flag (0 = none; a bounded wait gave up) */
 int b200_engine_device_error(b200_engine* e, int* out);

@@ -1298,6 +1298,7 @@ int b200_engine_debug_buffer(b200_engine* e, const char* name, void** ptr, long*
   const std::string n(name);
   if (n == "h") { *ptr = e->h; *bytes = (long)e->cfg.hidden * 2; }
   else if (n == "act") { *ptr = e->act; *bytes = (long)e->cfg.inter * 2; }
+  else if (n == "q") { *ptr = e->qbuf; *bytes = (long)e->cfg.n_heads * e->cfg.head_dim * 2; }
   else {
     set_error("debug_buffer: unknown or unallocated buffer '%s'", name);
     return B200_ERR_INVALID;
