@@ -75,6 +75,17 @@ int b200_gemm_wt(const void* X, long ldx, const void* W, const void* bias, const
                  long ldr, void* C, long ldc, float* partial, int T, int N, int K, int epilogue,
                  int mode, int inter, const int* cfg4, unsigned flags, void* stream);
 int b200_gemm_wt_auto_config(int T, int N, int K, int mode, int inter, int* cfg4_out);
+/* The configurations the measured choice times for this problem on sm_count SMs, the cost model's choice first:
+ * *n_out of them, the first max_n written to cfg_out as {TN, KS, stages, split} each.  Host code only: it makes no
+ * CUDA call and runs without a GPU. */
+int b200_gemm_wt_candidates(int T, int N, int K, int mode, int inter, int allow_split, int sm_count,
+                            long partial_bytes, int* cfg_out, int max_n, int* n_out);
+/* b200_gemm_wt with the measured choice the engine uses (timed once per 64-token bucket, N, K and mode, then cached)
+ * for sm_count SMs and a partial buffer of partial_bytes; cfg4_out (may be NULL) receives the configuration that
+ * ran, {TN, KS, stages, split}. */
+int b200_gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, const void* residual, long ldr,
+                       void* C, long ldc, float* partial, long partial_bytes, int T, int N, int K, int epilogue,
+                       int mode, int inter, int allow_split, int sm_count, int* cfg4_out, void* stream);
 /* h[t] = bf16(resid[t] + bf16(sum_s partial[s][t] + bias)), and xn[t] = the RMSNorm /
  * LayerNorm of h[t] that the next block applies (language.py:139-148, vision.py:177-194):
  * the split-K reduction, the residual add and the norm in ONE pass over the row. */
@@ -375,10 +386,11 @@ int b200_f32_vision_rope(float* qkv, long ld, const int* pos_hw, const float* in
 int b200_f32_gather_rows(const float* in, long ld_in, const int* idx, int n_idx, int unit, int n, float* out,
                          long ld_out, void* stream);
 /* nn.Linear on fp32 activations: X split operand [T, n_parts x Kp], W [N, K_w] bf16 (row pitch ldw);
- * mode B200_WT_F32: C32 = act(acc + bias) + res32; mode B200_WT_SPLIT: Csplit = [hi | lo] of act(acc + bias) */
+ * mode B200_WT_F32: C32 = act(acc + bias) + res32; mode B200_WT_SPLIT: Csplit = [hi | lo] of act(acc + bias).
+ * cfg4 = {TN, KS, stages, 1} runs that configuration; NULL (or cfg4[0] == 0) keeps the measured choice. */
 int b200_gemm_wt_f32(const void* X, long ldx, const void* W, long ldw, const void* bias, const float* res32,
                      long ldr32, float* C32, long ldc32, void* Csplit, long ld_split, int n_pad, int T, int N,
-                     int K_w, int n_parts, int epilogue, int mode, void* stream);
+                     int K_w, int n_parts, int epilogue, int mode, const int* cfg4, void* stream);
 
 /* ------------------------------------------------------------------------- */
 /* Lock-step batched decode (continuous batching; generate/ar.py:929-1390        */

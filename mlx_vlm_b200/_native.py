@@ -41,6 +41,8 @@ SIGNATURES = {
     "b200_cast_f32_bf16": (_I, [_P, _P, _L, _P]),
     "b200_gemm_wt": (_I, [_P, _L, _P, _P, _P, _L, _P, _L, _P, _I, _I, _I, _I, _I, _I, _P, C.c_uint, _P]),
     "b200_gemm_wt_auto_config": (_I, [_I, _I, _I, _I, _I, _P]),
+    "b200_gemm_wt_candidates": (_I, [_I, _I, _I, _I, _I, _I, _I, _L, _P, _I, _P]),
+    "b200_gemm_wt_tuned": (_I, [_P, _L, _P, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "b200_finish_rows": (_I, [_P, _I, _P, _P, _L, _P, _L, _I, _P, _P, _F, _P, _L, _I, _I, _P]),
     "b200_layer_norm": (_I, [_P, _P, _P, _P, _I, _I, _F, _P]),
     "b200_rms_norm": (_I, [_P, _P, _P, _I, _I, _F, _P]),
@@ -93,7 +95,7 @@ SIGNATURES = {
     "b200_attention_f32_varlen": (_I, [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _I, _I, _F, _P]),
     "b200_f32_vision_rope": (_I, [_P, _L, _P, _P, _I, _I, _I, _P]),
     "b200_f32_gather_rows": (_I, [_P, _L, _P, _I, _I, _I, _P, _L, _P]),
-    "b200_gemm_wt_f32": (_I, [_P, _L, _P, _L, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_gemm_wt_f32": (_I, [_P, _L, _P, _L, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "b200_engine_set_kv_row": (_I, [_P, _I]),
     "b200_batch_begin": (_I, [_P, _I, _P, _P, _P, _P, _P]),
     "b200_batch_decode": (_I, [_P, _I, _I, _P]),

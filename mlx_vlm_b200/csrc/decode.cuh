@@ -228,7 +228,7 @@ int gemm_wt(const void* X, long ldx, const void* W, const void* bias, const void
 int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, const void* residual, long ldr,
                   void* C, long ldc, float* partial, long partial_bytes, int T, int N, int K, int epilogue,
                   int mode, int inter, bool allow_split, int sm_count, int* split_out, cudaStream_t st,
-                  const WtExt* ext = nullptr);
+                  const WtExt* ext = nullptr, WtConfig* cfg_out = nullptr);
 int finish_rows(const float* P, int S, const void* bias, const void* resid, long ldr, void* h_out,
                 long ldh, int norm_kind, const void* nw, const void* nb, float eps, void* xn, long ldx,
                 int T, int N, cudaStream_t st);

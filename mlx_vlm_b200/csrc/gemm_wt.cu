@@ -745,10 +745,71 @@ static int tune_enabled() {
   return v;
 }
 
+// whether a configuration's fp32 partial tiles fit the caller's partial buffer
+static bool wt_fits(const WtConfig& c, int mode, int T, int N, long partial_bytes) {
+  return !(mode == B200_WT_PARTIAL && (long)c.split * T * N * 4 > partial_bytes);
+}
+
+// The ordered list of configurations gemm_wt_tuned times for a problem class, the cost model's choice first; empty
+// when not even one unsplit set of partial tiles fits `partial_bytes`.  Pure host code (no CUDA call).
+static std::vector<WtConfig> gemm_wt_candidates(int T, int N, int K, int mode, int inter, bool allow_split,
+                                                int sm_count, long partial_bytes) {
+  const int row_blocks = mode == B200_WT_SWIGLU ? cdiv(inter, 64) : cdiv(N, WT_ROWS);
+  const int kb_total = cdiv(K, WT_BK);
+  auto fits = [&](const WtConfig& c) { return wt_fits(c, mode, T, N, partial_bytes); };
+  std::vector<WtConfig> cand;
+  auto add = [&](int tn, int ks, int budget, int split) {
+    if (tn > round16(T)) tn = round16(T);
+    if (tn > WT_TN_AUTO) tn = WT_TN_AUTO;
+    const int stage = ks * (WT_WBLK + tn * 128);
+    int stg = budget / stage;
+    if (stg > 6) stg = 6;
+    if (stg < 2 || (long)stg * stage < (long)WT_EPI_TOK * WT_ROWS * 4) return;
+    split = cdiv(kb_total, cdiv(kb_total, split < 1 ? 1 : split));
+    WtConfig c{tn, ks, stg, split};
+    if (!fits(c)) return;
+    for (const auto& o : cand)
+      if (o.TN == c.TN && o.KS == c.KS && o.stages == c.stages && o.split == c.split) return;
+    cand.push_back(c);
+  };
+  WtConfig model;
+  gemm_wt_auto(T, row_blocks, K, allow_split, &model, sm_count);
+  if (fits(model)) cand.push_back(model);
+  int tns[8], n_tn = 0;
+  if (T <= 96) {
+    tns[n_tn++] = round16(T);
+    if (T > 48) tns[n_tn++] = round16(cdiv(T, 2));
+  } else {
+    for (int tn : {128, 96, 112, 64}) tns[n_tn++] = tn;
+  }
+  for (int i = 0; i < n_tn; ++i) {
+    const int tn = tns[i];
+    const long base = (long)row_blocks * cdiv(T, tn);
+    int sps[3] = {1, 1, 1};
+    if (allow_split) {
+      int a = (int)(sm_count / base), b = (int)(2L * sm_count / base);
+      const int cap_k = kb_total / 4 > 0 ? kb_total / 4 : 1;
+      sps[1] = a < 1 ? 1 : (a > cap_k ? cap_k : a);
+      sps[2] = b < 1 ? 1 : (b > cap_k ? cap_k : b);
+    }
+    // (measured and discarded: restricting the list to <= 110 KB configurations so that the NEXT kernel's prologue
+    // can always co-reside under PDL made the C2 prefill 2-5 % slower)
+    for (int sp : sps) {
+      add(tn, 2, 208 * 1024, sp);  // 256-byte weight-row bursts
+      add(tn, 1, 110 * 1024, sp);  // one k-block per stage, shorter ring
+    }
+  }
+  if (cand.empty()) {
+    gemm_wt_auto(T, row_blocks, K, false, &model, sm_count);
+    if (fits(model)) cand.push_back(model);
+  }
+  return cand;
+}
+
 int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, const void* residual, long ldr,
                   void* C, long ldc, float* partial, long partial_bytes, int T, int N, int K, int epilogue,
                   int mode, int inter, bool allow_split, int sm_count, int* split_out, cudaStream_t st,
-                  const WtExt* ext) {
+                  const WtExt* ext, WtConfig* cfg_out) {
   static std::unordered_map<TuneKey, WtConfig, TuneHash> cache;
   static std::mutex mu;
   const int row_blocks = mode == B200_WT_SWIGLU ? cdiv(inter, 64) : cdiv(N, WT_ROWS);
@@ -779,9 +840,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
       have = true;
     }
   }
-  auto fits = [&](const WtConfig& c) {
-    return !(mode == B200_WT_PARTIAL && (long)c.split * T * N * 4 > partial_bytes);
-  };
+  auto fits = [&](const WtConfig& c) { return wt_fits(c, mode, T, N, partial_bytes); };
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cap);
   if (!have && (!tune_enabled() || cap != cudaStreamCaptureStatusNone)) {
@@ -789,54 +848,10 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
     while (cfg.split > 1 && !fits(cfg)) cfg.split = cdiv(kb_total, cdiv(kb_total, cfg.split - 1));
     have = true;  // not cached: a later un-captured call may still tune
   } else if (!have) {
-    // ---- candidate list ----
-    std::vector<WtConfig> cand;
-    auto add = [&](int tn, int ks, int budget, int split) {
-      if (tn > round16(T)) tn = round16(T);
-      if (tn > WT_TN_AUTO) tn = WT_TN_AUTO;
-      const int stage = ks * (WT_WBLK + tn * 128);
-      int stg = budget / stage;
-      if (stg > 6) stg = 6;
-      if (stg < 2 || (long)stg * stage < (long)WT_EPI_TOK * WT_ROWS * 4) return;
-      split = cdiv(kb_total, cdiv(kb_total, split < 1 ? 1 : split));
-      WtConfig c{tn, ks, stg, split};
-      if (!fits(c)) return;
-      for (const auto& o : cand)
-        if (o.TN == c.TN && o.KS == c.KS && o.stages == c.stages && o.split == c.split) return;
-      cand.push_back(c);
-    };
-    WtConfig model;
-    gemm_wt_auto(T, row_blocks, K, allow_split, &model, sm_count);
-    if (fits(model)) cand.push_back(model);
-    int tns[8], n_tn = 0;
-    if (T <= 96) {
-      tns[n_tn++] = round16(T);
-      if (T > 48) tns[n_tn++] = round16(cdiv(T, 2));
-    } else {
-      for (int tn : {128, 96, 112, 64}) tns[n_tn++] = tn;
-    }
-    for (int i = 0; i < n_tn; ++i) {
-      const int tn = tns[i];
-      const long base = (long)row_blocks * cdiv(T, tn);
-      int sps[3] = {1, 1, 1};
-      if (allow_split) {
-        int a = (int)(sm_count / base), b = (int)(2L * sm_count / base);
-        const int cap_k = kb_total / 4 > 0 ? kb_total / 4 : 1;
-        sps[1] = a < 1 ? 1 : (a > cap_k ? cap_k : a);
-        sps[2] = b < 1 ? 1 : (b > cap_k ? cap_k : b);
-      }
-      // (measured and discarded: restricting the list to <= 110 KB configurations so that the NEXT kernel's prologue
-      // can always co-reside under PDL made the C2 prefill 2-5 % slower)
-      for (int sp : sps) {
-        add(tn, 2, 208 * 1024, sp);  // 256-byte weight-row bursts
-        add(tn, 1, 110 * 1024, sp);  // one k-block per stage, shorter ring
-      }
-    }
-    if (cand.empty()) {
-      gemm_wt_auto(T, row_blocks, K, false, &model, sm_count);
-      B200_REQUIRE(fits(model), "gemm_wt: the partial-tile buffer (%ld B) is too small for T=%d N=%d", partial_bytes, T, N);
-      cand.push_back(model);
-    }
+    const std::vector<WtConfig> cand =
+        gemm_wt_candidates(T, N, K, mode, inter, allow_split, sm_count, partial_bytes);
+    B200_REQUIRE(!cand.empty(), "gemm_wt: the partial-tile buffer (%ld B) is too small for T=%d N=%d", partial_bytes,
+                 T, N);
     // ---- time them (the tuning launches never add a residual: the output stays idempotent) ----
     // An output that is also its own residual (h += W.x in place, bf16 or fp32) must not be overwritten by the
     // measurement: whenever a residual is given, those launches write a scratch buffer from the stream-ordered
@@ -932,6 +947,7 @@ int gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, cons
   while (cfg.split > 1 && !fits(cfg)) cfg.split = cdiv(kb_total, cdiv(kb_total, cfg.split - 1));
   B200_REQUIRE(fits(cfg), "gemm_wt: the partial-tile buffer (%ld B) is too small for T=%d N=%d", partial_bytes, T, N);
   if (split_out) *split_out = cfg.split;
+  if (cfg_out) *cfg_out = cfg;
   return gemm_wt(X, ldx, W, bias, residual, ldr, C, ldc, partial, T, N, K, epilogue, mode, inter, cfg, 0, st, ext);
 }
 
@@ -985,5 +1001,31 @@ int b200_gemm_wt_auto_config(int T, int N, int K, int mode, int inter, int* cfg4
   gemm_wt_auto(T, rbs, K, mode == B200_WT_PARTIAL, &c, 132);
   cfg4_out[0] = c.TN; cfg4_out[1] = c.KS; cfg4_out[2] = c.stages; cfg4_out[3] = c.split;
   return B200_OK;
+}
+
+int b200_gemm_wt_candidates(int T, int N, int K, int mode, int inter, int allow_split, int sm_count,
+                            long partial_bytes, int* cfg_out, int max_n, int* n_out) {
+  B200_REQUIRE(T > 0 && N > 0 && K > 0 && sm_count > 0 && n_out && (max_n <= 0 || cfg_out),
+               "gemm_wt_candidates: T=%d N=%d K=%d sm_count=%d", T, N, K, sm_count);
+  const std::vector<WtConfig> cand =
+      gemm_wt_candidates(T, N, K, mode, inter, allow_split != 0, sm_count, partial_bytes);
+  *n_out = (int)cand.size();
+  for (int i = 0; i < (int)cand.size() && i < max_n; ++i) {
+    cfg_out[4 * i] = cand[i].TN; cfg_out[4 * i + 1] = cand[i].KS;
+    cfg_out[4 * i + 2] = cand[i].stages; cfg_out[4 * i + 3] = cand[i].split;
+  }
+  return B200_OK;
+}
+
+int b200_gemm_wt_tuned(const void* X, long ldx, const void* W, const void* bias, const void* residual, long ldr,
+                       void* C, long ldc, float* partial, long partial_bytes, int T, int N, int K, int epilogue,
+                       int mode, int inter, int allow_split, int sm_count, int* cfg4_out, void* stream) {
+  WtConfig c{0, 0, 0, 0};
+  const int rc = gemm_wt_tuned(X, ldx, W, bias, residual, ldr, C, ldc, partial, partial_bytes, T, N, K, epilogue,
+                               mode, inter, allow_split != 0, sm_count, nullptr, (cudaStream_t)stream, nullptr, &c);
+  if (cfg4_out) {
+    cfg4_out[0] = c.TN; cfg4_out[1] = c.KS; cfg4_out[2] = c.stages; cfg4_out[3] = c.split;
+  }
+  return rc;
 }
 }

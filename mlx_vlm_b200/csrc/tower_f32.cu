@@ -616,14 +616,18 @@ int b200_f32_gather_rows(const float* in, long ld_in, const int* idx, int n_idx,
   return f32_gather_rows(in, ld_in, idx, n_idx, unit, n, out, ld_out, (cudaStream_t)st);
 }
 /* fp32-accurate Linear on the tensor cores: X = split operand [T, n_parts x Kp] (Kp = K_w rounded up to 64),
- * W [N, K_w] bf16; mode B200_WT_F32 (C32 = act(acc + bias) + res32) or B200_WT_SPLIT (Csplit = [hi | lo]). */
+ * W [N, K_w] bf16; mode B200_WT_F32 (C32 = act(acc + bias) + res32) or B200_WT_SPLIT (Csplit = [hi | lo]).
+ * cfg4 = {TN, KS, stages, 1} runs that configuration; NULL keeps the measured choice. */
 int b200_gemm_wt_f32(const void* X, long ldx, const void* W, long ldw, const void* bias, const float* res32,
                      long ldr32, float* C32, long ldc32, void* Csplit, long ld_split, int n_pad, int T, int N,
-                     int K_w, int n_parts, int epilogue, int mode, void* stream) {
+                     int K_w, int n_parts, int epilogue, int mode, const int* cfg4, void* stream) {
   const int kbw = cdiv(K_w, 64);
   WtExt ext;
   ext.kb_w = kbw; ext.k_w = K_w; ext.ldw = ldw; ext.C32 = C32; ext.res32 = res32; ext.ldc32 = ldc32;
   ext.ldr32 = ldr32; ext.Csplit = (bf16*)Csplit; ext.ld_split = ld_split; ext.n_pad = n_pad;
+  if (cfg4 && cfg4[0] > 0)
+    return gemm_wt(X, ldx, W, bias, nullptr, 0, nullptr, 0, nullptr, T, N, n_parts * kbw * 64, epilogue, mode, 0,
+                   WtConfig{cfg4[0], cfg4[1], cfg4[2], cfg4[3]}, 0, (cudaStream_t)stream, &ext);
   return gemm_wt_tuned(X, ldx, W, bias, nullptr, 0, nullptr, 0, nullptr, 0, T, N, n_parts * kbw * 64, epilogue, mode, 0,
                        false, 132, nullptr, (cudaStream_t)stream, &ext);
 }

@@ -83,7 +83,7 @@ class TowerOps:
             x.t.data_ptr(), x.ld, w.data_ptr(), w.stride(0), N.ptr(bias), N.ptr(res32),
             res32.stride(0) if res32 is not None else 0, N.ptr(out32), out32.stride(0) if out32 is not None else 0,
             N.ptr(out_split.t) if out_split else 0, out_split.ld if out_split else 0,
-            out_split.n_pad if out_split else 0, x.T, n_out, k_w, n_parts, epi, mode, self.eng.s), "gemm_wt_f32")
+            out_split.n_pad if out_split else 0, x.T, n_out, k_w, n_parts, epi, mode, None, self.eng.s), "gemm_wt_f32")
 
     def attention(self, q, k, v, *, n_heads: int, n_kv: int, hd: int, Lq: int, S: int, n_seg: int, q_seg: int,
                   k_seg: int, scale: float, out32: Optional[torch.Tensor] = None, out_split: Optional[SplitBuf] = None,
